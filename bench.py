@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — DDFA GGNN hot path: CFG graphs/sec of a full train step on B200.
+"""bench.py — DDFA GGNN hot path: CFG graphs/sec of a full train step on H100.
 
 Workload (default, BASELINE.json configs[2] / SURVEY.md §8 "C1"): synthetic Big-Vul-shaped batches of 1024 CFGs
 per GPU x 150 nodes / 300 edges (incl. self loops), 4 x Embedding(1002,32) -> 128-d, T=8 propagation steps,
@@ -11,6 +11,7 @@ data-path collective).
   python bench.py --gpus 1 --steps K --warmup W            # our arm (CUDA, libddfa_b200.so)
   python bench.py --impl reference --steps K --warmup W    # reference arm: the reference path's CPU
                                                            # restatement (oracle/) on the host cores
+  python bench.py --steps K --dump-outputs DIR             # also write what the last timed step computed, DIR/<name>.npy
 One JSON line on stdout (rank 0).  See DESIGN.md §6 for every field.
 """
 from __future__ import annotations
@@ -35,7 +36,6 @@ CFG = dict(graphs=1024, nodes=150, edges_per_node=2.0, input_dim=1002, hidden_di
 METRIC = "CFG graphs/sec (train step)"
 UNIT = "graphs/s"
 NUM_BATCHES = 8  # distinct resident batches rotated through the timed region
-MIN_TIMED_MS = float(os.environ.get("DDFA_BENCH_MIN_TIMED_MS", "300"))  # (0 for profiler runs) the K-step timed region is repeated until this much device time is covered; the median region is reported
 
 
 def workload_tag(graphs):
@@ -56,7 +56,7 @@ def workload_config(graphs, world):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler (nvidia-smi at 100 ms: SM clock, power, throttle reasons over the timed region)
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -158,13 +158,13 @@ def measured_peaks():
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "source": "measured"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet (700 W), not measured"}
 
 
 def ncu_traffic(kernel, n_nodes, mode):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the committed table of `ncu --set full`
-    captures (profiles/ncu_traffic.json, written by scripts/ncu_lines.py from the .ncu-rep of the named capture), keyed by kernel,
-    node count and mode.  None when no capture of that shape is committed — never a guess."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from a table of `ncu --set full` captures
+    (profiles/ncu_traffic.json, written by scripts/ncu_traffic.py from the .ncu-rep of the named capture), keyed by kernel,
+    node count and mode.  None when no capture of that shape is in the tree — never a guess."""
     try:
         with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
             table = json.load(f)
@@ -258,26 +258,21 @@ class Ctx:
     pass
 
 
-def timed_regions(ctx, fn_step, steps, min_ms=MIN_TIMED_MS, max_regions=25):
-    """Times regions of EXACTLY `steps` steps each (barrier + synchronize on both sides, CUDA events, max over ranks) until
-    `min_ms` of device time is covered; returns the per-region milliseconds."""
+def timed_regions(ctx, fn_step, steps):
+    """Times ONE region of exactly `steps` steps (barrier + synchronize on both sides, CUDA events, max over ranks); returns
+    [milliseconds] (a list, so the JSON fields keep their shape)."""
     import torch.distributed as dist
-    out = []
-    while True:
-        ctx.barrier()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for i in range(steps):
-            fn_step(i)
-        e1.record()
-        ctx.barrier()
-        t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=ctx.dev)
-        if ctx.world > 1:
-            dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        out.append(float(t.item()))
-        # every rank sees the same (max-reduced) numbers, so all ranks leave the loop together
-        if sum(out) >= min_ms or len(out) >= max_regions:
-            return out
+    ctx.barrier()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(steps):
+        fn_step(i)
+    e1.record()
+    ctx.barrier()
+    t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=ctx.dev)
+    if ctx.world > 1:
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    return [float(t.item())]
 
 
 def roofline_lines(prof, ms_region, N, Eg, engine, peaks, mode_tag):
@@ -317,7 +312,7 @@ def roofline_lines(prof, ms_region, N, Eg, engine, peaks, mode_tag):
     packed = tc and bool(_E.OPTIONS.get("packed_state"))
     fwd_P, bwd_P = (5, 16) if packed else (9, 18)
     tr = ncu_traffic("gru_fwd3_kernel", N, "train") if tc else None
-    fwd_line = hbm_line("gru_fwd3_kernel (GRU step forward, tcgen05: weights in TMEM, bf16x3)" if tc else "GRU step forward (simt engine)",
+    fwd_line = hbm_line("gru_fwd3_kernel (GRU step forward, wgmma: weights resident in shared memory, bf16x3)" if tc else "GRU step forward (simt engine)",
                         fwd_P * P, gru_f_ms, gru_f_n, share["ddfa_gru_step_fwd"], design_bytes=f"{fwd_P}P (P = N x 128 x 4 B)",
                         traffic=tr["bytes"] if tr else None, traffic_source=tr["source"] if tr else None,
                         algorithmic_bytes_8d=int(3 * P), frac_8d=3 * P / (gru_f_ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
@@ -342,9 +337,23 @@ def roofline_lines(prof, ms_region, N, Eg, engine, peaks, mode_tag):
         lines.insert(2, hbm_line(f"wgrad_kernel + wgrad_reduce_kernel (weight gradients of all {T} steps in one launch)",
                                  6 * P * T, wg_ms, wg_n, share["wgrad_batched"], traffic=None,
                                  tensor_tflops_issued=3 * flops_fold * T / (wg_ms * 1e-3) / 1e12))
-    roofline = dict(fwd_line, note="the forward GRU step kernel: ~24 % of the step and the hot kernel furthest below its roofline (the gate-backward + dgrad pair is the larger share, ~42 %, at ~0.95 of peak: roofline_kernels); frac = design bytes (bytes_per_launch; 5P with the packed saved state) "
-                                   "over the launch time vs the measured HBM peak, frac_8d / tensor_frac_8d = SURVEY.md §8(d)'s algorithmic bytes / FLOPs")
+    roofline = dict(fwd_line, note="the forward GRU step kernel; frac = design bytes (bytes_per_launch; 5P with the packed saved state) "
+                                   "over the launch time vs the HBM peak (peak_source), frac_8d / tensor_frac_8d = SURVEY.md §8(d)'s algorithmic bytes / FLOPs")
     return roofline, lines
+
+
+def dump_outputs(out_dir, trainer, batch_index):
+    """What the timed path hands its caller after its last step: the loss of that step's batch and the model's parameters after
+    the Adam update, as float32 / float64 .npy files (a few MB in all; every input is seeded, so two builds
+    run with the same arguments can be compared file by file)."""
+    import numpy as np
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": trainer.loss_slot.detach().double().reshape(-1), "batch_index": torch.tensor([float(batch_index)], dtype=torch.float64)}
+    for name, p in trainer.module.named_parameters():
+        arrays["param." + name] = p.detach().float()
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
 
 
 def measure_workload(ctx, args, graphs, full):
@@ -426,7 +435,9 @@ def measure_workload(ctx, args, graphs, full):
     res["final_loss"] = float(trainer.loss_slot.item())
     res["value"] = global_batch * steps / (ms_total * 1e-3)
     res["ms_per_step"] = ms_total / steps
-    res["timed_regions"] = {"count": len(regions), "steps_each": steps, "ms": [round(x, 3) for x in regions], "reported": "median"}
+    res["timed_regions"] = {"count": len(regions), "steps_each": steps, "ms": [round(x, 3) for x in regions], "reported": "single region"}
+    if full and args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, (steps - 1) % NUM_BATCHES)
     res["gpu_launches_per_step"] = int(launches_per_step)
     res["nodes"], res["edges"] = N, Eg
 
@@ -444,7 +455,7 @@ def measure_workload(ctx, args, graphs, full):
         state["nxt"] = fresh(host_batches[(i + 1) % NUM_BATCHES])
         trainer.prefetch(state["nxt"], global_batch)          # the next step's H2D copies run on a side stream during this step
         state["loss"] = float(loss_t.item())
-    e2e_regions = timed_regions(ctx, step_e2e, steps, min_ms=MIN_TIMED_MS / 2, max_regions=10)
+    e2e_regions = timed_regions(ctx, step_e2e, steps)
     ms_e2e = statistics.median(e2e_regions)
     res["e2e"] = {"value": global_batch * steps / (ms_e2e * 1e-3), "unit": UNIT, "h2d_bytes_per_step": batch_bytes(host_batches[0]),
                   "d2h_bytes_per_step": 4, "steps": steps, "regions": len(e2e_regions),
@@ -465,7 +476,7 @@ def measure_workload(ctx, args, graphs, full):
 
     def step_arena(i):
         state["loss"] = float(trainer.step_ids(arena, id_lists[i % NUM_BATCHES], global_batch).item())
-    ar_regions = timed_regions(ctx, step_arena, steps, min_ms=MIN_TIMED_MS / 2, max_regions=10)
+    ar_regions = timed_regions(ctx, step_arena, steps)
     res["e2e_arena"] = {"value": global_batch * steps / (statistics.median(ar_regions) * 1e-3), "unit": UNIT, "h2d_bytes_per_step": 4 * graphs,
                         "d2h_bytes_per_step": 4, "steps": steps,
                         "path": f"graph-id list (pinned) -> H2D -> ddfa_arena_batch over a resident arena of {arena.num_graphs} graphs -> "
@@ -488,7 +499,7 @@ def measure_workload(ctx, args, graphs, full):
             state["loss"] = float(loss.item())
         for i in range(3):
             step_api(i)
-        api_regions = timed_regions(ctx, step_api, steps, min_ms=MIN_TIMED_MS / 2, max_regions=10)
+        api_regions = timed_regions(ctx, step_api, steps)
         res["e2e_module_api"] = {"value": global_batch * steps / (statistics.median(api_regions) * 1e-3), "unit": UNIT,
                                  "h2d_bytes_per_step": batch_bytes(host_batches[0]), "d2h_bytes_per_step": 4, "steps": steps,
                                  "path": "FlowGNNGGNNModule.training_step((host batch, {})) -> loss.backward() -> torch.optim.Adam.step() -> "
@@ -528,7 +539,7 @@ def measure_variable_stream(ctx, args, graphs):
         state["nxt"] = fresh(host[(i + 1) % n_batches])
         trainer.prefetch(state["nxt"], global_batch)
         state["loss"] = float(loss_t.item())
-    regions = timed_regions(ctx, step_var, n_batches, min_ms=MIN_TIMED_MS / 2, max_regions=6)
+    regions = timed_regions(ctx, step_var, n_batches)
     ms = statistics.median(regions)
     shapes = sorted({(b.num_nodes(), b.num_edges()) for b in host})
     return {"value": global_batch * n_batches / (ms * 1e-3), "unit": UNIT, "ms_per_step": ms / n_batches, "steps": n_batches,
@@ -556,7 +567,7 @@ def run_ours(args):
         dist.init_process_group("nccl", device_id=dev)
     ctx.L = L = _lib.lib()
     if L.call("ddfa_device_supported") != 1:
-        raise SystemExit("bench.py: device is not compute capability 10.x")
+        raise SystemExit("bench.py: device is not an H100 (compute capability 9.0); the library is built for sm_90a only")
 
     def barrier():
         if world > 1:
@@ -616,7 +627,7 @@ def run_ours(args):
         "dtype": "f32" if args.engine == "simt" else "f32 (GRU GEMMs: bf16x3 split operands, f32 accumulate)",
         "data": "synthetic", "config": workload_config(args.graphs, world),
         "engine": args.engine,
-        "l2": f"per-step working set ~{N * 128 * 4 * 49 / 1e9:.2f} GB of saved activations > 126 MB L2; {NUM_BATCHES} distinct resident batches rotated",
+        "l2": f"per-step working set ~{N * 128 * 4 * 49 / 1e9:.2f} GB of saved activations > 50 MB L2; {NUM_BATCHES} distinct resident batches rotated",
         "timed_regions": primary["timed_regions"],
         "clocks": primary.get("clocks"),
         "e2e": primary["e2e"], "e2e_arena": primary.get("e2e_arena"), "e2e_module_api": primary.get("e2e_module_api"),
@@ -649,6 +660,8 @@ def main():
     ap.add_argument("--no-graphs", dest="cuda_graphs", action="store_false", help="launch every kernel eagerly in the timed region")
     ap.add_argument("--no-secondary", dest="secondary", action="store_false", help="skip the C0 second workload of the default run")
     ap.add_argument("--no-variable", dest="variable", action="store_false", help="skip the variable-shape stream line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (loss, updated parameters) as DIR/<name>.npy")
     ap.add_argument("--quick", action="store_true", help="headline value + e2e only (no per-kernel spans, arena / module-API lines, CPU baseline): scaling A/Bs")
     args = ap.parse_args()
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""deepdfa_b200 — B200-native (sm_100a) implementation of DeepDFA's DDFA ``code_gnn`` GGNN hot path.
+"""deepdfa_b200 — H100-native (sm_90a) implementation of DeepDFA's DDFA ``code_gnn`` GGNN hot path.
 
 Public surface (mirrors the reference for this path only):
   FlowGNNGGNNModule   — drop-in for code_gnn.models.flow_gnn.ggnn.FlowGNNGGNNModule

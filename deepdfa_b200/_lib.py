@@ -119,7 +119,7 @@ class _Lib:
             raise DdfaError(f"ABI version mismatch: library {abi}, binding 1")
         # A/B scripts select launch configurations through the environment of the PYTHON layer; the library itself reads none
         for env, key in (("DDFA_L2_HINTS", TUNE_L2_HINTS), ("DDFA_PDL", TUNE_PDL_MASK), ("DDFA_GATHER_VARIANT", TUNE_GATHER_VARIANT),
-                         ("DDFA_FWD_PAIR", TUNE_FWD_PAIR), ("DDFA_GATE_BWD_TMA", TUNE_GATE_BWD_TMA),
+                         ("DDFA_GATE_BWD_TMA", TUNE_GATE_BWD_TMA),
                          ("DDFA_GATHER_SRC_GROUPS", TUNE_GATHER_SRC_GROUPS)):
             if os.environ.get(env) is not None:
                 self._dll.ddfa_tuning_set(key, int(os.environ[env]))

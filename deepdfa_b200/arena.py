@@ -3,7 +3,7 @@
 The reference assembles every training batch on the host: ``dgl.batch([...])`` inside the ``GraphDataLoader`` collate
 (``DDFA/sastvd/linevd/datamodule.py:116-141``) or on the fly in ``BigVulDatasetLineVD.get_indices``
 (``DDFA/sastvd/linevd/dataset.py:63-76`` — ``dgl.batch([self[i] for i in ...]).to(device)``), after which DGL builds its
-CSR lazily on the device.  A 180 GB GPU holds the whole Big-Vul graph set (~10^7 nodes) many times over, so here the
+CSR lazily on the device.  An 80 GB H100 holds the whole Big-Vul graph set (~10^7 nodes) many times over, so here the
 dataset is uploaded ONCE — already in the layout the kernels read — and a batch is a list of graph ids:
 
     arena = GraphArena.from_graphs(list_of_single_graphs, device="cuda")     # one-time: H2D + one ddfa_build_csr

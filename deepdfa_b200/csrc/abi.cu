@@ -27,14 +27,13 @@ static std::atomic<int> g_tuning[DDFA_TUNE__COUNT] = {
     {23},   // DDFA_TUNE_L2_HINTS: measured best on whole-step A/Bs (profiles/r02l-m): 1 + 2 + 4 + 16
     {15},   // DDFA_TUNE_PDL_MASK: all four chain kernels
     {9},    // DDFA_TUNE_GATHER_VARIANT: r01b sweep — 2 rows/pass, 4 loads in flight, 128-thread CTAs
-    {0},    // DDFA_TUNE_FWD_PAIR: 1 = gru_fwd3_kernel launched as CTA pairs (tcgen05.mma.cta_group::2)
+    {0},    // DDFA_TUNE_FWD_PAIR: reserved, only 0 is accepted (no CTA-pair form of the forward kernel on sm_90a)
     {2},    // DDFA_TUNE_GATE_BWD_TMA: 0 register loads; 1 TMA-staged streaming operands (packed saved state); 2 = 1 + CSR scalars pipelined
     {0},    // DDFA_TUNE_GATHER_SRC_GROUPS: image->image gather, row groups per warp (0 = default = 1; 2 / 4 selectable)
 };
 int l2_hints() { return g_tuning[DDFA_TUNE_L2_HINTS].load(std::memory_order_relaxed); }
 int pdl_mask() { return g_tuning[DDFA_TUNE_PDL_MASK].load(std::memory_order_relaxed); }
 int gather_variant() { return g_tuning[DDFA_TUNE_GATHER_VARIANT].load(std::memory_order_relaxed); }
-int fwd_pair() { return g_tuning[DDFA_TUNE_FWD_PAIR].load(std::memory_order_relaxed); }
 int gate_bwd_tma() { return g_tuning[DDFA_TUNE_GATE_BWD_TMA].load(std::memory_order_relaxed); }
 int gather_src_groups() { return g_tuning[DDFA_TUNE_GATHER_SRC_GROUPS].load(std::memory_order_relaxed); }
 
@@ -60,6 +59,7 @@ int ddfa_engine_available(int engine) {
 
 int ddfa_tuning_set(int key, int value) {
   DDFA_REQUIRE(key >= 0 && key < DDFA_TUNE__COUNT, "ddfa_tuning_set: unknown key %d", key);
+  DDFA_REQUIRE(key != DDFA_TUNE_FWD_PAIR || value == 0, "ddfa_tuning_set: DDFA_TUNE_FWD_PAIR must be 0 (no CTA-pair forward kernel on sm_90a)");
   ddfa::g_tuning[key].store(value, std::memory_order_relaxed);
   return DDFA_OK;
 }
@@ -70,7 +70,7 @@ int ddfa_tuning_get(int key) {
 
 int ddfa_debug_set(int key, int value) {
   switch (key) {
-    case 2: {   // pipeline timeline stamps of the tcgen05 kernels: 0 off, 1 = gru_fwd3 + dgrad3, 2 = gru_fwd3 + wgrad
+    case 2: {   // pipeline timeline stamps of the tensor-core kernels: 0 off, 1 = gru_fwd3 + dgrad3, 2 = gru_fwd3 + wgrad
       int rc = ddfa::gru_tc3_trace_enable(value);
       return rc != DDFA_OK ? rc : ddfa::gru_tc2b_trace_enable(value);
     }
@@ -80,7 +80,7 @@ int ddfa_debug_set(int key, int value) {
 
 int ddfa_debug_read(int key, void *host_out, size_t bytes) {
   DDFA_REQUIRE(host_out != nullptr, "ddfa_debug_read: null output");
-  switch (key) {   // [148 CTAs][12 tiles][12 events] int64 SM-clock stamps
+  switch (key) {   // [132 CTAs][12 tiles][12 events] int64 SM-clock stamps
     case 2: return ddfa::gru_tc2b_trace_read(host_out, bytes);    // dgrad3_kernel / wgrad_kernel
     case 3: return ddfa::gru_tc3_trace_read(host_out, bytes);     // gru_fwd3_kernel
     case 4: {                                                     // int32: bounded-wait failures of the TMA-staged gather variants
@@ -98,9 +98,10 @@ long long ddfa_launch_count(void) { return ddfa::g_launches.load(std::memory_ord
 int ddfa_device_supported(void) {
   int dev = 0;
   DDFA_CUDA(cudaGetDevice(&dev));
-  int major = 0;
+  int major = 0, minor = 0;
   DDFA_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  return major == 10 ? 1 : 0;
+  DDFA_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  return (major == 9 && minor == 0) ? 1 : 0;      // the code is built for sm_90a only
 }
 
 }  // extern "C"

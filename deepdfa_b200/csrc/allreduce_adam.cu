@@ -137,7 +137,7 @@ extern "C" int ddfa_allreduce_adam_p2p(void *const *peer_params, const void *con
   const int64_t per = ((numel >> 2) + world - 1) / world;
   int blocks = (int)((per + 255) / 256);
   if (blocks < 1) blocks = 1;
-  if (blocks > 64) blocks = 64;        // all CTAs must be co-resident: they spin on flags (64 x 256 threads fit any idle B200)
+  if (blocks > 64) blocks = 64;        // all CTAs must be co-resident: they spin on flags (64 x 256 threads fit any idle H100)
   p2p::allreduce_adam_p2p_kernel<<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out, ticket,
                                                              lr, beta1, beta2, eps, weight_decay);
   DDFA_CHECK_LAUNCH("allreduce_adam_p2p_kernel");

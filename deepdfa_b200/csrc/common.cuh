@@ -1,4 +1,4 @@
-// Shared helpers for libddfa_b200.so (sm_100a only).
+// Shared helpers for libddfa_b200.so (sm_90a only: NVIDIA H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,8 +43,8 @@ inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------------------------------
 // The per-step kernels form a chain in one stream.  Launched with the programmatic-serialization attribute, kernel i+1's CTAs
 // may start as soon as every CTA of kernel i has called pdl_launch_dependents() and an SM has room — i.e. in kernel i's tail
-// (the persistent GEMM kernels leave 10-19 % of the SMs idle at the end: 300 tiles over 37 / 74 CTA groups) — run their
-// prologue (barrier init, TMEM allocation, weights -> TMEM) and then block in pdl_wait() until kernel i has completed and its
+// (the persistent GEMM kernels leave part of the SMs idle at the end, when the tiles do not divide evenly over the CTA groups) —
+// run their prologue (barrier init, the weight copy into shared memory) and then block in pdl_wait() until kernel i has completed and its
 // writes are visible.  Rules for every kernel launched this way:
 //   * nothing is written before pdl_wait();
 //   * the only global data read before pdl_wait() are the packed weights of the pass;
@@ -60,13 +60,12 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 int pdl_mask();       // abi.cu: DDFA_TUNE_PDL_MASK — bit mask of the kernels launched programmatically (1 gather_image, 2 gru_fwd3, 4 gate_bwd, 8 dgrad3)
 int gather_variant(); // abi.cu: DDFA_TUNE_GATHER_VARIANT
-int fwd_pair();       // abi.cu: DDFA_TUNE_FWD_PAIR — forward GRU kernel as CTA pairs (cta_group::2)
 int gather_src_groups();   // abi.cu: DDFA_TUNE_GATHER_SRC_GROUPS — row groups per warp of the image->image gather (0 = by size)
 int gate_bwd_tma();   // abi.cu: DDFA_TUNE_GATE_BWD_TMA — TMA-staged gate backward kernel (packed saved state)
 void chain_break();   // abi.cu: the next launch_chain() on this thread is a normal (fully serialised) launch
 bool chain_take_break();
 
-// cluster_x > 1: the grid is launched as thread-block clusters of that many CTAs along x (CTA pairs for cta_group::2 kernels)
+// cluster_x > 1: the grid is launched as thread-block clusters of that many CTAs along x
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_chain_cluster(int which, int cluster_x, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
                                         cudaStream_t stream, Args... args) {
@@ -103,15 +102,15 @@ int adam_step_inc_launch(int32_t *step_count, cudaStream_t stream);   // loss_ad
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // sgemm.cu — SIMT fp32 GEMM, C = alpha*op(A)op(B) + beta*C (row-major)
 int sgemm(int ta, int tb, int M, int N, int K, float alpha, const float *A, int lda, const float *B, int ldb,
           float beta, float *C, int ldc, int split_k, cudaStream_t stream);
-// gru_tc_fwd3.cu — tcgen05 engine, forward (D == 128): activation images
+// gru_tc_fwd3.cu — tensor-core engine, forward (D == 128): activation images
 size_t act_image_bytes(int64_t n);
 int act_to_image(const float *x, int32_t N, void *image, cudaStream_t stream);
-// gru_tc_fwd3.cu — forward, weights-in-TMEM orientation
+// gru_tc_fwd3.cu — forward, weights resident in shared memory (wgmma)
 size_t gru_tc3_packed_bytes();
 int gru_tc3_prepare(const float *w_fold, const float *b_fold, const float *b_ih, const float *w_hh, const float *b_hh, void *packed,
                     cudaStream_t stream);
@@ -127,7 +126,7 @@ int gru_tc2_prepare(const float *w_fold, const float *b_fold, const float *b_ih,
 int gru_tc2_step_fwd(const void *s_img, const void *h_img, const float *h, const int32_t *indptr, int32_t N, float *h_out,
                      void *h_out_img, float *save_gates, void *save_gates_packed, const void *workspace, size_t workspace_bytes,
                      cudaStream_t stream);
-// gru_tc_bwd.cu — tcgen05 engine, backward (gate backward -> q images, dgrad, wgrad)
+// gru_tc_bwd.cu — tensor-core engine, backward (gate backward -> q images, dgrad, wgrad)
 size_t gru_tc2_bwd_workspace_bytes(int32_t N, int32_t slots);
 void *gru_tc2_bwd_s_image_scratch(void *workspace, int32_t N);   // one image inside the workspace for the fp32-s entry point
 int gru_tc2_prepare_bwd(const float *w_fold, const float *w_hh, void *workspace, size_t workspace_bytes, cudaStream_t stream);
@@ -155,7 +154,7 @@ __device__ __forceinline__ float4 ldg_nc_f4(const float *p) {
 __device__ __forceinline__ float4 ldg_cg_f4(const float *p) { return __ldcg(reinterpret_cast<const float4 *>(p)); }
 
 // ---- L2 eviction-priority hints (createpolicy + .L2::cache_hint) -----------------------------------------------------------
-// The train step moves ~5.9 GB through a 126 MB L2 per step; what a kernel writes for a consumer many kernels later (the saved
+// The train step moves several GB through a 50 MB L2 per step; what a kernel writes for a consumer many kernels later (the saved
 // gates) should not push out what the next kernel needs, and what dies after the next kernel (ds, dh, dh'z) should stay.
 // kind: 0 = evict_normal, 1 = evict_first, 2 = evict_last.
 __device__ __forceinline__ uint64_t l2_policy(int kind) {
@@ -170,6 +169,12 @@ __device__ __forceinline__ void st_f32_hint(float *p, float v, uint64_t pol) {
 }
 __device__ __forceinline__ void st_f4_hint(float *p, const float4 &v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_f2_hint(float *p, const float2 &v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1,%2}, %3;" ::"l"(p), "f"(v.x), "f"(v.y), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_u4_hint(void *p, const uint4 &v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
 }
 __device__ __forceinline__ float4 ldg_cg_f4_hint(const float *p, uint64_t pol) {
   float4 v;

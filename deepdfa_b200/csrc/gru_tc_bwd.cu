@@ -1,4 +1,4 @@
-// tcgen05 engine, backward of one GRU step (D == 128) — activation images in, TMA-fed, persistent kernels.
+// Tensor-core engine, backward of one GRU step (D == 128) — activation images in, TMA-fed, persistent kernels.
 // Backward of the same math the forward kernel implements (gru_tc_fwd3.cu; reference: DDFA/code_gnn/models/flow_gnn/
 // ggnn.py:60-63 through dgl.nn.GatedGraphConv / torch.nn.GRUCell autograd).
 //
@@ -8,12 +8,12 @@
 //         transposed edge gather of the previous step's ds is folded into this kernel's row loop (no dh' round trip
 //         through HBM and one launch less per step).
 //   (2) dgrad3_kernel           ds = [q_r q_z q_n] W' ;  dh = dh' * z + [q_r q_z q_nr] Whh      K = 3D
-//         transposed GEMM: the weights live in tensor memory as the A operand, the q images stream through three 64 KB
-//         stages as the B operand, a CTA owns all 128 columns of ds or of dh (see the comment at the kernel)
+//         wgmma with the q image tiles as the A operand (two 64 KB stages) and 64 columns of the weights resident in shared
+//         memory as the B operand; a CTA owns one output (ds or dh) and one column half (see the comment at the kernel)
 //   (3) wgrad_kernel            dW' += [q_r q_z q_n]^T s ;  dWhh += [q_r q_z q_nr]^T h            K = nodes
 //         both operands are read "MN-major" straight from the images (whole 128-node tiles, three 64 KB slots); a CTA keeps
-//         its [384 x 128] fp32 partial sum in TMEM over all its tiles and folds it into a private global partial at the
-//         end; wgrad_reduce_kernel sums the partials once per backward pass.
+//         one [128 x 128] gate block of the fp32 sum in registers over all its tiles and writes it to a private global partial
+//         at the end; wgrad_reduce_kernel sums the partials once per backward pass.
 // Precision: bf16x3 everywhere (hi*hi + hi*lo + lo*hi), fp32 accumulate.
 #include <cuda_fp16.h>
 
@@ -421,99 +421,76 @@ __global__ void __launch_bounds__(kGtThreads, 1) gate_bwd_tma_kernel(const float
 }
 
 // =================================================================================================
-// (2) dgrad, weight-in-TMEM orientation ("dgrad3")
+// (2) dgrad
 // =================================================================================================
-// The in-kernel timeline of its predecessor (weight slices in shared memory; profiles/r01l_trace_dgrad.log) showed the operand feed as the bound: 96 KB of
-// shared memory hold the weight slice, only 2 x 32 KB are left for activations, and with ~1 us per copy in flight that
-// is ~35 GB/s per SM while every CTA has to pull 256 KB per tile (each q tile is read by four slice CTAs).
-// Here the GEMM is transposed:  D^T[col, node] = W^T[col, K] * Q[node, K]^T
-//   * A = the weights, held in TENSOR MEMORY for the life of the CTA (lane = output column, two bf16 per 32-bit column:
-//     K = 3 x 128 -> 192 columns hi + 192 columns lo), loaded once with tcgen05.st from a packed global array;
-//   * B = the q images (K-major SWIZZLE_128B, N = nodes), streamed through THREE 64 KB stages — all of shared memory
-//     is pipeline now (copy_bench2: 64 KB x 3 stages feeds ~130 GB/s per SM);
-//   * a CTA owns all 128 columns of one output (role 0: ds = [q_r q_z q_n] W', role 1: dh = [q_r q_z q_nr] Whh), so a q
-//     tile is read by 2 CTAs instead of 4 and 192 KB are pulled per 128 x 128 outputs (was 256 KB per 128 x 64);
-//   * D = two 64-node accumulator halves (64 TMEM columns each) so the epilogue of one half overlaps the MMAs of the other;
-//   * the epilogue thread holds one output column for 16 nodes per tcgen05.ld: a warp-wide store covers 32 consecutive
-//     columns of one node = one full 128-byte line, no shared-memory staging.
-constexpr int kD3Stages = 3;
+//   D[node, col] = Q[node, K] * W[K, col]   (role 0: ds, Q = [q_r q_z q_n], W = W' ; role 1: dh, Q = [q_r q_z q_nr], W = Whh)
+//   * B = the CTA's 64 output columns of W, resident in shared memory (K = 384 x 64 columns, hi and lo: 96 KB, one bulk copy);
+//   * A = the q image tiles (K-major SWIZZLE_128B, 128 nodes), streamed through two 64 KB stages, one bulk copy per q matrix;
+//   * a CTA = (role, column half); two consumer warpgroups of 64 nodes each, m64n64k16, bf16x3, fp32 accumulate in registers.
+//     A stage is released as soon as the MMAs of the next q matrix are issued (wgmma_wait<1>), so the copy of the next operand
+//     overlaps the MMAs of the current one.
+constexpr int kD3Stages = 2;
 constexpr int kD3StageBytes = kImageTileBytes;               // one q-matrix tile: [hi|lo][kb0|kb1], 64 KB
-constexpr int kD3WColsHalf = 192;                            // K = 384 bf16 -> 192 packed columns per variant
-constexpr int kD3AccCol = 2 * kD3WColsHalf;                  // accumulators start at TMEM column 384
-constexpr int kD3OffBar = kD3Stages * kD3StageBytes;         // 192 KB
-constexpr int kD3NumBars = 2 * kD3Stages + 4 + 1;            // a_full, a_empty, acc_full[2], acc_empty[2], w_ready
-constexpr int kD3OffTmemPtr = kD3OffBar + kD3NumBars * 8;
-constexpr int kD3SmemAlloc = kD3OffTmemPtr + 16 + 1024;
-constexpr int kD3Chunks = 2 * kD3WColsHalf / 16;             // 24 chunks of 16 TMEM columns
-constexpr size_t kD3PackedBytes = (size_t)2 * kD3Chunks * 128 * 64;   // [role][chunk][lane][16 words] = 384 KB
+constexpr int kD3WChunkBytes = 64 * 128;                     // [64 columns x 64 bf16 of K]
+constexpr int kD3WBytes = 12 * kD3WChunkBytes;               // [g][hi|lo][kb] = 96 KB per (role, column half)
+constexpr int kD3OffStage = kD3WBytes;
+constexpr int kD3OffBar = kD3OffStage + kD3Stages * kD3StageBytes;   // 224 KB
+constexpr int kD3SmemAlloc = kD3OffBar + (2 * kD3Stages + 1) * 8 + 1024;   // + slack for the 1024-byte round-up below
+constexpr int kD3Threads = 32 * kEpiWarps + 32;              // two consumer warpgroups + one producer warp
+constexpr size_t kD3PackedBytes = (size_t)4 * kD3WBytes;     // [role][column half] = 384 KB
+static_assert(kD3SmemAlloc <= 232448, "shared memory budget");
 
-// packed[role][chunk][lane j][i]: TMEM column chunk*16+i of lane j = bf16 pair (W[kk][j], W[kk+1][j]), hi for columns
-// 0..191, lo for 192..383, kk = 2 * (column mod 192); W = W' (role 0) or Whh (role 1), both [3D x D] row-major.
-__global__ void dgrad3_pack_kernel(const float *__restrict__ w_fold, const float *__restrict__ w_hh, uint32_t *__restrict__ packed) {
+// packed[role][half]: chunk (g, v, kb) at ((g * 2 + v) * 2 + kb) * 8 KB; row n holds W[128 g + 64 kb .. + 63][64 half + n]
+// (W = W' or Whh, both [3D x D] row-major).  One thread per 8-element unit.
+__global__ void dgrad3_pack_kernel(const float *__restrict__ w_fold, const float *__restrict__ w_hh, uint8_t *__restrict__ packed) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= 2 * kD3Chunks * 128) return;
-  const int lane = idx % 128, chunk = (idx / 128) % kD3Chunks, role = idx / (128 * kD3Chunks);
+  if (idx >= 4 * 3 * 64 * 16) return;
+  const int u = idx % 16, n = (idx / 16) % 64, g = (idx / (16 * 64)) % 3, rh = idx / (16 * 64 * 3);
+  const int role = rh >> 1, half = rh & 1, kb = u >> 3;
   const float *W = role == 0 ? w_fold : w_hh;
-  uint32_t w[16];
+  float x[8];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const int col = chunk * 16 + i;
-    const int v = col >= kD3WColsHalf ? 1 : 0;
-    const int kk = (col - v * kD3WColsHalf) * 2;
-    __nv_bfloat16 h0, l0, h1, l1;
-    split_bf16(W[(size_t)kk * kD + lane], h0, l0);
-    split_bf16(W[(size_t)(kk + 1) * kD + lane], h1, l1);
-    w[i] = v ? ((uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16))
-             : ((uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16));
-  }
-  uint4 *dst = reinterpret_cast<uint4 *>(packed + (size_t)idx * 16);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) dst[i] = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
+  for (int i = 0; i < 8; ++i) x[i] = W[(size_t)(g * kD + u * 8 + i) * kD + half * 64 + n];
+  uint4 ph, pl;
+  split8(x, ph, pl);
+  uint8_t *base = packed + (size_t)rh * kD3WBytes + sw128_offset(n, (u & 7) * 8);
+  *reinterpret_cast<uint4 *>(base + ((g * 2 + 0) * 2 + kb) * kD3WChunkBytes) = ph;
+  *reinterpret_cast<uint4 *>(base + ((g * 2 + 1) * 2 + kb) * kD3WChunkBytes) = pl;
 }
 
-__global__ void __launch_bounds__(kThreads, 1) dgrad3_kernel(const uint8_t *__restrict__ q_img, size_t img_stride,
-                                                             const float *__restrict__ dhz,
-                                                             const uint32_t *__restrict__ packed3, int32_t N,
-                                                             float *__restrict__ ds, float *__restrict__ dh, int hints) {
+__global__ void __launch_bounds__(kD3Threads, 1) dgrad3_kernel(const uint8_t *__restrict__ q_img, size_t img_stride,
+                                                               const float *__restrict__ dhz, const uint8_t *__restrict__ packed3,
+                                                               int32_t N, float *__restrict__ ds, float *__restrict__ dh, int hints) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + kD3OffBar;
-  auto a_full = [&](int i) { return bar0 + 8u * i; };
-  auto a_empty = [&](int i) { return bar0 + 8u * (kD3Stages + i); };
-  auto acc_full = [&](int i) { return bar0 + 8u * (2 * kD3Stages + i); };
-  auto acc_empty = [&](int i) { return bar0 + 8u * (2 * kD3Stages + 2 + i); };
-  const uint32_t w_ready = bar0 + 8u * (2 * kD3Stages + 4);
-  volatile uint32_t *tmem_ptr_smem = reinterpret_cast<volatile uint32_t *>(smem + kD3OffTmemPtr);
+  auto full = [&](int i) { return bar0 + 8u * i; };
+  auto empty = [&](int i) { return bar0 + 8u * (kD3Stages + i); };
+  const uint32_t w_full = bar0 + 8u * (2 * kD3Stages);
+  const int tron = (g_trace_on == 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int role = blockIdx.x & 1;
-  const int group = blockIdx.x >> 1, num_groups = gridDim.x >> 1;
+  const int rh = blockIdx.x & 3, role = rh >> 1, half = rh & 1;
+  const int group = blockIdx.x >> 2, num_groups = gridDim.x >> 2;
   const int num_tiles = (N + kTileM - 1) / kTileM;
   const int my_tiles = (num_tiles > group) ? (num_tiles - 1 - group) / num_groups + 1 : 0;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kD3Stages; ++i) { mbar_init(a_full(i), 1); mbar_init(a_empty(i), 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(acc_full(i), 1); mbar_init(acc_empty(i), kEpiWarps); }
-    mbar_init(w_ready, kEpiWarps);
+    for (int i = 0; i < kD3Stages; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), kEpiWarps); }
+    mbar_init(w_full, 1);
     mbar_fence_init();
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(smem_u32((const void *)tmem_ptr_smem), 512);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const int tron = (g_trace_on == 1);
   if (threadIdx.x == 0) trace_stamp(tron, 0, 0);
   pdl_launch_dependents();
 
-  if (warp == 0) {
-    // ===== producer: per tile the three q matrices of this role, one 64 KB copy each =====
-    if (elect_one()) {
-      pdl_wait();      // the q images come from gate_bwd_image_kernel, the previous kernel of the chain
+  if (warp == kEpiWarps) {
+    // ===== producer: the weights once, then per tile the three q matrices of this role, one 64 KB copy each =====
+    if (my_tiles > 0 && elect_one()) {
+      mbar_arrive_expect_tx(w_full, kD3WBytes);
+      bulk_g2s(sbase, packed3 + (size_t)rh * kD3WBytes, kD3WBytes, w_full);
+      pdl_wait();      // the q images come from the gate backward kernel, the previous kernel of the chain
       const uint64_t pol_q = l2_policy((hints & 64) ? 1 : 0);
       int cc = 0;
       for (int k = 0; k < my_tiles; ++k) {
@@ -521,317 +498,210 @@ __global__ void __launch_bounds__(kThreads, 1) dgrad3_kernel(const uint8_t *__re
         for (int g = 0; g < 3; ++g, ++cc) {
           const int m = g < 2 ? g : (role == 0 ? 2 : 3);      // q_r, q_z, then q_n (ds) or q_nr (dh)
           const int stage = cc % kD3Stages, use = cc / kD3Stages;
-          if (use > 0) mbar_wait(a_empty(stage), (use - 1) & 1);
-          if (g == 0) trace_stamp(tron, k, 1);
-          mbar_arrive_expect_tx(a_full(stage), kD3StageBytes);
-          bulk_g2s_hint(sbase + stage * kD3StageBytes, q_img + (size_t)m * img_stride + (size_t)tile * kImageTileBytes, kD3StageBytes,
-                        a_full(stage), pol_q);
-          if (g == 2) trace_stamp(tron, k, 2);
+          if (use > 0) mbar_wait_bounded(empty(stage), (use - 1) & 1);
+          mbar_arrive_expect_tx(full(stage), kD3StageBytes);
+          bulk_g2s_hint(sbase + kD3OffStage + stage * kD3StageBytes, q_img + (size_t)m * img_stride + (size_t)tile * kImageTileBytes,
+                        kD3StageBytes, full(stage), pol_q);
+          if (g != 1) trace_stamp(tron, k, g == 0 ? 1 : 2);      // 1: first / 2: last q copy of the tile issued
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (my_tiles > 0 && elect_one()) {
-      constexpr uint32_t kIdesc64 = make_idesc(64);
-      mbar_wait(w_ready, 0);
-      tc_fence_after();
-      int cc = 0;
-      for (int k = 0; k < my_tiles; ++k) {
-        for (int g = 0; g < 3; ++g, ++cc) {
-          const int stage = cc % kD3Stages, use = cc / kD3Stages;
-          mbar_wait(a_full(stage), use & 1);
-          tc_fence_after();
-          if (g == 0) trace_stamp(tron, k, 4);
-          if (g == 2) trace_stamp(tron, k, 5);
-          for (int half = 0; half < 2; ++half) {
-            if (g == 0 && k > 0) {
-              mbar_wait(acc_empty(half), (k - 1) & 1);
-              tc_fence_after();
-              if (half == 0) trace_stamp(tron, k, 3);
-            }
-            const uint32_t d_addr = tmem_base + (uint32_t)(kD3AccCol + half * 64);
-            // nodes 64*half.. of each 16 KB chunk: [hi kb0 | hi kb1 | lo kb0 | lo kb1]
-            const uint64_t b_base = make_desc(sbase + stage * kD3StageBytes + (uint32_t)half * 8192u);
-            const uint32_t a_base = tmem_base + (uint32_t)(g * 64);
-#pragma unroll
-            for (int kb = 0; kb < 2; ++kb) {
-#pragma unroll
-              for (int k4 = 0; k4 < 4; ++k4) {
-                const uint32_t kk2 = (uint32_t)(kb * 32 + k4 * 8);                           // packed weight column of this K step
-                const uint64_t b_hi = desc_advance(b_base, (uint32_t)kb * kChunkBytes + k4 * 32);
-                const uint64_t b_lo = desc_advance(b_base, (uint32_t)(2 + kb) * kChunkBytes + k4 * 32);
-                const uint32_t first = (g == 0 && kb == 0 && k4 == 0) ? 0u : 1u;
-                umma_f16_ts(d_addr, a_base + kk2, b_hi, kIdesc64, first);                       // w_hi q_hi
-                umma_f16_ts(d_addr, a_base + kD3WColsHalf + kk2, b_hi, kIdesc64, 1u);           // w_lo q_hi
-                umma_f16_ts(d_addr, a_base + kk2, b_lo, kIdesc64, 1u);                          // w_hi q_lo
-              }
-            }
-            if (g == 2) umma_commit(acc_full(half));
-          }
-          umma_commit(a_empty(stage));
-        }
-        trace_stamp(tron, k, 6);
-      }
-    }
-  } else {
-    // ===== weights -> tensor memory, then the epilogue =====
-    const int q = warp & 3;                  // TMEM lane quarter: output columns 32q .. 32q+31
-    const int e = (warp - 2) >> 2;           // which 32 nodes of a 64-node half (and which 12 weight chunks)
-    const int col = q * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    if (my_tiles > 0) {
-      const uint4 *src = reinterpret_cast<const uint4 *>(packed3) + ((size_t)role * kD3Chunks * 128 + (size_t)col) * 4;
-#pragma unroll 4
-      for (int c = 0; c < kD3Chunks / 2; ++c) {
-        const int chunk = e * (kD3Chunks / 2) + c;
-        const uint4 *p = src + (size_t)chunk * 128 * 4;
-        const uint4 x0 = __ldcg(p), x1 = __ldcg(p + 1), x2 = __ldcg(p + 2), x3 = __ldcg(p + 3);   // L2 loads: PDL rules, common.cuh
-        const uint32_t w[16] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w, x2.x, x2.y, x2.z, x2.w, x3.x, x3.y, x3.z, x3.w};
-        tmem_st16(lane_addr + (uint32_t)(chunk * 16), w);
-      }
-      tmem_st_wait();
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(w_ready);
-    pdl_wait();
-
-    float *out = role == 0 ? ds : dh;
-    const uint64_t pol_tmp = l2_policy((hints & 4) ? 2 : 0);       // ds / dh die after the next kernel has read them
-    const uint64_t pol_dhz = l2_policy((hints & 8) ? 1 : 0);       // last read of dh'z
-    const bool tr = (warp == 2 && lane == 0);
-    for (int k = 0; k < my_tiles; ++k) {
-      const int tile = num_tiles - 1 - (group + k * num_groups);
-      if (tr) trace_stamp(tron, k, 7);
-      for (int half = 0; half < 2; ++half) {
-        const int64_t node0 = (int64_t)tile * kTileM + half * 64 + e * 32;
-        int rows_valid = (int)((int64_t)N - node0);
-        rows_valid = rows_valid < 0 ? 0 : (rows_valid > 32 ? 32 : rows_valid);
-        float dv[32];
-        if (role == 1) {       // dh = acc + (dh' * z) : fetch the elementwise term (written by gate_bwd) while the MMAs run
-#pragma unroll
-          for (int i = 0; i < 32; ++i) dv[i] = (i < rows_valid) ? ldg_cg_f32_hint(dhz + (node0 + i) * kD + col, pol_dhz) : 0.f;
-        }
-        mbar_wait(acc_full(half), k & 1);
-        tc_fence_after();
-        if (tr && half == 0) trace_stamp(tron, k, 8);
-        const uint32_t taddr = lane_addr + (uint32_t)(kD3AccCol + half * 64 + e * 32);
-        float v0[16], v1[16];
-        tmem_ld16(taddr, v0);
-        tmem_ld16(taddr + 16, v1);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(acc_empty(half));
-        if (tr && half == 0) trace_stamp(tron, k, 9);
-        float *o = out + node0 * kD + col;
-        if (role == 1) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            v0[i] += dv[i];
-            v1[i] += dv[16 + i];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          if (i < rows_valid) st_f32_hint(o + (size_t)i * kD, v0[i], pol_tmp);
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          if (16 + i < rows_valid) st_f32_hint(o + (size_t)(16 + i) * kD, v1[i], pol_tmp);
-      }
-      if (tr) trace_stamp(tron, k, 10);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  // ===== consumers: warpgroup wg owns nodes 64 wg .. 64 wg + 63 of every tile =====
+  pdl_wait();
+  if (my_tiles == 0) return;
+  const int wg = warp >> 2;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int col0 = half * 64 + 2 * (lane & 3);
+  float *out = role == 0 ? ds : dh;
+  const uint64_t pol_tmp = l2_policy((hints & 4) ? 2 : 0);       // ds / dh die after the next kernel has read them
+  const uint64_t pol_dhz = l2_policy((hints & 8) ? 1 : 0);       // last read of dh'z
+  mbar_wait_bounded(w_full, 0);
+  const bool tr = (warp == 0 && lane == 0);
+  int cc = 0, pending = -1;      // pending: the stage whose MMAs were issued last and not yet waited for
+  for (int k = 0; k < my_tiles; ++k) {
+    const int tile = num_tiles - 1 - (group + k * num_groups);
+    float acc[32];
+    if (tr) { trace_stamp(tron, k, 7); trace_stamp(tron, k, 3); }
+    for (int g = 0; g < 3; ++g, ++cc) {
+      const int stage = cc % kD3Stages, use = cc / kD3Stages;
+      mbar_wait_bounded(full(stage), use & 1);
+      if (tr && g != 1) trace_stamp(tron, k, g == 0 ? 4 : 5);      // 4: first / 5: last q tile landed
+      wgmma_fence();
+      const uint32_t a0 = sbase + kD3OffStage + stage * kD3StageBytes + wg * 8192;
+      const uint32_t w0 = sbase + g * 4 * kD3WChunkBytes;
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb) {
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4) {
+          const uint64_t a_hi = gmma_desc(a0 + kb * kChunkBytes + k4 * 32), a_lo = gmma_desc(a0 + (2 + kb) * kChunkBytes + k4 * 32);
+          const uint64_t b_hi = gmma_desc(w0 + kb * kD3WChunkBytes + k4 * 32), b_lo = gmma_desc(w0 + (2 + kb) * kD3WChunkBytes + k4 * 32);
+          wgmma_n64<0, 0>(acc, a_hi, b_hi, (g == 0 && kb == 0 && k4 == 0) ? 0u : 1u);
+          wgmma_n64<0, 0>(acc, a_hi, b_lo, 1u);
+          wgmma_n64<0, 0>(acc, a_lo, b_hi, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      __syncwarp();
+      if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+      pending = stage;
+    }
+    // dh = acc + (dh' * z): fetch the elementwise term (written by the gate backward) while the last MMAs run
+    float2 dv[2][8];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        dv[hh][j] = make_float2(0.f, 0.f);
+        if (role == 1 && node < N) {
+          const float *p = dhz + node * kD + col0 + 8 * j;
+          dv[hh][j] = make_float2(ldg_cg_f32_hint(p, pol_dhz), ldg_cg_f32_hint(p + 1, pol_dhz));
+        }
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (tr) { trace_stamp(tron, k, 6); trace_stamp(tron, k, 8); }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty(pending));
+    pending = -1;
+    if (tr) trace_stamp(tron, k, 9);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
+      if (node < N) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          st_f2_hint(out + node * kD + col0 + 8 * j, make_float2(acc[4 * j + 2 * hh] + dv[hh][j].x, acc[4 * j + 2 * hh + 1] + dv[hh][j].y), pol_tmp);
+      }
+    }
+    if (tr) trace_stamp(tron, k, 10);
   }
 }
 
 // =================================================================================================
 // (3) wgrad
 // =================================================================================================
-// Operands are whole 128-node image tiles (64 KB, ONE bulk copy each — see the copy-size note in gru_tc_fwd.cu),
-// three 64 KB slots.  Per tile the operand sequence is B_t, A_0, A_1, A_2 (B_t = s or h tile, A_g = q tiles);
-// B_t must stay until A_2 is consumed, so the slots rotate:  slot(B_i) = (-i) mod 3, A_0 -> slot(B)+1, A_1 ->
-// slot(B)+2, A_2 -> the slot A_0 just released.  Both operands are read MN-major (K = nodes).
-constexpr int kWgSlotBytes = kImageTileBytes;             // 64 KB
-constexpr int kWgSlots = 3;
-constexpr int kWgOffBar = kWgSlots * kWgSlotBytes;        // 192 KB
-constexpr int kWgNumBars = 2 * kWgSlots + 1;
-constexpr int kWgOffTmemPtr = kWgOffBar + kWgNumBars * 8;
-constexpr int kWgSmemAlloc = kWgOffTmemPtr + 16 + 1024;
-constexpr size_t kWgPartialFloats = (size_t)3 * kD * kD;  // one CTA's [384 x 128] partial sum
-
-__device__ __forceinline__ int wg_slot(int tile_i, int w) {   // w: 0 = B, 1..3 = A_0..A_2
-  const int sb = (3 - tile_i % 3) % 3;
-  return w == 0 ? sb : (w == 2 ? (sb + 2) % 3 : (sb + 1) % 3);
-}
-
-// grid = (ctas, 2): blockIdx.y = role: 0: A in {q_r,q_z,q_n}, B = s image -> dW' ; 1: A in {q_r,q_z,q_nr}, B = h image -> dWhh.
+//   dW'[128 g + m, n] += sum_node q_g[node, m] s[node, n] ;  dWhh likewise with h (K = nodes)
+// grid = (ctas, 6): blockIdx.y = 3 role + g.  A CTA owns one [128 x 128] gate block of one role: per tile it streams the s / h tile
+// (B) and the q_g tile (A) through a ring of three 64 KB slots; both operands are read MN-major straight from the images.  Two
+// consumer warpgroups hold rows 0-63 / 64-127 of the block (m64n128k16, bf16x3) in registers over all the CTA's tiles and
+// write them to a private partial sum at the end.
 // partial: [2][ctas][384*128] fp32, private per CTA: accumulate (first == 0) or overwrite (first != 0); the sum over CTAs
 // is taken once per backward pass by wgrad_reduce_kernel (no atomics on the hot path).
 // One launch may cover several time steps (K = steps x nodes): the q images of step t are at q_img + t * step_stride, its
 // B operands are batch.s_img[t] / batch.h_img[t].  Batching all T steps of a backward pass into one launch removes T-1
-// epilogues (read-modify-write of the 58 MB of private partial sums), T-1 pipeline ramps and T-1 launches.
+// epilogues (read-modify-write of the private partial sums), T-1 pipeline ramps and T-1 launches.
+constexpr int kWgSlotBytes = kImageTileBytes;             // 64 KB
+constexpr int kWgSlots = 3;
+constexpr int kWgOffBar = kWgSlots * kWgSlotBytes;        // 192 KB
+constexpr int kWgSmemAlloc = kWgOffBar + 2 * kWgSlots * 8 + 1024;
+constexpr int kWgThreads = 32 * kEpiWarps + 32;
+constexpr size_t kWgPartialFloats = (size_t)3 * kD * kD;  // one CTA slot's [384 x 128] partial sum
 constexpr int kWgMaxSteps = 16;
 struct WgBatch {
   const uint8_t *s_img[kWgMaxSteps];
   const uint8_t *h_img[kWgMaxSteps];
   int32_t steps;
 };
-__global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const uint8_t *__restrict__ q_img, size_t img_stride, size_t step_stride,
-                                                            const __grid_constant__ WgBatch batch,
-                                                            int32_t N, float *__restrict__ partial, int first, int hints) {
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const uint8_t *__restrict__ q_img, size_t img_stride, size_t step_stride,
+                                                              const __grid_constant__ WgBatch batch,
+                                                              int32_t N, float *__restrict__ partial, int first, int hints) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + kWgOffBar;
-  auto full_bar = [&](int i) { return bar0 + 8u * i; };
-  auto empty_bar = [&](int i) { return bar0 + 8u * (kWgSlots + i); };
-  const uint32_t acc_bar = bar0 + 8u * (2 * kWgSlots);
-  volatile uint32_t *tmem_ptr_smem = reinterpret_cast<volatile uint32_t *>(smem + kWgOffTmemPtr);
+  auto full = [&](int i) { return bar0 + 8u * i; };
+  auto empty = [&](int i) { return bar0 + 8u * (kWgSlots + i); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int role = blockIdx.y;
+  const int role = blockIdx.y / 3, g = blockIdx.y % 3;
+  const int qm = g < 2 ? g : (role == 0 ? 2 : 3);            // q_r, q_z, then q_n (dW') or q_nr (dWhh)
   const int num_tiles = (N + kTileM - 1) / kTileM;           // per time step
   const int all_tiles = num_tiles * batch.steps;
   const int my_tiles = (all_tiles > (int)blockIdx.x) ? (all_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kWgSlots; ++i) { mbar_init(full_bar(i), 1); mbar_init(empty_bar(i), 1); }
-    mbar_init(acc_bar, 1);
+    for (int i = 0; i < kWgSlots; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), kEpiWarps); }
     mbar_fence_init();
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(smem_u32((const void *)tmem_ptr_smem), 512);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const int tron = (g_trace_on == 2) && blockIdx.y == 0;   // timeline of the role-0 CTAs (ddfa_debug_set key 2, value 2)
+  const int tron = (g_trace_on == 2) && blockIdx.y == 0;   // timeline of the gate-block-0 CTAs of dW' (ddfa_debug_set key 2, value 2)
   if (threadIdx.x == 0) trace_stamp(tron, 0, 0);
 
-  if (warp == 0) {
+  if (warp == kEpiWarps) {
+    // ===== producer: per tile the B tile (s or h) then the A tile (q_g) =====
     if (elect_one()) {
       const uint64_t pol_wg = l2_policy((hints & 32) ? 1 : 0);     // every operand of the batched launch is read once
-      int uses[kWgSlots] = {0, 0, 0};
       for (int i = 0; i < my_tiles; ++i) {
         const int idx = (int)blockIdx.x + i * (int)gridDim.x;
         const int t = idx / num_tiles, tile = idx - t * num_tiles;
-        for (int w = 0; w < 4; ++w) {
-          const int slot = wg_slot(i, w);
-          if (uses[slot] > 0) mbar_wait(empty_bar(slot), (uses[slot] - 1) & 1);
-          ++uses[slot];
-          if (w == 0) trace_stamp(tron, i, 1);
-          if (w == 3) trace_stamp(tron, i, 2);
-          const uint8_t *src;
-          if (w == 0) src = (role == 0) ? batch.s_img[t] : batch.h_img[t];
-          else {
-            const int pl = (w == 3) ? (role == 0 ? 2 : 3) : (w - 1);
-            src = q_img + (size_t)t * step_stride + (size_t)pl * img_stride;
-          }
-          mbar_arrive_expect_tx(full_bar(slot), kWgSlotBytes);
-          bulk_g2s_hint(sbase + slot * kWgSlotBytes, src + (size_t)tile * kImageTileBytes, kWgSlotBytes, full_bar(slot), pol_wg);
+        for (int w = 0; w < 2; ++w) {
+          const int cc = 2 * i + w, slot = cc % kWgSlots, use = cc / kWgSlots;
+          if (use > 0) mbar_wait_bounded(empty(slot), (use - 1) & 1);
+          const uint8_t *src = w == 0 ? (role == 0 ? batch.s_img[t] : batch.h_img[t]) : q_img + (size_t)t * step_stride + (size_t)qm * img_stride;
+          mbar_arrive_expect_tx(full(slot), kWgSlotBytes);
+          bulk_g2s_hint(sbase + slot * kWgSlotBytes, src + (size_t)tile * kImageTileBytes, kWgSlotBytes, full(slot), pol_wg);
+          trace_stamp(tron, i, 1 + w);      // 1: B (s / h) copy issued, 2: A (q) copy issued
         }
       }
     }
-  } else if (warp == 1) {
-    if (my_tiles > 0 && elect_one()) {
-      constexpr uint32_t kIdescMN = make_idesc(128, true, true);
-      int uses[kWgSlots] = {0, 0, 0};
-      for (int i = 0; i < my_tiles; ++i) {
-        const int slot_b = wg_slot(i, 0);
-        mbar_wait(full_bar(slot_b), uses[slot_b] & 1);
-        ++uses[slot_b];
-        trace_stamp(tron, i, 3);
-        for (int g = 0; g < 3; ++g) {
-          const int slot_a = wg_slot(i, 1 + g);
-          mbar_wait(full_bar(slot_a), uses[slot_a] & 1);
-          ++uses[slot_a];
-          tc_fence_after();
-          if (g == 0) trace_stamp(tron, i, 4);
-          if (g == 2) trace_stamp(tron, i, 5);
-          const uint32_t a0 = sbase + slot_a * kWgSlotBytes, b0 = sbase + slot_b * kWgSlotBytes;
-          const uint32_t d_addr = tmem_base + (uint32_t)g * 128u;
+    return;
+  }
+
+  const int wg = warp >> 2;
+  float acc[64];
 #pragma unroll
-          for (int k16 = 0; k16 < kTileM / 16; ++k16) {
-            const uint32_t koff = (uint32_t)k16 * 2048u;     // 16 nodes = two 8-node groups of 1024 B
-            const uint32_t vs = 2 * kChunkBytes;             // hi -> lo variant ([v][kb] chunks of 16 KB)
-            const uint32_t acc = (i > 0 || k16 > 0) ? 1u : 0u;
-            umma_f16(d_addr, make_desc_mn(a0 + koff, kChunkBytes), make_desc_mn(b0 + koff, kChunkBytes), kIdescMN, acc);       // a_hi b_hi
-            umma_f16(d_addr, make_desc_mn(a0 + vs + koff, kChunkBytes), make_desc_mn(b0 + koff, kChunkBytes), kIdescMN, 1u);   // a_lo b_hi
-            umma_f16(d_addr, make_desc_mn(a0 + koff, kChunkBytes), make_desc_mn(b0 + vs + koff, kChunkBytes), kIdescMN, 1u);   // a_hi b_lo
-          }
-          umma_commit(empty_bar(slot_a));
-        }
-        umma_commit(empty_bar(slot_b));
-        trace_stamp(tron, i, 6);
-      }
-      umma_commit(acc_bar);
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int i = 0; i < my_tiles; ++i) {
+    const int cb = 2 * i, ca = 2 * i + 1;
+    mbar_wait_bounded(full(cb % kWgSlots), (cb / kWgSlots) & 1);
+    if (warp == 0 && lane == 0) trace_stamp(tron, i, 3);
+    mbar_wait_bounded(full(ca % kWgSlots), (ca / kWgSlots) & 1);
+    if (warp == 0 && lane == 0) { trace_stamp(tron, i, 4); trace_stamp(tron, i, 5); }
+    const uint32_t b0 = sbase + (cb % kWgSlots) * kWgSlotBytes;
+    const uint32_t a0 = sbase + (ca % kWgSlots) * kWgSlotBytes + wg * kChunkBytes;      // q columns 64 wg .. 64 wg + 63
+    constexpr uint32_t vs = 2 * kChunkBytes;                                              // hi -> lo variant
+    wgmma_fence();
+#pragma unroll
+    for (int k16 = 0; k16 < kTileM / 16; ++k16) {
+      const uint32_t koff = (uint32_t)k16 * 2048u;      // 16 nodes = two 8-node groups of 1024 B
+      const uint64_t a_hi = gmma_desc(a0 + koff, kChunkBytes), a_lo = gmma_desc(a0 + vs + koff, kChunkBytes);
+      const uint64_t b_hi = gmma_desc(b0 + koff, kChunkBytes), b_lo = gmma_desc(b0 + vs + koff, kChunkBytes);
+      wgmma_n128<1, 1>(acc, a_hi, b_hi, 1u);
+      wgmma_n128<1, 1>(acc, a_lo, b_hi, 1u);
+      wgmma_n128<1, 1>(acc, a_hi, b_lo, 1u);
     }
-  } else {
-    // epilogue: this CTA's private partial sums.  Thread = one of the 128 rows of a gate block, this warp's 64 columns;
-    // the read-modify-write of the partial slot goes through a warp-private staging tile [32 rows][68 floats] carved out
-    // of the (now idle) operand ring, so global accesses are 256-byte row segments instead of 16-byte pieces.
-    const int lw = warp - 2, qd = warp & 3, chalf = lw >> 2;
-    constexpr int kLd = 68;
-    float *dst0 = partial + ((size_t)role * gridDim.x + blockIdx.x) * kWgPartialFloats;
-    if (my_tiles > 0) {
-      mbar_wait(acc_bar, 0);       // every MMA (and therefore every read of the ring) has completed
-      tc_fence_after();
-    }
-    if (warp == 2 && lane == 0) trace_stamp(tron, 0, 8);
-    float *stg = reinterpret_cast<float *>(smem) + (size_t)lw * 32 * kLd;
-#pragma unroll 1
-    for (int g = 0; g < 3; ++g) {
-      // rows 32*qd .. +31 of gate block g, columns 64*chalf .. +63: lane = (row parity, 16-byte piece).  The old partial
-      // sums are requested first — all 16 loads in flight while the accumulator block is staged (the loop used to expose
-      // one memory round trip per 4 rows: 14 us of a 42 us kernel in profiles/r01o)
-      float *gdst = dst0 + (size_t)(g * 128 + qd * 32) * kD + chalf * 64;
-      const int piece = lane & 15;
-      float4 old[16];
+    wgmma_commit();
+    if (warp == 0 && lane == 0) trace_stamp(tron, i, 6);
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(empty(cb % kWgSlots)); mbar_arrive(empty(ca % kWgSlots)); }
+  }
+  wgmma_fence_regs(acc);
+  if (warp == 0 && lane == 0) trace_stamp(tron, 0, 8);
+  // this CTA's private partial: rows 128 g + (fragment row), 128 columns; every CTA writes its slot (zeros if it owns no tile)
+  float *dst = partial + ((size_t)role * gridDim.x + blockIdx.x) * kWgPartialFloats;
+  const int row0 = g * kD + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float *rowp = dst + (size_t)(row0 + 8 * hh) * kD + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      float2 v = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
       if (!first) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) old[j] = *reinterpret_cast<const float4 *>(gdst + (size_t)(2 * j + (lane >> 4)) * kD + piece * 4);
+        const float2 o = *reinterpret_cast<const float2 *>(rowp + 8 * j);
+        v.x += o.x;
+        v.y += o.y;
       }
-#pragma unroll 1
-      for (int cc = 0; cc < 4; ++cc) {
-        float a[16];
-        if (my_tiles > 0) {
-          tmem_ld16(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(g * 128 + chalf * 64 + cc * 16), a);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int x = 0; x < 16; ++x) a[x] = 0.f;
-        }
-#pragma unroll
-        for (int x4 = 0; x4 < 4; ++x4)
-          *reinterpret_cast<float4 *>(stg + lane * kLd + cc * 16 + x4 * 4) = make_float4(a[x4 * 4], a[x4 * 4 + 1], a[x4 * 4 + 2], a[x4 * 4 + 3]);
-      }
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int row = 2 * j + (lane >> 4);
-        float4 v = *reinterpret_cast<const float4 *>(stg + row * kLd + piece * 4);
-        if (!first) f4_add(v, old[j]);
-        *reinterpret_cast<float4 *>(gdst + (size_t)row * kD + piece * 4) = v;
-      }
-      __syncwarp();
+      *reinterpret_cast<float2 *>(rowp + 8 * j) = v;
     }
-    if (warp == 2 && lane == 0) trace_stamp(tron, 0, 10);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
+  if (warp == 0 && lane == 0) trace_stamp(tron, 0, 10);
 }
 
 // dW'[384,128] += sum_cta partial[0][cta] ; dWhh += sum_cta partial[1][cta]     (once per backward pass)
@@ -852,7 +722,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float *__restri
 }  // namespace tc2b
 
 // workspace = [dgrad per-slice transposed weight images (384 KB)][q images x4][h image][wgrad partial sums: 2 x 74 x 384 x 128 fp32]
-constexpr int kWgCtas = kNumSMs / 2;
+constexpr int kWgCtas = kNumSMs / 6;       // x 6 gate blocks = one CTA per SM
 static size_t wg_partial_bytes() { return (size_t)2 * kWgCtas * tc2b::kWgPartialFloats * sizeof(float); }
 int gru_tc2b_trace_enable(int on) {
   DDFA_CUDA(cudaMemcpyToSymbol(tcc::g_trace_on, &on, sizeof(int)));
@@ -863,7 +733,6 @@ int gru_tc2b_trace_read(void *host, size_t bytes) {
   DDFA_CUDA(cudaMemcpyFromSymbol(host, tcc::g_trace, bytes));
   return DDFA_OK;
 }
-
 // workspace: [dgrad3 packed weights 384 KB][h image][dh' * z plane (image-sized)][s image (fp32-s entry only)]
 //            [wgrad partial sums][q images x 4] x slots   (one slot, or one per time step when the weight-gradient GEMM of a
 //            whole backward pass is batched into one launch)
@@ -880,8 +749,8 @@ int gru_tc2_prepare_bwd(const float *w_fold, const float *w_hh, void *workspace,
     set_error("tcgen05 engine (bwd): workspace too small");
     return DDFA_ERR_WORKSPACE;
   }
-  const int total = 2 * tc2b::kD3Chunks * 128;
-  tc2b::dgrad3_pack_kernel<<<(total + 127) / 128, 128, 0, stream>>>(w_fold, w_hh, static_cast<uint32_t *>(workspace));
+  const int total = 4 * 3 * 64 * 16;
+  tc2b::dgrad3_pack_kernel<<<(total + 127) / 128, 128, 0, stream>>>(w_fold, w_hh, static_cast<uint8_t *>(workspace));
   DDFA_CHECK_LAUNCH("tc2b::dgrad3_pack_kernel");
   chain_break();
   return DDFA_OK;
@@ -956,10 +825,10 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
   const int tiles = (N + tcc::kTileM - 1) / tcc::kTileM;
   {
     DDFA_CUDA(cudaFuncSetAttribute(tc2b::dgrad3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
-    int groups = kNumSMs / 2;
+    int groups = kNumSMs / 4;
     if (groups > tiles) groups = tiles;
-    DDFA_CUDA(launch_chain(8, tc2b::dgrad3_kernel, dim3(groups * 2), dim3(tc2b::kThreads), tc2b::kD3SmemAlloc, stream, q_img, img, dhz,
-                           reinterpret_cast<const uint32_t *>(packed), N, ds, dh, l2_hints()));
+    DDFA_CUDA(launch_chain(8, tc2b::dgrad3_kernel, dim3(groups * 4), dim3(tc2b::kD3Threads), tc2b::kD3SmemAlloc, stream, q_img, img, dhz,
+                           static_cast<const uint8_t *>(packed), N, ds, dh, l2_hints()));
     DDFA_CHECK_LAUNCH("tc2b::dgrad3_kernel");
   }
   if (wgrad_mode >= 16) return DDFA_OK;       // q images kept; the batched weight-gradient launch follows the last step
@@ -968,7 +837,7 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
   one.s_img[0] = static_cast<const uint8_t *>(s_img);
   one.h_img[0] = h_img;
   one.steps = 1;
-  tc2b::wgrad_kernel<<<dim3(kWgCtas, 2), tc2b::kThreads, tc2b::kWgSmemAlloc, stream>>>(q_img, img, 0, one, N, partial, wgrad_mode == 2 ? 0 : 1, 0);
+  tc2b::wgrad_kernel<<<dim3(kWgCtas, 6), tc2b::kWgThreads, tc2b::kWgSmemAlloc, stream>>>(q_img, img, 0, one, N, partial, wgrad_mode == 2 ? 0 : 1, 0);
   DDFA_CHECK_LAUNCH("tc2b::wgrad_kernel");
   if (wgrad_mode == 0) return gru_tc2_bwd_finish(N, dw_fold, dw_hh, workspace, workspace_bytes, stream);
   return DDFA_OK;
@@ -1001,7 +870,7 @@ int gru_tc2_bwd_wgrad_batched(const void *const *s_imgs, const void *const *h_im
   }
   b.steps = steps;
   DDFA_CUDA(cudaFuncSetAttribute(tc2b::wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kWgSmemAlloc));
-  tc2b::wgrad_kernel<<<dim3(kWgCtas, 2), tc2b::kThreads, tc2b::kWgSmemAlloc, stream>>>(q_img, img, 4 * img, b, N, partial, 1, l2_hints());
+  tc2b::wgrad_kernel<<<dim3(kWgCtas, 6), tc2b::kWgThreads, tc2b::kWgSmemAlloc, stream>>>(q_img, img, 4 * img, b, N, partial, 1, l2_hints());
   DDFA_CHECK_LAUNCH("tc2b::wgrad_kernel");
   return gru_tc2_bwd_finish(N, dw_fold, dw_hh, workspace, workspace_bytes, stream);
 }

@@ -1,4 +1,4 @@
-// tcgen05 engine, forward GRU step v3 (D == 128) — weights in TENSOR MEMORY, activations streamed as the B operand.
+// Tensor-core engine, forward GRU step (D == 128) on Hopper warpgroup MMA (wgmma), activations streamed as the A operand.
 //
 // Replaces DGL GatedGraphConv's per-step `a = W h (summed over in-edges); h = GRUCell(a, h)` (reference:
 // DDFA/code_gnn/models/flow_gnn/ggnn.py:60-63 -> dgl.nn.GatedGraphConv.forward -> torch.nn.GRUCell) for one step, given
@@ -6,21 +6,13 @@
 //     gi = s W'^T + deg * b' + b_ih ,  gh = h Whh^T + b_hh ,  r,z = sigmoid(gi + gh) ,  n = tanh(gi_n + r * gh_n) ,
 //     h' = n + z (h - n)
 //
-// Why v3.  The v2 kernel (removed; history in DESIGN.md §3) kept a 96 KB weight slice in shared memory, which leaves two 32 KB operand
-// stages; its timeline (profiles/r01l_trace_fwd.log) shows ~1 us per copy in flight, i.e. a feed of ~35 GB/s per SM, and
-// copy_bench2 (profiles/r01m_copy_bench2.log) shows a B200 SM needs >= 3 x 64 KB in flight to pull > 100 GB/s.
-// Here the GEMM is transposed,  D^T[gate column, node] = W[gate column, K] * X[node, K]^T :
-//   * A = the weight slice, resident in TMEM for the life of the CTA: lane = one of the slice's 4 x 32 pre-activation
-//     columns [gi_n | r | z | gh_n], K = 256 = [s part | h part] (zero blocks where a pre-activation does not use a part),
-//     two bf16 per 32-bit column: 128 columns hi + 128 columns lo;
-//   * B = the s and h image tiles (K-major SWIZZLE_128B, N = 128 nodes), THREE 64 KB stages, one bulk copy per tile;
-//   * D = two 128-node accumulator buffers (TMEM columns 256..511): 48 MMAs (M = 128, N = 128, K = 16) per tile,
-//     bf16x3: w_hi x_hi + w_lo x_hi + w_hi x_lo;
-//   * lane order inside a TMEM lane quarter q: lane = 8 * gate + c  (gate: 0 gi_n, 1 r, 2 z, 3 gh_n; c: column 8 q + c of
-//     the slice), so the four pre-activations of an output element are in ONE warp.  Sixteen epilogue warps (lane quarter x
-//     32-node quarter of the tile) each read 16 nodes per tcgen05.ld, swap them through a warp-private, conflict-free
-//     shared-memory tile (thread (gate, c) -> thread (node mod 4, c)), and finish nodes {g, g+4, g+8, g+12} x column c:
-//     no cross-warp barrier anywhere in the epilogue; global accesses are 32-byte row segments (full sectors).
+// A CTA owns a slice of 32 output columns and streams 128-node tiles:
+//   * B = the slice's weights, resident in shared memory for the life of the CTA (96 KB, one bulk copy): for each part
+//     (s -> W', h -> Whh) the 96 pre-activation rows [r | z | n] x 32 columns, K = 128, hi and lo bf16, K-major SWIZZLE_128B;
+//   * A = the s and h image tiles (K-major SWIZZLE_128B, 128 nodes), two 64 KB stages, one bulk copy per tile;
+//   * two consumer warpgroups, 64 nodes each: acc_s = s W'^T over [r | z | gi_n] and acc_h = h Whh^T over [r | z | gh_n]
+//     (m64n96k16, bf16x3: x_hi w_hi + x_hi w_lo + x_lo w_hi, fp32 accumulate in registers).  A thread's fragment holds all
+//     four pre-activations of its (node, column) pairs, and adjacent column pairs, so the epilogue needs no data exchange.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -32,82 +24,54 @@ using namespace tcc;
 
 constexpr int kSlices = 4;
 constexpr int kSliceCols = kD / kSlices;                  // 32 output columns per CTA
-constexpr int kStages = 3;
+constexpr int kRowsPerPart = 3 * kSliceCols;              // 96 pre-activation rows per part: [r | z | n]
+constexpr int kWChunkBytes = kRowsPerPart * 128;          // [96 rows x 64 bf16] = 12 KB
+constexpr int kSliceWBytes = 8 * kWChunkBytes;            // [part][hi|lo][kb] = 96 KB
 constexpr int kStageBytes = kImageTileBytes;              // 64 KB: one operand tile [hi|lo][kb0|kb1]
-constexpr int kWColsHalf = 128;                           // K = 256 bf16 -> 128 packed columns per variant
-constexpr int kAccCol = 2 * kWColsHalf;                   // accumulators: TMEM columns 256 .. 511
-constexpr int kChunks = 2 * kWColsHalf / 16;              // 16 chunks of 16 TMEM columns
-constexpr int kEpiWarps = 16;
-constexpr int kXGateLd = 16 * 8 + 8;                      // floats between gates in a warp's exchange tile [gate][16 nodes][8 cols] (+8: bank skew)
-constexpr int kXFloats = 4 * kXGateLd;                    // 544 floats = 2176 B per warp
-constexpr int kOffX = kStages * kStageBytes;              // 192 KB
-constexpr int kXBytes = kEpiWarps * kXFloats * 4;         // 34 KB
-constexpr int kOffBar = kOffX + kXBytes;
-constexpr int kPairStages = 6;                            // CTA-pair form: six 32 KB stages (each CTA holds 64 of a tile's 128 nodes)
-constexpr int kPairStageBytes = kStageBytes / 2;
-constexpr int kNumBars = 3 * kPairStages + 4 + 1;         // a_full, a_empty, (pair: peer_full), acc_full[2], acc_empty[2], w_ready
-constexpr int kOffTmemPtr = kOffBar + kNumBars * 8;
-constexpr int kSmemAlloc = kOffTmemPtr + 16;              // the dynamic shared window itself is 1024-byte aligned (checked)
-constexpr int kThreads = 64 + 32 * kEpiWarps;             // 576
+constexpr int kOffStage = kSliceWBytes;
+constexpr int kOffBias = kOffStage + 2 * kStageBytes;     // 224 KB
 constexpr int kBiasSlice = 7 * kSliceCols;                // per slice: const {gi_n, r, z, gh_n} then degree {gi_n, r, z}, 32 columns each
-constexpr size_t kPackedWBytes = (size_t)kSlices * kChunks * 128 * 64;     // [slice][chunk][lane][16 words] = 512 KB
+constexpr int kOffBar = kOffBias + kBiasSlice * 4;
+constexpr int kSmemAlloc = kOffBar + 5 * 8;               // full[2], empty[2], w_full; the dynamic window is 1024-byte aligned (checked)
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 32 * kConsumerWarps + 32;        // two consumer warpgroups + one producer warp
+constexpr size_t kPackedWBytes = (size_t)kSlices * kSliceWBytes;   // 384 KB
 constexpr size_t kPackedBytes = kPackedWBytes + (size_t)kSlices * kBiasSlice * 4;
 static_assert(kSmemAlloc <= 232448, "shared memory budget");
 
-// lane L of slice j: quarter q = L / 32, pre-activation blk = (L / 8) % 4 (0 gi_n, 1 r, 2 z, 3 gh_n), output column
-// oc = 32 j + 8 q + L % 8.  K index kk: part p = kk / 128 (0: s -> W', 1: h -> Whh), c = kk % 128.
-__device__ __forceinline__ float weight_of(const float *__restrict__ w_fold, const float *__restrict__ w_hh, int blk, int oc, int kk) {
-  const int p = kk >> 7, c = kk & 127;
-  if (blk == 0) return p == 0 ? w_fold[(size_t)(2 * kD + oc) * kD + c] : 0.f;
-  if (blk == 3) return p == 1 ? w_hh[(size_t)(2 * kD + oc) * kD + c] : 0.f;
-  const int gate = blk - 1;
-  return (p == 0 ? w_fold : w_hh)[(size_t)(gate * kD + oc) * kD + c];
-}
-
+// packed[slice]: chunk (part p, variant v, kb) at ((p * 2 + v) * 2 + kb) * 12 KB; row n = 32 b + c holds
+// W_p[b * 128 + 32 slice + c][64 kb .. 64 kb + 63] (W_0 = W', W_1 = Whh; b: 0 r, 1 z, 2 n).  One thread per 8-element unit.
 __global__ void pack_kernel(const float *__restrict__ w_fold, const float *__restrict__ w_hh, const float *__restrict__ b_fold,
                             const float *__restrict__ b_ih, const float *__restrict__ b_hh, uint8_t *__restrict__ packed) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= kSlices * kChunks * 128) return;
-  const int lane = idx % 128, chunk = (idx / 128) % kChunks, slice = idx / (128 * kChunks);
-  const int blk = (lane >> 3) & 3, oc = slice * kSliceCols + (lane >> 5) * 8 + (lane & 7);
-  uint32_t w[16];
+  if (idx >= kSlices * 2 * kRowsPerPart * 16) return;
+  const int u = idx % 16, n = (idx / 16) % kRowsPerPart, p = (idx / (16 * kRowsPerPart)) % 2, slice = idx / (32 * kRowsPerPart);
+  const int kb = u >> 3, k0 = u * 8;
+  const float *W = (p == 0 ? w_fold : w_hh) + (size_t)((n / kSliceCols) * kD + slice * kSliceCols + n % kSliceCols) * kD;
+  float x[8];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const int col = chunk * 16 + i;
-    const int v = col >= kWColsHalf ? 1 : 0;
-    const int kk = (col - v * kWColsHalf) * 2;
-    __nv_bfloat16 h0, l0, h1, l1;
-    split_bf16(weight_of(w_fold, w_hh, blk, oc, kk), h0, l0);
-    split_bf16(weight_of(w_fold, w_hh, blk, oc, kk + 1), h1, l1);
-    w[i] = v ? ((uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16))
-             : ((uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16));
-  }
-  uint4 *dst = reinterpret_cast<uint4 *>(packed) + (size_t)idx * 4;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) dst[i] = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
-  if (chunk == 0 && lane < kSliceCols) {
-    const int t = slice * kSliceCols + lane;       // output column
+  for (int i = 0; i < 8; ++i) x[i] = W[k0 + i];
+  uint4 ph, pl;
+  split8(x, ph, pl);
+  uint8_t *base = packed + (size_t)slice * kSliceWBytes + sw128_offset(n, (u & 7) * 8);
+  *reinterpret_cast<uint4 *>(base + ((p * 2 + 0) * 2 + kb) * kWChunkBytes) = ph;
+  *reinterpret_cast<uint4 *>(base + ((p * 2 + 1) * 2 + kb) * kWChunkBytes) = pl;
+  if (p == 0 && u == 0 && n < kSliceCols) {
+    const int t = slice * kSliceCols + n;       // output column
     float *bias = reinterpret_cast<float *>(packed + kPackedWBytes) + slice * kBiasSlice;
-    bias[0 * kSliceCols + lane] = b_ih[2 * kD + t];
-    bias[1 * kSliceCols + lane] = b_ih[t] + b_hh[t];
-    bias[2 * kSliceCols + lane] = b_ih[kD + t] + b_hh[kD + t];
-    bias[3 * kSliceCols + lane] = b_hh[2 * kD + t];
-    bias[4 * kSliceCols + lane] = b_fold[2 * kD + t];
-    bias[5 * kSliceCols + lane] = b_fold[t];
-    bias[6 * kSliceCols + lane] = b_fold[kD + t];
+    bias[0 * kSliceCols + n] = b_ih[2 * kD + t];
+    bias[1 * kSliceCols + n] = b_ih[t] + b_hh[t];
+    bias[2 * kSliceCols + n] = b_ih[kD + t] + b_hh[kD + t];
+    bias[3 * kSliceCols + n] = b_hh[2 * kD + t];
+    bias[4 * kSliceCols + n] = b_fold[2 * kD + t];
+    bias[5 * kSliceCols + n] = b_fold[t];
+    bias[6 * kSliceCols + n] = b_fold[kD + t];
   }
 }
 
 // HIMG: the z*h term reads h from the activation image (h == nullptr) instead of an fp32 plane.
 // GATES: 0 = nothing saved (inference), 1 = four fp32 planes (`gates`), 2 = packed 64-bit words (`gates_packed`, pack_gates).
-// PAIR: launched as 2-CTA clusters; the CTAs (2k, 2k+1) — two column slices of the same tile group — issue ONE
-//   tcgen05.mma.cta_group::2 (M = 256: rows 0-127 = the even CTA's slice, 128-255 = the odd CTA's) whose B operand, the 128-node
-//   activation tile, is split between their shared memories: each CTA copies only ITS 64 nodes of every s / h tile (4 x 8 KB
-//   pieces), so a tile is pulled from L2 twice instead of four times and the same 192 KB of shared memory hold six stages = three
-//   tiles in flight instead of one and a half.  Protocol: every CTA's copies complete on its own a_full; warp 1 of the odd CTA
-//   relays that to the leader's peer_full; the leader's MMA thread waits for both, issues, and commits with a multicast to
-//   a_empty / acc_full of BOTH CTAs; the epilogue warps of both CTAs report to the leader's acc_empty / w_ready.
-template <bool HIMG, int GATES, bool PAIR>
+template <bool HIMG, int GATES>
 __global__ void __launch_bounds__(kThreads, 1) gru_fwd3_kernel(const uint8_t *__restrict__ s_img, const uint8_t *__restrict__ h_img,
                                                                const float *__restrict__ h, const int32_t *__restrict__ indptr,
                                                                const uint8_t *__restrict__ packed, int32_t N,
@@ -117,21 +81,9 @@ __global__ void __launch_bounds__(kThreads, 1) gru_fwd3_kernel(const uint8_t *__
   const uint32_t sbase = smem_u32(smem);
   if ((sbase & 1023u) != 0) __trap();        // SWIZZLE_128B operand tiles need 1024-byte alignment
   const uint32_t bar0 = sbase + kOffBar;
-  constexpr int NS = PAIR ? kPairStages : kStages;
-  constexpr uint32_t SB = PAIR ? kPairStageBytes : kStageBytes;
-  auto a_full = [&](int i) { return bar0 + 8u * i; };
-  auto a_empty = [&](int i) { return bar0 + 8u * (kPairStages + i); };
-  auto peer_full = [&](int i) { return bar0 + 8u * (2 * kPairStages + i); };
-  auto acc_full = [&](int i) { return bar0 + 8u * (3 * kPairStages + i); };
-  auto acc_empty = [&](int i) { return bar0 + 8u * (3 * kPairStages + 2 + i); };
-  const uint32_t w_ready = bar0 + 8u * (3 * kPairStages + 4);
-  auto WAIT = [](uint32_t bar, uint32_t parity) {     // pair form: bounded (a protocol error traps instead of hanging the device)
-    if constexpr (PAIR) mbar_wait_trap(bar, parity);
-    else mbar_wait(bar, parity);
-  };
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0u;
-  volatile uint32_t *tmem_ptr_smem = reinterpret_cast<volatile uint32_t *>(smem + kOffTmemPtr);
+  auto full = [&](int i) { return bar0 + 8u * i; };
+  auto empty = [&](int i) { return bar0 + 8u * (2 + i); };
+  const uint32_t w_full = bar0 + 32u;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int slice = blockIdx.x % kSlices;
@@ -140,289 +92,161 @@ __global__ void __launch_bounds__(kThreads, 1) gru_fwd3_kernel(const uint8_t *__
   const int my_tiles = (num_tiles > group) ? (num_tiles - 1 - group) / num_groups + 1 : 0;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NS; ++i) { mbar_init(a_full(i), 1); mbar_init(a_empty(i), 1); mbar_init(peer_full(i), 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(acc_full(i), 1); mbar_init(acc_empty(i), PAIR ? 2 * kEpiWarps : kEpiWarps); }
-    mbar_init(w_ready, PAIR ? 2 * kEpiWarps : kEpiWarps);
+    for (int i = 0; i < 2; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), kConsumerWarps); }
+    mbar_init(w_full, 1);
     mbar_fence_init();
   }
-  if (warp == 0) {
-    __syncwarp();
-    if constexpr (PAIR) tmem_alloc_pair(smem_u32((const void *)tmem_ptr_smem), 512);
-    else tmem_alloc(smem_u32((const void *)tmem_ptr_smem), 512);
-  }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all();      // the peer's barriers are initialised before anyone arrives on them remotely
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  __syncthreads();
   const int tron = g_trace_on;
   if (threadIdx.x == 0) trace_stamp(tron, 0, 0);
   pdl_launch_dependents();
 
-  if (warp == 0) {
-    // ===== producer: per tile the s tile and the h tile, one 64 KB bulk copy each =====
+  if (warp == kConsumerWarps) {
+    // ===== producer: the slice's weights once, then per tile the s tile (stage 0) and the h tile (stage 1) =====
     if (my_tiles > 0 && elect_one()) {
+      mbar_arrive_expect_tx(w_full, kSliceWBytes);      // the packed weights are the one input read before pdl_wait (common.cuh)
+      bulk_g2s(sbase, packed + (size_t)slice * kSliceWBytes, kSliceWBytes, w_full);
       pdl_wait();      // the images are written by the previous kernels of the chain
-      int cc = 0;
       for (int k = 0; k < my_tiles; ++k) {
-        const int tile = group + k * num_groups;
-        for (int p = 0; p < 2; ++p, ++cc) {
-          const int stage = cc % NS, use = cc / NS;
-          if (use > 0) WAIT(a_empty(stage), (use - 1) & 1);
-          if (p == 0) trace_stamp(tron, k, 1);
-          mbar_arrive_expect_tx(a_full(stage), SB);
-          const uint8_t *src = (p == 0 ? s_img : h_img) + (size_t)tile * kImageTileBytes;
-          if constexpr (PAIR) {     // this CTA's 64 nodes of each of the four [128 x 64] chunks: rows 64 r .. 64 r + 63 = 8 KB each
-#pragma unroll
-            for (int ch = 0; ch < 4; ++ch)
-              bulk_g2s(sbase + stage * SB + ch * (kChunkBytes / 2), src + (size_t)ch * kChunkBytes + (size_t)rank * (kChunkBytes / 2),
-                       kChunkBytes / 2, a_full(stage));
-          } else {
-            bulk_g2s(sbase + stage * SB, src, SB, a_full(stage));
-          }
-          if (p == 1) trace_stamp(tron, k, 2);
+        const size_t toff = (size_t)(group + k * num_groups) * kImageTileBytes;
+        for (int p = 0; p < 2; ++p) {
+          if (k > 0) mbar_wait_bounded(empty(p), (k - 1) & 1);
+          mbar_arrive_expect_tx(full(p), kStageBytes);
+          bulk_g2s(sbase + kOffStage + p * kStageBytes, (p == 0 ? s_img : h_img) + toff, kStageBytes, full(p));
+          trace_stamp(tron, k, 1 + p);      // 1: s tile copy issued, 2: h tile copy issued
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (pair form: leader CTA only; the odd CTA's warp 1 relays "my half of the stage has landed") =====
-    if (PAIR && !leader) {
-      if (my_tiles > 0 && elect_one()) {
-        for (int cc = 0; cc < 2 * my_tiles; ++cc) {
-          const int stage = cc % NS, use = cc / NS;
-          WAIT(a_full(stage), use & 1);
-          mbar_arrive_cluster(mapa_rank(peer_full(stage), 0));
-        }
-      }
-    } else if (my_tiles > 0 && elect_one()) {
-      constexpr uint32_t kIdesc = PAIR ? make_idesc_m256(128) : make_idesc(128);
-      constexpr uint32_t CB = PAIR ? kChunkBytes / 2 : kChunkBytes;       // bytes of one chunk inside a stage
-      if constexpr (PAIR) mbar_wait_cluster(w_ready, 0);
-      else WAIT(w_ready, 0);
-      tc_fence_after();
-      int cc = 0;
-      for (int k = 0; k < my_tiles; ++k) {
-        const int buf = k & 1, buse = k >> 1;
-        if (buse > 0) {
-          if constexpr (PAIR) mbar_wait_cluster(acc_empty(buf), (buse - 1) & 1);
-          else WAIT(acc_empty(buf), (buse - 1) & 1);
-        }
-        tc_fence_after();
-        trace_stamp(tron, k, 3);
-        const uint32_t d_addr = tmem_base + (uint32_t)(kAccCol + buf * 128);
-        for (int p = 0; p < 2; ++p, ++cc) {
-          const int stage = cc % NS, use = cc / NS;
-          WAIT(a_full(stage), use & 1);
-          if constexpr (PAIR) mbar_wait_cluster(peer_full(stage), use & 1);
-          tc_fence_after();
-          if (p == 0) trace_stamp(tron, k, 4);
-          if (p == 1) trace_stamp(tron, k, 5);
-          const uint64_t b_base = make_desc(sbase + stage * SB);     // chunks [hi kb0 | hi kb1 | lo kb0 | lo kb1]
-          const uint32_t a_base = tmem_base + (uint32_t)(p * 64);
-#pragma unroll
-          for (int kb = 0; kb < 2; ++kb) {
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              const uint32_t kk2 = (uint32_t)(kb * 32 + k4 * 8);              // packed weight column of this K step
-              const uint64_t b_hi = desc_advance(b_base, (uint32_t)kb * CB + k4 * 32);
-              const uint64_t b_lo = desc_advance(b_base, (uint32_t)(2 + kb) * CB + k4 * 32);
-              const uint32_t first = (p == 0 && kb == 0 && k4 == 0) ? 0u : 1u;
-              if constexpr (PAIR) {
-                umma_f16_ts_pair(d_addr, a_base + kk2, b_hi, kIdesc, first);                    // w_hi x_hi
-                umma_f16_ts_pair(d_addr, a_base + kWColsHalf + kk2, b_hi, kIdesc, 1u);          // w_lo x_hi
-                umma_f16_ts_pair(d_addr, a_base + kk2, b_lo, kIdesc, 1u);                       // w_hi x_lo
-              } else {
-                umma_f16_ts(d_addr, a_base + kk2, b_hi, kIdesc, first);
-                umma_f16_ts(d_addr, a_base + kWColsHalf + kk2, b_hi, kIdesc, 1u);
-                umma_f16_ts(d_addr, a_base + kk2, b_lo, kIdesc, 1u);
-              }
-            }
-          }
-          if constexpr (PAIR) umma_commit_pair(a_empty(stage), (uint16_t)3);
-          else umma_commit(a_empty(stage));
-        }
-        if constexpr (PAIR) umma_commit_pair(acc_full(buf), (uint16_t)3);
-        else umma_commit(acc_full(buf));
-        trace_stamp(tron, k, 6);
-      }
-    }
-  } else {
-    // ===== weights -> tensor memory, then the epilogue =====
-    const int q = warp & 3;                  // TMEM lane quarter: columns 8q .. 8q+7 of the slice, all four pre-activations
-    const int e = (warp - 2) >> 2;           // nodes 32 e .. 32 e + 31 of the tile
-    const int g = lane >> 3, c = lane & 7;   // this lane's TMEM row = pre-activation g of column c; it finishes nodes = g (mod 4)
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    const int scol = q * 8 + c;                       // column inside the slice
-    const int gcol = slice * kSliceCols + scol;       // column of h
-    float b_gin = 0.f, b_r = 0.f, b_z = 0.f, b_ghn = 0.f, d_gin = 0.f, d_r = 0.f, d_z = 0.f;
-    if (my_tiles > 0) {
-      const uint4 *src = reinterpret_cast<const uint4 *>(packed) + ((size_t)slice * kChunks * 128 + (size_t)(q * 32 + lane)) * 4;
-#pragma unroll
-      for (int cc = 0; cc < kChunks / 4; ++cc) {
-        const int chunk = e * (kChunks / 4) + cc;
-        const uint4 *p = src + (size_t)chunk * 128 * 4;
-        const uint4 x0 = __ldcg(p), x1 = __ldcg(p + 1), x2 = __ldcg(p + 2), x3 = __ldcg(p + 3);   // L2 loads: PDL rules, common.cuh
-        const uint32_t w[16] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w, x2.x, x2.y, x2.z, x2.w, x3.x, x3.y, x3.z, x3.w};
-        tmem_st16(lane_addr + (uint32_t)(chunk * 16), w);
-      }
-      tmem_st_wait();
-      const float *bias = reinterpret_cast<const float *>(packed + kPackedWBytes) + slice * kBiasSlice + scol;
-      b_gin = __ldcg(bias); b_r = __ldcg(bias + kSliceCols); b_z = __ldcg(bias + 2 * kSliceCols); b_ghn = __ldcg(bias + 3 * kSliceCols);
-      d_gin = __ldcg(bias + 4 * kSliceCols); d_r = __ldcg(bias + 5 * kSliceCols); d_z = __ldcg(bias + 6 * kSliceCols);
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-      if (PAIR && !leader) mbar_arrive_cluster(mapa_rank(w_ready, 0));
-      else mbar_arrive(w_ready);
-    }
-    pdl_wait();        // everything above (barriers, TMEM, the packed weights) is independent of the previous kernel
-
-    const size_t plane = (size_t)N * kD;
-    const uint64_t pol_gates = l2_policy((hints & 1) ? 1 : 0);      // the saved gates are next read in the backward pass
-    const uint64_t pol_next = l2_policy((hints & 16) ? 2 : 0);      // h' and its image feed the next two kernels
-    // image addressing of this thread's (even) column pair: chunk = [variant c & 1][k-block], swizzle by row & 7
-    const int kcol = (gcol & ~1) & 63;
-    const uint32_t img_chunk_off = (uint32_t)(((c & 1) * 2 + (gcol >> 6)) * kChunkBytes);
-    uint32_t img_lane_off[2];
-#pragma unroll
-    for (int jj = 0; jj < 2; ++jj) {
-      const int r7 = g + 4 * jj;
-      img_lane_off[jj] = (uint32_t)(r7 * 128 + ((((kcol >> 3) ^ r7) & 7) << 4) + (kcol & 7) * 2);
-    }
-    float *X = reinterpret_cast<float *>(smem + kOffX) + (size_t)(warp - 2) * kXFloats;   // warp-private exchange tile
-    const bool tr = (warp == 2 && lane == 0);
-    // h and the in-degree of the 8 nodes this thread finishes per tile (two 16-node chunks x nodes g, g+4, g+8, g+12) are
-    // fetched one tile ahead, so their latency hides behind the current tile's work
-    // All loads are L2 loads (PDL rules, common.cuh).  The in-degrees of the warp's 32 nodes come in as two coalesced loads
-    // (lane = node) and are handed to the threads that need them by shuffles at use time.
-    // h itself: fp32 plane when the caller has one (h_0 = the embeddings), else reconstructed from the activation image the
-    // MMA reads (h = hi + lo, 2^-17 relative): the even lane of a column pair fetches the pair's hi word, the odd lane its lo
-    // word — the same 4-byte pieces, at the same offsets, as the image stores below — and they swap at use time.
-    float hp_n[8];
-    int ip0_n = 0, ip1_n = 0;    // raw indptr entries of node nw + lane: the subtraction waits until the values are used
-    auto prefetch = [&](int kk) {
-      const int64_t nw = (int64_t)(group + kk * num_groups) * kTileM + e * 32;
-      if constexpr (!HIMG) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int64_t node = nw + (i >> 2) * 16 + g + 4 * (i & 3);
-          const bool ok = kk < my_tiles && node < N;
-          hp_n[i] = ok ? __ldcg(h + node * kD + gcol) : 0.f;
-        }
-      } else {
-        const uint8_t *src = h_img + (size_t)(group + kk * num_groups) * kImageTileBytes + img_chunk_off + (size_t)e * 4096;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)      // i = 4 ch + j  ->  8-row group 2 ch + (j >> 1), row & 7 = g + 4 (j & 1); rows past N are zero in the image
-          hp_n[i] = kk < my_tiles ? __uint_as_float(__ldcg(reinterpret_cast<const uint32_t *>(src + ((i >> 2) * 2 + ((i & 3) >> 1)) * 1024 + img_lane_off[i & 1]))) : 0.f;
-      }
-      const bool okl = kk < my_tiles && nw + lane < N;
-      ip0_n = okl ? __ldcg(indptr + nw + lane) : 0;
-      ip1_n = okl ? __ldcg(indptr + nw + lane + 1) : 0;
-    };
-    prefetch(0);
-    for (int k = 0; k < my_tiles; ++k) {
-      const int tile = group + k * num_groups;
-      const int buf = k & 1, buse = k >> 1;
-      const int64_t node_w = (int64_t)tile * kTileM + e * 32;          // first of this warp's 32 nodes
-      if (tr) trace_stamp(tron, k, 7);
-      float hp[8], deg[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) hp[i] = hp_n[i];
-      if constexpr (HIMG) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const uint32_t mine = __float_as_uint(hp[i]), other = __shfl_xor_sync(0xffffffffu, mine, 1);
-          const uint32_t w_hi = (c & 1) ? other : mine, w_lo = (c & 1) ? mine : other;      // (col pair) hi word, lo word
-          hp[i] = (c & 1) ? __uint_as_float(w_hi & 0xffff0000u) + __uint_as_float(w_lo & 0xffff0000u)
-                          : __uint_as_float(w_hi << 16) + __uint_as_float(w_lo << 16);
-        }
-      }
-      {
-        const float dl = (float)(ip1_n - ip0_n);           // in-degree of node node_w + lane
-#pragma unroll
-        for (int i = 0; i < 8; ++i) deg[i] = __shfl_sync(0xffffffffu, dl, (i >> 2) * 16 + g + 4 * (i & 3));
-      }
-      prefetch(k + 1);
-      WAIT(acc_full(buf), buse & 1);
-      tc_fence_after();
-      if (tr) trace_stamp(tron, k, 8);
-      float v0[16], v1[16];
-      const uint32_t taddr = lane_addr + (uint32_t)(kAccCol + buf * 128 + e * 32);
-      tmem_ld16(taddr, v0);
-      tmem_ld16(taddr + 16, v1);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                              // this warp has read its part of the accumulator buffer
-        if (PAIR && !leader) mbar_arrive_cluster(mapa_rank(acc_empty(buf), 0));
-        else mbar_arrive(acc_empty(buf));
-      }
-      if (tr) trace_stamp(tron, k, 9);
-      // Addresses: every output of this thread is (per-tile base) + (compile-time offset): node = node_w + 16 ch + g + 4 j, so
-      // row-major planes move by (16 ch + 4 j) rows, and inside the image the 8-row group index is 4 e + 2 ch + (j >> 1) while
-      // row & 7 = g + 4 (j & 1) selects one of two swizzle offsets computed once per kernel (img_lane_off).
-      const int rows_left = (int)min((int64_t)N - node_w - g, (int64_t)64);      // node node_w + g + d is a real row iff d < rows_left
-      float *const ho = h_out ? h_out + (node_w + g) * kD + gcol : nullptr;
-      float *const gp0 = GATES == 1 ? gates + (node_w + g) * kD + gcol : nullptr;
-      uint2 *const gpk = GATES == 2 ? gates_packed + (node_w + g) * kD + gcol : nullptr;
-      uint8_t *const ip = h_out_img ? h_out_img + (size_t)tile * kImageTileBytes + img_chunk_off + (size_t)e * 4096 : nullptr;
-      // (one code path: a separate predicate-free body for full tiles was faster in isolation, 48 vs 53 us, but pushed the kernel
-      // past the instruction cache — 43 KB of SASS — and lost in the real step, 54.7 vs 53.5 us: profiles/r02j)
-      {
-#pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          // thread (g, c) holds pre-activation g of column c for nodes 0..15 of the chunk -> X[g][node][c]
-#pragma unroll
-          for (int i = 0; i < 16; ++i) X[g * kXGateLd + i * 8 + c] = ch == 0 ? v0[i] : v1[i];
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int i = g + 4 * j;                                     // node of the chunk finished by this thread
-            const bool valid = ch * 16 + 4 * j < rows_left;
-            const float dg = deg[ch * 4 + j];
-            const float gin = X[0 * kXGateLd + i * 8 + c] + fmaf(dg, d_gin, b_gin);
-            const float r = fast_sigmoid(X[1 * kXGateLd + i * 8 + c] + fmaf(dg, d_r, b_r));
-            const float z = fast_sigmoid(X[2 * kXGateLd + i * 8 + c] + fmaf(dg, d_z, b_z));
-            const float ghn = X[3 * kXGateLd + i * 8 + c] + b_ghn;
-            const float n = fast_tanh(fmaf(r, ghn, gin));
-            const float hnew = valid ? fmaf(z, hp[ch * 4 + j] - n, n) : 0.f;   // rows past N stay zero in the image
-            const int row_off = (ch * 16 + 4 * j) * kD;
-            // every store is predicated, not branched (common.cuh): the four element bodies of a chunk stay one basic block
-            st_f32_hint_if(valid && ho != nullptr, ho + row_off, hnew, pol_next);
-            if constexpr (GATES == 2)       // the four saved gate values of an element as ONE 8-byte store (tc_common.cuh: pack_gates)
-              st_u2_hint_if(valid, gpk + row_off, pack_gates(r, z, n, ghn), pol_gates);
-            if constexpr (GATES == 1) {
-              st_f32_hint_if(valid, gp0 + row_off, r, pol_gates);
-              st_f32_hint_if(valid, gp0 + plane + row_off, z, pol_gates);
-              st_f32_hint_if(valid, gp0 + 2 * plane + row_off, n, pol_gates);
-              st_f32_hint_if(valid, gp0 + 3 * plane + row_off, ghn, pol_gates);
-            }
-            {
-              // image word: columns (c, c+1), c even: the even lane writes the hi word, the odd lane the lo word
-              const float other = __shfl_xor_sync(0xffffffffu, hnew, 1);
-              const float x0 = (c & 1) ? other : hnew, x1 = (c & 1) ? hnew : other;
-              // one cvt.rn.bf16x2.f32 per word: hi = bf16(x), lo = bf16(x - hi) — the same values split_bf16 produces
-              const __nv_bfloat162 hi2 = __floats2bfloat162_rn(x0, x1);
-              const uint32_t hw = *reinterpret_cast<const uint32_t *>(&hi2);
-              const __nv_bfloat162 lo2 = __floats2bfloat162_rn(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xffff0000u));
-              const uint32_t word = (c & 1) ? *reinterpret_cast<const uint32_t *>(&lo2) : hw;
-              st_u32_hint_if(ip != nullptr, ip + (ch * 2 + (j >> 1)) * 1024 + img_lane_off[j & 1], word, pol_next);
-            }
-          }
-          __syncwarp();
-        }
-      }
-      if (tr) trace_stamp(tron, k, 10);
-    }
+    return;
   }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all();      // neither CTA frees tensor memory (or exits) while the pair's MMAs may still touch it
-  else __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_pair(tmem_base, 512);
-    else tmem_dealloc(tmem_base, 512);
+
+  // ===== consumers: warpgroup wg owns nodes 64 wg .. 64 wg + 63 of every tile =====
+  float *sbias = reinterpret_cast<float *>(smem + kOffBias);
+  for (int i = threadIdx.x; i < kBiasSlice; i += 32 * kConsumerWarps)
+    sbias[i] = __ldcg(reinterpret_cast<const float *>(packed + kPackedWBytes) + slice * kBiasSlice + i);
+  asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory");
+  pdl_wait();
+  if (my_tiles == 0) return;
+  const int wg = warp >> 2;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // fragment rows row0 and row0 + 8 of the tile
+  const int c4 = 2 * (lane & 3);                               // fragment columns 8 j + c4, 8 j + c4 + 1
+  const size_t plane = (size_t)N * kD;
+  const uint64_t pol_gates = l2_policy((hints & 1) ? 1 : 0);      // the saved gates are next read in the backward pass
+  const uint64_t pol_next = l2_policy((hints & 16) ? 2 : 0);      // h' and its image feed the next two kernels
+  mbar_wait_bounded(w_full, 0);
+  const bool tr = (warp == 0 && lane == 0);
+
+  for (int k = 0; k < my_tiles; ++k) {
+    const int tile = group + k * num_groups;
+    float acc_s[48], acc_h[48];
+    if (tr) { trace_stamp(tron, k, 7); trace_stamp(tron, k, 3); }
+    mbar_wait_bounded(full(0), k & 1);
+    if (tr) trace_stamp(tron, k, 4);
+    wgmma_fence();
+#pragma unroll
+    for (int p = 0; p < 2; ++p) {
+      if (p == 1) {
+        mbar_wait_bounded(full(1), k & 1);
+        if (tr) trace_stamp(tron, k, 5);
+      }
+      const uint32_t a0 = sbase + kOffStage + p * kStageBytes + wg * 8192;      // this warpgroup's 64 rows of each chunk
+      const uint32_t w0 = sbase + p * 4 * kWChunkBytes;
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb) {
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4) {
+          const uint64_t a_hi = gmma_desc(a0 + kb * kChunkBytes + k4 * 32), a_lo = gmma_desc(a0 + (2 + kb) * kChunkBytes + k4 * 32);
+          const uint64_t b_hi = gmma_desc(w0 + kb * kWChunkBytes + k4 * 32), b_lo = gmma_desc(w0 + (2 + kb) * kWChunkBytes + k4 * 32);
+          const uint32_t acc = (kb == 0 && k4 == 0) ? 0u : 1u;
+          if (p == 0) {
+            wgmma_n96<0, 0>(acc_s, a_hi, b_hi, acc);
+            wgmma_n96<0, 0>(acc_s, a_hi, b_lo, 1u);
+            wgmma_n96<0, 0>(acc_s, a_lo, b_hi, 1u);
+          } else {
+            wgmma_n96<0, 0>(acc_h, a_hi, b_hi, acc);
+            wgmma_n96<0, 0>(acc_h, a_hi, b_lo, 1u);
+            wgmma_n96<0, 0>(acc_h, a_lo, b_hi, 1u);
+          }
+        }
+      }
+      wgmma_commit();
+    }
+    // operands of the epilogue, requested while the MMAs run: in-degree and h of this thread's 2 rows x 8 columns
+    float deg[2], hp[2][8];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
+      const bool valid = node < N;
+      deg[hh] = valid ? (float)(__ldcg(indptr + node + 1) - __ldcg(indptr + node)) : 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int gcol = slice * kSliceCols + 8 * j + c4;
+        if constexpr (HIMG) {      // h = hi + lo of the image (rows past N are zero there)
+          const uint32_t whi = __ldcg(reinterpret_cast<const uint32_t *>(h_img + image_offset(node, gcol, 0)));
+          const uint32_t wlo = __ldcg(reinterpret_cast<const uint32_t *>(h_img + image_offset(node, gcol, 1)));
+          hp[hh][2 * j] = __uint_as_float(whi << 16) + __uint_as_float(wlo << 16);
+          hp[hh][2 * j + 1] = __uint_as_float(whi & 0xffff0000u) + __uint_as_float(wlo & 0xffff0000u);
+        } else {
+          const float2 v = valid ? __ldcg(reinterpret_cast<const float2 *>(h + node * kD + gcol)) : make_float2(0.f, 0.f);
+          hp[hh][2 * j] = v.x;
+          hp[hh][2 * j + 1] = v.y;
+        }
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc_s);
+    wgmma_fence_regs(acc_h);
+    if (tr) { trace_stamp(tron, k, 6); trace_stamp(tron, k, 8); }
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(empty(0)); mbar_arrive(empty(1)); }     // this warp's MMAs have read both stages
+    if (tr) trace_stamp(tron, k, 9);
+
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
+      const bool valid = node < N;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int c = 8 * j + c4, gcol = slice * kSliceCols + c;
+        float hn[2], rr[2], zz[2], nn[2], gg[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int i = 2 * hh + e;
+          const float dg = deg[hh];
+          const float gin = acc_s[4 * (8 + j) + i] + fmaf(dg, sbias[4 * kSliceCols + c + e], sbias[c + e]);
+          const float r = fast_sigmoid(acc_s[4 * j + i] + acc_h[4 * j + i] + fmaf(dg, sbias[5 * kSliceCols + c + e], sbias[kSliceCols + c + e]));
+          const float z = fast_sigmoid(acc_s[4 * (4 + j) + i] + acc_h[4 * (4 + j) + i] +
+                                       fmaf(dg, sbias[6 * kSliceCols + c + e], sbias[2 * kSliceCols + c + e]));
+          const float ghn = acc_h[4 * (8 + j) + i] + sbias[3 * kSliceCols + c + e];
+          const float n = fast_tanh(fmaf(r, ghn, gin));
+          hn[e] = valid ? fmaf(z, hp[hh][2 * j + e] - n, n) : 0.f;      // rows past N stay zero in the image
+          rr[e] = r; zz[e] = z; nn[e] = n; gg[e] = ghn;
+        }
+        const size_t off = (size_t)node * kD + gcol;
+        if (valid && h_out != nullptr) st_f2_hint(h_out + off, make_float2(hn[0], hn[1]), pol_next);
+        if constexpr (GATES == 2) {
+          if (valid) {
+            const uint2 g0 = pack_gates(rr[0], zz[0], nn[0], gg[0]), g1 = pack_gates(rr[1], zz[1], nn[1], gg[1]);
+            st_u4_hint(gates_packed + off, make_uint4(g0.x, g0.y, g1.x, g1.y), pol_gates);
+          }
+        }
+        if constexpr (GATES == 1) {
+          if (valid) {
+            st_f2_hint(gates + off, make_float2(rr[0], rr[1]), pol_gates);
+            st_f2_hint(gates + plane + off, make_float2(zz[0], zz[1]), pol_gates);
+            st_f2_hint(gates + 2 * plane + off, make_float2(nn[0], nn[1]), pol_gates);
+            st_f2_hint(gates + 3 * plane + off, make_float2(gg[0], gg[1]), pol_gates);
+          }
+        }
+        if (h_out_img != nullptr) {      // hi = bf16(x), lo = bf16(x - hi): the values split_bf16 produces
+          const uint32_t hw = bf16x2_bits(hn[0], hn[1]);
+          const uint32_t lw = bf16x2_bits(hn[0] - __uint_as_float(hw << 16), hn[1] - __uint_as_float(hw & 0xffff0000u));
+          st_u32_hint(h_out_img + image_offset(node, gcol, 0), hw, pol_next);
+          st_u32_hint(h_out_img + image_offset(node, gcol, 1), lw, pol_next);
+        }
+      }
+    }
+    if (tr) trace_stamp(tron, k, 10);
   }
 }
 
@@ -432,7 +256,7 @@ size_t gru_tc3_packed_bytes() { return tc3::kPackedBytes; }
 
 int gru_tc3_prepare(const float *w_fold, const float *b_fold, const float *b_ih, const float *w_hh, const float *b_hh, void *packed,
                     cudaStream_t stream) {
-  const int total = tc3::kSlices * tc3::kChunks * 128;
+  const int total = tc3::kSlices * 2 * tc3::kRowsPerPart * 16;
   tc3::pack_kernel<<<(total + 127) / 128, 128, 0, stream>>>(w_fold, w_hh, b_fold, b_ih, b_hh, static_cast<uint8_t *>(packed));
   DDFA_CHECK_LAUNCH("tc3::pack_kernel");
   chain_break();
@@ -452,20 +276,14 @@ int gru_tc3_step_fwd(const void *s_img, const void *h_img, const float *h, const
     set_error("tcgen05 engine (fwd): fp32 gate planes go with the fp32 h operand (legacy form)");
     return DDFA_ERR_INVALID_ARG;
   }
-  // CTA-pair form (DDFA_TUNE_FWD_PAIR): needs an even number of CTAs per tile group, which kSlices = 4 gives
-  const bool pair = fwd_pair() != 0;
-#define DDFA_FWD3_LAUNCH_P(HIMG, GATES, PAIR)                                                                                              \
-  do {                                                                                                                                     \
-    DDFA_CUDA(cudaFuncSetAttribute(tc3::gru_fwd3_kernel<HIMG, GATES, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc3::kSmemAlloc)); \
-    DDFA_CUDA(launch_chain_cluster(2, PAIR ? 2 : 1, tc3::gru_fwd3_kernel<HIMG, GATES, PAIR>, dim3(groups * tc3::kSlices), dim3(tc3::kThreads), \
-                                   tc3::kSmemAlloc, stream, static_cast<const uint8_t *>(s_img), static_cast<const uint8_t *>(h_img), h, indptr, \
-                                   static_cast<const uint8_t *>(packed), N, h_out, static_cast<uint8_t *>(h_out_img), save_gates,        \
-                                   static_cast<uint2 *>(save_gates_packed), l2_hints()));                                                \
-  } while (0)
-#define DDFA_FWD3_LAUNCH(HIMG, GATES)                \
-  do {                                               \
-    if (pair) DDFA_FWD3_LAUNCH_P(HIMG, GATES, true); \
-    else DDFA_FWD3_LAUNCH_P(HIMG, GATES, false);     \
+  if (tiles == 0) return DDFA_OK;
+#define DDFA_FWD3_LAUNCH(HIMG, GATES)                                                                                                     \
+  do {                                                                                                                                   \
+    DDFA_CUDA(cudaFuncSetAttribute(tc3::gru_fwd3_kernel<HIMG, GATES>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc3::kSmemAlloc));     \
+    DDFA_CUDA(launch_chain(2, tc3::gru_fwd3_kernel<HIMG, GATES>, dim3(groups * tc3::kSlices), dim3(tc3::kThreads), tc3::kSmemAlloc,        \
+                           stream, static_cast<const uint8_t *>(s_img), static_cast<const uint8_t *>(h_img), h, indptr,                   \
+                           static_cast<const uint8_t *>(packed), N, h_out, static_cast<uint8_t *>(h_out_img), save_gates,                \
+                           static_cast<uint2 *>(save_gates_packed), l2_hints()));                                                        \
   } while (0)
   if (h) {
     if (save_gates) DDFA_FWD3_LAUNCH(false, 1);
@@ -476,7 +294,6 @@ int gru_tc3_step_fwd(const void *s_img, const void *h_img, const float *h, const
     else DDFA_FWD3_LAUNCH(true, 0);
   }
 #undef DDFA_FWD3_LAUNCH
-#undef DDFA_FWD3_LAUNCH_P
   DDFA_CHECK_LAUNCH("tc3::gru_fwd3_kernel");
   return DDFA_OK;
 }

@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(int M, int N, int K, float a
   }
 }
 
-// Small problems (weight folding, MLP head forward / backward: M, N <= a few hundred) would occupy 1-6 of the 148 SMs with the
+// Small problems (weight folding, MLP head forward / backward: M, N <= a few hundred) would occupy 1-6 of the 132 SMs with the
 // 128x128 tile and run for tens of microseconds; this kernel uses 32x32 output tiles so the same work spreads over dozens of
 // CTAs.  64 threads, 4x4 outputs per thread (16 FFMA per two LDS.128 — the 2x2 form of round 1 was bound by its shared-memory
 // loads), K staged 32 at a time through shared memory with the next stage prefetched into registers.
@@ -250,8 +250,8 @@ int sgemm(int ta, int tb, int M, int N, int K, float alpha, const float *A, int 
     // is a chain of K/32 load latencies on a handful of SMs: slice K over gridDim.z and accumulate with RED.ADD instead.
     int split = 1;
     const int tiles = (int)(grid.x * grid.y);
-    if (beta == 1.f && K >= 256 && tiles < 148) {
-      split = (2 * 148 + tiles - 1) / tiles;
+    if (beta == 1.f && K >= 256 && tiles < kNumSMs) {
+      split = (2 * kNumSMs + tiles - 1) / tiles;
       if (split > K / 64) split = K / 64;
       if (split < 1) split = 1;
     }

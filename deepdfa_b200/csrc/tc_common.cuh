@@ -1,10 +1,10 @@
-// Shared device helpers for the tcgen05 kernels: mbarrier, TMA bulk copy, UMMA descriptors, TMEM access,
+// Shared device helpers for the tensor-core engine: mbarrier, TMA bulk copy, wgmma descriptors and instructions,
 // the bf16 hi/lo operand split and the "activation image" layout.
 //
-// Activation image (tcgen05 engine only): an [N,128] fp32 matrix X is also kept as MMA-ready operands:
+// Activation image (tensor-core engine only): an [N,128] fp32 matrix X is also kept as MMA-ready operands:
 //   image[tile = node/128][variant v: 0 = hi, 1 = lo][kblock kb: cols 0-63 | 64-127] = one 16 KB chunk,
 //   chunk = [128 rows x 64 bf16], rows 128 B apart, 16-byte units XOR-swizzled by (row & 7)
-//   (the UMMA canonical K-major SWIZZLE_128B layout; read as "MN-major" it is the [col][node] operand of the
+//   (the wgmma canonical K-major SWIZZLE_128B layout; read as "MN-major" it is the [col][node] operand of the
 //   weight-gradient GEMM).  hi = bf16(x), lo = bf16(x - hi).  Rows past N are zero.  64 KB per 128-node tile —
 //   exactly the bytes of the fp32 matrix — so producer kernels write it instead of / next to fp32 and the GEMM
 //   kernels stream it with plain 1-D TMA bulk copies (no in-kernel conversion pass).
@@ -77,101 +77,63 @@ __device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void *src, uin
                "l"(src), "r"(bytes), "r"(bar), "l"(pol)
                : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+// ---- warpgroup MMA (sm_90a wgmma) ------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor: start >> 4 in bits 0-13, leading byte offset >> 4 in 16-29, stride byte offset >> 4 in 32-45,
+// layout in 62-63 (1 = SWIZZLE_128B).  Every operand here is a stack of 128-byte rows in 1024-byte groups of eight (SBO = 1024).
+//   K-major (A or B, no transpose): rows = M or N, 64 bf16 of K per row; LBO is unused for swizzled K-major layouts.  A K step of
+//     16 advances the start address by 32 bytes inside the swizzle atom.
+//   MN-major (transposed): rows = K, 64 consecutive M / N elements per row; LBO = byte distance to the next 64 M / N elements.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes = 16u) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols));
-}
-
-// Instruction descriptor, kind::f16: D = f32, A = B = bf16, M = 128; N and operand majors as given.
-__host__ __device__ constexpr uint32_t make_idesc(int n, bool a_mn_major = false, bool b_mn_major = false) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor: start>>4 | LBO=1 | SBO = 1024 B | version 1 | layout 2
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-// MN-major SWIZZLE_128B descriptor: LBO = byte stride between 64-element MN blocks, SBO = 1024 B between 8-row K groups
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with the A operand read from tensor memory: A = [128 lanes = rows of the M dimension][K, two bf16 per 32-bit column]
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma_wait()
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// registers -> tensor memory: this thread's lane, 16 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// Accumulator fragment of an m64nN wgmma: thread t of the warpgroup holds element d[4 j + 2 h + e] =
+// D[16 (t / 32) + (t % 32) / 4 + 8 h][8 j + 2 (t % 4) + e]   (h, e in {0, 1}, j < N / 8).
 
-// ---- CTA pairs (cta_group::2): two CTAs of a 2-cluster issue ONE MMA with M = 256 — each CTA's tensor memory holds its own 128
-// rows of A and of D, the B operand (N x K) is split by rows of N between the two CTAs' shared memories (same offsets), the leader
-// (cluster rank 0) issues, and tcgen05.commit multicasts the completion to mbarriers of both CTAs ------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// D[64 x 64] (+)= A[64 x 16] * B[16 x 64], bf16 operands from shared memory, fp32 accumulator in registers
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void cluster_sync_all() {      // every thread of every CTA of the cluster
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+
+// D[64 x 96] (+)= A[64 x 16] * B[16 x 96], bf16 operands from shared memory, fp32 accumulator in registers
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n96(float (&d)[48], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
 }
-// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
+
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], bf16 operands from shared memory, fp32 accumulator in registers
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {      // arrive on an mbarrier of another CTA of the cluster
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// cta-scope wait, bounded like the one below (used by every role of a pair-form kernel)
-__device__ __forceinline__ void mbar_wait_trap(uint32_t bar, uint32_t parity) {
-  for (uint32_t it = 0; it < (1u << 26); ++it) {
+
+// wait bounded in time: a protocol error ends the kernel with a trap instead of hanging the device
+__device__ __forceinline__ void mbar_wait_bounded(uint32_t bar, uint32_t parity) {
+  for (uint32_t it = 0; it < (1u << 24); ++it) {
     uint32_t done;
     asm volatile(
         "{\n"
@@ -186,50 +148,7 @@ __device__ __forceinline__ void mbar_wait_trap(uint32_t bar, uint32_t parity) {
   }
   __trap();
 }
-// wait with cluster-scope acquire (the arrivals come from the peer CTA); bounded: a protocol error traps instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  for (uint32_t it = 0; it < (1u << 26); ++it) {
-    uint32_t done;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (done) return;
-  }
-  __trap();
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t smem_dst, uint32_t cols) {      // one warp of EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols));
-}
-// D[tmem, 256 rows over the pair] (+)= A[tmem of each CTA] * B[shared memory of both CTAs]; issued by one thread of the leader CTA
-__device__ __forceinline__ void umma_f16_ts_pair(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0)
-      : "memory");
-}
-// completion of all MMAs issued so far -> one arrival on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(cta_mask)
-               : "memory");
-}
-// instruction descriptor with M = 256 (cta_group::2)
-__host__ __device__ constexpr uint32_t make_idesc_m256(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((256u >> 4) << 24);
-}
+
 
 // byte offset of element (row, k) inside a [rows x 64] bf16 K-major SWIZZLE_128B chunk
 __host__ __device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
@@ -316,7 +235,7 @@ __device__ __forceinline__ float fast_tanh(float x) {
 
 // ---- pipeline timeline (development aid; ddfa_debug_set key 2 switches it on, ddfa_debug_read fetches it) -----------
 // Each translation unit that includes this header gets its own buffer: [CTA][tile][event] SM-clock stamps.
-constexpr int kTraceCtas = 148, kTraceTiles = 12, kTraceEvents = 12;
+constexpr int kTraceCtas = 132, kTraceTiles = 12, kTraceEvents = 12;
 constexpr size_t kTraceWords = (size_t)kTraceCtas * kTraceTiles * kTraceEvents;
 static __device__ long long g_trace[kTraceWords];
 static __device__ int g_trace_on = 0;

@@ -57,7 +57,7 @@ def _call(name, *args, tag=None):
 def _require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise DdfaError("deepdfa_b200 runs on CUDA (sm_100a) only: got a CPU tensor; there is no CPU fallback")
+            raise DdfaError("deepdfa_b200 runs on CUDA (sm_90a) only: got a CPU tensor; there is no CPU fallback")
 
 
 # ------------------------------------------------------------------------------------------

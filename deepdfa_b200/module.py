@@ -12,7 +12,7 @@ reference's ``state_dict`` names and shapes, so a reference checkpoint loads unc
     pooling.gate_nn.{weight [1,2D], bias [1]}
     output_layer.{0,2,4,...}.{weight, bias}
 
-All arithmetic runs in libddfa_b200.so (hand-written sm_100a kernels) through the C ABI; the
+All arithmetic runs in libddfa_b200.so (hand-written sm_90a kernels) through the C ABI; the
 torch modules below are parameter containers only and raise if called.  No CPU / DGL / PyTorch
 compute fallback exists: a CPU graph is moved to the module's CUDA device, a CPU module raises.
 """
@@ -179,7 +179,7 @@ class FlowGNNGGNNModule(nn.Module):
             self.register_buffer("_node_gate_b", torch.zeros(1), persistent=False)
         else:
             raise NotImplementedError(
-                f"label_style={label_style!r}: the 'graph' (shipped) and 'node' styles are implemented on the B200 path; the "
+                f"label_style={label_style!r}: the 'graph' (shipped) and 'node' styles are implemented on the CUDA path; the "
                 "dataflow_solution_* styles (reference base_module.py:88-91) are not")
 
         self._num_layers = 0
@@ -234,7 +234,7 @@ class FlowGNNGGNNModule(nn.Module):
     def _prepare(self, graph):
         dev = self.device
         if dev.type != "cuda":
-            raise DdfaError("FlowGNNGGNNModule (deepdfa_b200) must live on a CUDA device (B200); move it with .cuda(). "
+            raise DdfaError("FlowGNNGGNNModule (deepdfa_b200) must live on a CUDA device (H100); move it with .cuda(). "
                             "There is no CPU fallback.")
         g = as_batched_cfg(graph)
         dg = E.prepare_graph(g, dev, need_transpose=True)
@@ -420,7 +420,7 @@ class FlowGNNGGNNModule(nn.Module):
             return loss, torch.sigmoid(out), labels.int()
 
     def configure_optimizers(self, lr=1e-3, weight_decay=1e-2):
-        """config_default.yaml:43-47 (torch.optim.Adam, coupled L2).  The fused B200 optimizer is
+        """config_default.yaml:43-47 (torch.optim.Adam, coupled L2).  The fused CUDA optimizer is
         ``deepdfa_b200.trainer.FusedTrainer``; this returns the stock optimizer for drop-in scripts."""
         return torch.optim.Adam(self.parameters(), lr=lr, weight_decay=weight_decay)
 

@@ -1,4 +1,4 @@
-"""Fused data-parallel train step for ``FlowGNNGGNNModule`` on B200.
+"""Fused data-parallel train step for ``FlowGNNGGNNModule`` on H100.
 
 One process per GPU.  Per step: forward (T x {gather, GRU}) -> readout+MLP -> labels+BCE ->
 hand-written backward -> ONE all-reduce of the flat gradient buffer (NCCL over NVLink/NVSwitch via

@@ -1,5 +1,5 @@
 /*
- * ddfa_b200.h — C ABI of libddfa_b200.so: the B200 (sm_100a) implementation of the DDFA
+ * ddfa_b200.h — C ABI of libddfa_b200.so: the H100 (sm_90a) implementation of the DDFA
  * code_gnn GGNN hot path (embedding -> T x {edge gather-sum, GRU} -> attention readout -> MLP,
  * loss, backward, Adam).
  *
@@ -40,7 +40,7 @@ typedef enum ddfa_status {
 
 /* GEMM engines for the dense GRU matmuls */
 #define DDFA_ENGINE_SIMT 0     /* fp32 FFMA reference kernels (any D % 4 == 0)              */
-#define DDFA_ENGINE_TCGEN05 1  /* tcgen05 / TMEM, bf16x3 split operands, fp32 accumulate (D == 128) */
+#define DDFA_ENGINE_TCGEN05 1  /* tensor-core engine (name kept): Hopper wgmma, bf16x3 split operands, fp32 accumulate (D == 128) */
 
 int ddfa_abi_version(void);
 const char *ddfa_last_error(void);
@@ -54,14 +54,14 @@ enum {
   DDFA_TUNE_L2_HINTS = 0,       /* bit mask of L2 eviction-priority hints, default 23 (csrc/common.cuh) */
   DDFA_TUNE_PDL_MASK = 1,       /* bit mask of kernels launched with programmatic stream serialization, default 15 */
   DDFA_TUNE_GATHER_VARIANT = 2, /* launch shape of the D = 128 edge gather (ddfa_gather_sum_variant ids), default 9 */
-  DDFA_TUNE_FWD_PAIR = 3,       /* 1: forward GRU kernel launched as 2-CTA clusters issuing tcgen05.mma.cta_group::2 (default 0) */
+  DDFA_TUNE_FWD_PAIR = 3,       /* reserved: only 0 is accepted (the CTA-pair form of the forward kernel does not exist on sm_90a) */
   DDFA_TUNE_GATE_BWD_TMA = 4,   /* gate backward: 0 register loads; 1 dh / gates / h stream through a TMA-fed shared-memory ring; 2 (default) = 1 + the folded gather's CSR scalars pipelined across iterations */
   DDFA_TUNE_GATHER_SRC_GROUPS = 5, /* image->image edge gather: row groups (of 4 rows) walked per warp with the CSR chain pipelined; 0 (default) = 1 group (2 / 4 measured neutral), or 1 / 2 / 4 */
   DDFA_TUNE__COUNT = 6
 };
 int ddfa_tuning_set(int key, int value);
 int ddfa_tuning_get(int key);
-/* development aid: in-kernel pipeline timeline of the tcgen05 kernels (SM-clock stamps per CTA / tile / event).
+/* development aid: in-kernel pipeline timeline of the tensor-core kernels (SM-clock stamps per CTA / tile / event, 132 x 12 x 12).
  * ddfa_debug_set(2, v): v = 0 off, 1 = forward + dgrad kernels, 2 = forward + wgrad kernels;
  * ddfa_debug_read(2 | 3, host, bytes): stamps of the backward (2) or forward (3) kernel's last launch;
  * ddfa_debug_read(4, host, 4): int32 count of timed-out mbarrier waits in the TMA-staged gather variants (0 when healthy). */
@@ -174,7 +174,7 @@ int ddfa_fold_weights_bwd(const float *w_msg, const float *b_msg, const float *w
  * ------------------------------------------------------------------------------------- */
 size_t ddfa_gru_step_workspace_bytes(int32_t num_nodes, int32_t dim, int engine);
 /* Once per forward (weights are constant over the T steps): engine-specific pre-packing of the
- * step's weights into `workspace` (tcgen05: bf16 hi/lo split, UMMA swizzled smem images; SIMT:
+ * step's weights into `workspace` (tcgen05: bf16 hi/lo split, SWIZZLE_128B shared-memory operand images; SIMT:
  * no-op).  The same workspace must then be passed to every ddfa_gru_step_fwd of that forward. */
 int ddfa_gru_step_prepare(const float *w_fold, const float *b_fold, const float *b_ih,
                           const float *w_hh, const float *b_hh, int32_t dim, int engine,

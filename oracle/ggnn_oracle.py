@@ -23,7 +23,7 @@ PARITY STATUS: **partially pinned**.
     graph-label rule and the loss are pinned to the reference's executing code.
   * The two **DGL** ops are restated from the pinned upstream version (``dgl<1.1.3``,
     ``environment.yml:10``; ``dgl-cu113==0.9.0`` in ``LineVul/requirements.txt``), whose
-    source is NOT vendored in ``/root/reference`` and is not installed:
+    source is NOT vendored in the reference project and is not installed:
       - ``dgl.nn.pytorch.conv.GatedGraphConv.forward`` (n_etypes == 1 fast path):
         zero-pad ``feat`` to ``out_feats``; repeat ``n_steps`` times
         ``graph.ndata['h'] = linears[0](feat)``;
@@ -233,3 +233,56 @@ def folded_step_formula(h, src, dst, w, b, w_ih, w_hh, b_ih, b_hh):
     z = torch.sigmoid(gi[:, d:2 * d] + gh[:, d:2 * d])
     nn_ = torch.tanh(gi[:, 2 * d:] + r * gh[:, 2 * d:])
     return (1 - z) * nn_ + z * h
+
+
+# ------------------------------------------------------------------------------------------------
+# Compact golden fixtures: parameters drawn from a seeded generator instead of stored, gradients as a fixed sample
+# ------------------------------------------------------------------------------------------------
+def init_stats(state):
+    """{name: (mean, std)} of each floating-point tensor of a freshly initialised state_dict: the scale seeded_state_dict
+    reproduces, so compact fixtures keep the magnitudes (and the graph-dependent signal) of the model's own initialisation."""
+    return {k: (float(v.double().mean()), float(v.double().std(unbiased=False))) for k, v in state.items()
+            if v.is_floating_point() and v.numel() > 0}
+
+
+def seeded_state_dict(shapes, seed, scale, fixed=None):
+    """Deterministic tensor values for a state_dict with the given {name: shape}: names in sorted order, each drawn uniform
+    with the (mean, std) of `scale[name]` (a constant tensor when std == 0, e.g. LayerNorm weights) from one CPU generator
+    seeded with `seed`; `fixed` entries (buffers, hand-set values) replace what was drawn for them."""
+    fixed = fixed or {}
+    gen = torch.Generator().manual_seed(int(seed))
+    out = {}
+    for k in sorted(shapes):      # every entry draws its values, so which entries are fixed does not move the others
+        shape = tuple(int(s) for s in shapes[k])
+        u = torch.rand(shape, generator=gen, dtype=torch.float64) * 2 - 1
+        mean, std = scale.get(k, (0.0, 0.0))
+        out[k] = (mean + u * (std * 3.0 ** 0.5)).float()
+        if k in fixed:
+            out[k] = fixed[k].clone()
+    return out
+
+
+def golden_state(entry):
+    """The state_dict a compact golden entry {"shapes", "seed", "scale", "fixed"} stands for (seeded_state_dict)."""
+    return seeded_state_dict(entry["shapes"], entry["seed"], entry["scale"], entry["fixed"])
+
+
+GRAD_SAMPLE = 256
+
+
+def sample_grad(grad, seed):
+    """A fixed, seeded sample of a gradient tensor: all of it up to GRAD_SAMPLE entries, else GRAD_SAMPLE flat positions,
+    with the tensor's max |value| (the scale the comparisons use)."""
+    flat = grad.detach().reshape(-1).cpu()
+    if flat.numel() <= GRAD_SAMPLE:
+        idx = torch.arange(flat.numel())
+    else:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(int(seed)))[:GRAD_SAMPLE].sort().values
+    return {"idx": idx.to(torch.int32), "values": flat[idx].clone(), "absmax": float(flat.abs().max()), "shape": tuple(grad.shape)}
+
+
+def grad_sample_error(grad, ref):
+    """max |grad - ref| over the sampled positions of a sample_grad() record, and the reference's max |value|."""
+    assert tuple(grad.shape) == tuple(ref["shape"])
+    got = grad.detach().reshape(-1).cpu()[ref["idx"].long()]
+    return float((got - ref["values"]).abs().max()), ref["absmax"]

@@ -33,9 +33,9 @@ def bench(fn, flush=None, iters=20):
 
 def main():
     peaks = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"] \
-        if os.path.exists(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else 6650.0
+        if os.path.exists(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else 3350.0
     L = lib()
-    flush = torch.zeros(128 * 1024 * 1024, device=DEV)  # 512 MB > 126 MB L2
+    flush = torch.zeros(128 * 1024 * 1024, device=DEV)  # 512 MB > 50 MB L2
     for graphs, variable in ((256, False), (1024, False), (256, True)):
         g = synth.make_batch(graphs, 150, seed=1, variable=variable)
         dg = prepare_graph(g, DEV)

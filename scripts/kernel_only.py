@@ -1,4 +1,4 @@
-"""Runs single tcgen05-engine kernels on a C0-sized batch, for `ncu -k regex:...` captures.
+"""Runs single tensor-core-engine kernels on a C0-sized batch, for `ncu -k regex:...` captures.
    python scripts/kernel_only.py fwd|bwd [graphs]
    DDFA_TRACE=1 additionally prints the in-kernel pipeline timeline (ddfa_debug_set key 2 / ddfa_debug_read)."""
 import os
@@ -12,6 +12,8 @@ from deepdfa_b200._lib import ENGINE_TCGEN05, lib
 from deepdfa_b200.engine import _p, _stream_ptr, prepare_graph
 
 DEV, D = "cuda:0", 128
+# SM clock used to turn clock64() stamps into ns: the H100 SXM maximum unless DDFA_TRACE_GHZ gives the clock of the run
+GHZ = float(os.environ.get("DDFA_TRACE_GHZ", "1.98"))
 which = sys.argv[1] if len(sys.argv) > 1 else "fwd"
 graphs = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 L = lib()
@@ -59,16 +61,16 @@ print("done", which, N)
 
 def dump_trace(key, label):
     import numpy as np
-    CT, TL, EV = 148, 12, 12
+    CT, TL, EV = 132, 12, 12
     buf = np.zeros(CT * TL * EV, dtype=np.int64)
     L.call("ddfa_debug_read", key, buf.ctypes.data, buf.nbytes)
     t = buf.reshape(CT, TL, EV).astype(np.float64)
-    ghz = 1.965
+    ghz = GHZ
     names = ["start", "prod:first copy issued", "prod:last copy issued", "mma:acc buffer free", "mma:first operand landed",
-             "mma:last operand landed", "mma:tile committed", "epi:iteration begin", "epi:accumulator ready", "epi:tmem drained",
+             "mma:last operand landed", "mma:tile committed", "epi:iteration begin", "epi:accumulator ready", "epi:stages released",
              "epi:iteration end"]
     print(f"---- {label}: per-tile timeline, ns since the CTA's kernel start (SM clock / {ghz} GHz)")
-    for cta in (0, 1, 5, 74, 147):
+    for cta in (0, 1, 5, 66, 131):
         t0 = t[cta, 0, 0]
         print(f"CTA {cta}:")
         for k in range(TL):
@@ -83,7 +85,7 @@ def dump_trace(key, label):
     print("events: " + " | ".join(f"{i + 1}={n}" for i, n in enumerate(names[1:])))
     for a, b, what in ((1, 4, "first copy issue -> landed"), (1, 2, "producer: first -> last copy issued"), (4, 5, "mma: first -> last operand landed"),
                        (5, 6, "mma: last operand -> commit issued"), (6, 8, "commit issued -> epilogue sees accumulator"),
-                       (8, 9, "epilogue: tmem drain"), (9, 10, "epilogue: after drain -> iteration end"), (7, 10, "epilogue iteration"),
+                       (8, 9, "epilogue: stage release"), (9, 10, "epilogue: after drain -> iteration end"), (7, 10, "epilogue iteration"),
                        (7, 8, "epilogue: begin -> accumulator ready (prefetch + wait)")):
         m, p90 = span(a, b)
         print(f"   {what:56s} mean {m:8.0f} ns   p90 {p90:8.0f} ns")
@@ -109,11 +111,11 @@ if os.environ.get("DDFA_TRACE"):
                N, D, _p(ds), _p(dh), _p(acc[0]), _p(acc[1]), _p(acc[2]), _p(acc[3]), _p(acc[4]), _p(ws), wsb, 2, st)
         torch.cuda.synchronize()
         import numpy as np
-        buf = np.zeros(148 * 12 * 12, dtype=np.int64)
+        buf = np.zeros(132 * 12 * 12, dtype=np.int64)
         L.call("ddfa_debug_read", 2, buf.ctypes.data, buf.nbytes)
-        t = buf.reshape(148, 12, 12).astype(np.float64) / 1.965
-        print("---- wgrad_kernel (role 0 CTAs): ns since kernel start: B issue | A2 issue | B landed | A0 landed | A2 landed | tile MMAs issued")
-        for cta in (0, 1, 40, 73):
+        t = buf.reshape(132, 12, 12).astype(np.float64) / GHZ
+        print("---- wgrad_kernel (gate block 0 of dW'): ns since kernel start: B issue | A issue | B landed | A landed | A landed | tile MMAs issued")
+        for cta in (0, 1, 11, 21):
             t0 = t[cta, 0, 0]
             print(f"CTA {cta}: epilogue begins {t[cta, 0, 8] - t0:.0f}, ends {t[cta, 0, 10] - t0:.0f}")
             for k in range(12):

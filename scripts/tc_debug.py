@@ -1,5 +1,5 @@
-"""GPU diagnostic for the tcgen05 GRU-step kernel: structured inputs that expose descriptor / swizzle /
-TMEM-layout mistakes (gh_n is a raw accumulator + bias, so with Whh_n = I it must reproduce h exactly),
+"""GPU diagnostic for the tensor-core GRU-step kernel: structured inputs that expose descriptor / swizzle /
+fragment-layout mistakes (gh_n is a raw accumulator + bias, so with Whh_n = I it must reproduce h exactly),
 then a random case against the fp64 formula.  Run under `timeout`; prints a compact error map."""
 import sys
 import os

@@ -14,8 +14,11 @@ fixture therefore pins, against the reference's own executing code: parameter co
 feature-key and embedding order, the concatenations, where pooling and the MLP sit, `.squeeze()`, `encoder_mode`, the
 graph-label rule (`dgl.unbatch` + max of `_VULN`), `BCEWithLogitsLoss(pos_weight)` and the training-step loss.
 
-Run in the build container (needs /root/reference):   python tests/golden/make_reference_ctrlflow_golden.py
-Writes tests/golden/reference_ctrlflow_golden.pt; tests/test_oracle.py::test_oracle_matches_reference_control_flow reads it.
+Run with a checkout of the reference project:   python tests/golden/make_reference_ctrlflow_golden.py <reference root>
+Writes tests/golden/reference_ctrlflow_golden.pt, read by tests/test_host.py and tests/test_parity_gpu.py.  To keep the file small the
+parameters are not stored: oracle.ggnn_oracle.seeded_state_dict draws them from a stored seed at the per-tensor mean / std of the
+reference's own initialisation (buffers stored as they are),
+and each parameter gradient is kept as a fixed, seeded sample (oracle.ggnn_oracle.sample_grad).
 """
 import inspect
 import os
@@ -27,7 +30,6 @@ from torch import nn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REFERENCE = "/root/reference/DDFA"
 
 from deepdfa_b200 import batched_graph as BG  # noqa: E402
 from deepdfa_b200 import synth  # noqa: E402
@@ -111,9 +113,9 @@ def install_stand_ins():
     sys.modules.update(mods)
 
 
-def main():
+def main(reference_root):
     install_stand_ins()
-    sys.path.insert(0, REFERENCE)
+    sys.path.insert(0, os.path.join(reference_root, "DDFA"))
     from code_gnn.models.flow_gnn.ggnn import FlowGNNGGNNModule as RefModule      # the real reference class
 
     feat = "_ABS_DATAFLOW_datatype_all_limitall_1000_limitsubkeys_1000"
@@ -148,10 +150,16 @@ def main():
         ref = RefModule(**spec["ctor"])
         with torch.no_grad():
             ref.ggnn.linears[0].bias.uniform_(-0.1, 0.1)             # DGL zero-initialises it; make the bias path visible
+        sd = ref.state_dict()
+        params = dict(ref.named_parameters())
+        # seeded values at the scale of the reference's own initialisation (per-tensor mean / std)
+        state = {"shapes": {k: tuple(v.shape) for k, v in sd.items()}, "seed": 1000 + i, "scale": O.init_stats(sd),
+                 "fixed": {k: v.clone() for k, v in sd.items() if k not in params}}
+        ref.load_state_dict(O.golden_state(state))
         g = synth.make_batch(**spec["graphs"])
         if not spec["ctor"].get("concat_all_absdf"):
             g.ndata["_ABS_DATAFLOW"] = g.ndata["_ABS_DATAFLOW_datatype"] % spec["ctor"]["input_dim"]
-        case = {"name": spec["name"], "ctor": spec["ctor"], "state_dict": {k: v.clone() for k, v in ref.state_dict().items()},
+        case = {"name": spec["name"], "ctor": spec["ctor"], "state": state,
                 "graph": {"src": g.edges()[0], "dst": g.edges()[1], "batch_num_nodes": g.batch_num_nodes(), "ndata": dict(g.ndata)}}
         ref.eval()
         with torch.no_grad():
@@ -165,7 +173,7 @@ def main():
             loss = ref.training_step((g, {}), 0)
             loss.backward()
             case["train_loss"] = loss.detach().clone()
-            case["grads"] = {k: p.grad.clone() for k, p in ref.named_parameters() if p.grad is not None}
+            case["grads"] = {k: O.sample_grad(p.grad, 7 * i + j) for j, (k, p) in enumerate(ref.named_parameters()) if p.grad is not None}
         cases.append(case)
     out = os.path.join(ROOT, "tests", "golden", "reference_ctrlflow_golden.pt")
     torch.save({"cases": cases, "note": "outputs of the reference's own ggnn.py / base_module.py code; DGL ops bound to the oracle restatements"}, out)
@@ -173,4 +181,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

@@ -1,6 +1,6 @@
 """Pins deepdfa_b200/bigvul_io.py against the reference's own data-loading code — by running that code.
 
-Runs, from /root/reference/DDFA, on the synthetic processed-dataset files of tests/bigvul_fixture.py:
+Runs, from <reference root>/DDFA (first argument), on the synthetic processed-dataset files of tests/bigvul_fixture.py:
 
     sastvd/linevd/graphmogrifier.py   get_nodes_df (:20-40), get_graphs (:59-95)      the REAL functions
     sastvd/helpers/dclass.py          BigVulDataset.get_epoch_indices (:84-105)       the REAL method (on a stand-in `self`)
@@ -28,7 +28,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-REFERENCE = "/root/reference/DDFA"
+REFERENCE = os.path.join(sys.argv[1] if len(sys.argv) > 1 else ".", "DDFA")
 
 from bigvul_fixture import FEAT, write_dataset  # noqa: E402
 from deepdfa_b200 import bigvul_io as IO  # noqa: E402

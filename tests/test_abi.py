@@ -1,4 +1,4 @@
-"""CPU: the C-ABI shared library builds for sm_100a, loads, and exports every symbol that
+"""CPU: the C-ABI shared library builds for sm_90a, loads, and exports every symbol that
 include/ddfa_b200.h declares.  No compute calls (there is no GPU here)."""
 import ctypes
 import re
@@ -40,9 +40,9 @@ def test_binding_arity_matches_header():
         assert n == len(argtypes), f"{name}: header has {n} parameters, binding has {len(argtypes)}"
 
 
-def test_library_is_sm100a_and_torch_free(libpath):
-    out = subprocess.run(["cuobjdump", "-lelf", str(libpath)], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+def test_library_is_sm90a_and_torch_free(libpath):
+    out = subprocess.run([str(build.cuda_tool("cuobjdump")), "-lelf", str(libpath)], capture_output=True, text=True).stdout
+    assert "sm_90a" in out and "sm_100" not in out
     ldd = subprocess.run(["ldd", str(libpath)], capture_output=True, text=True).stdout
     assert "libtorch" not in ldd and "libc10" not in ldd and "libpython" not in ldd     # C ABI only: no torch / Python types behind the boundary
 
@@ -56,6 +56,8 @@ def test_argument_validation_is_reported_without_a_gpu(libpath):
     with pytest.raises(_lib.DdfaError, match="ddfa_sgemm"):
         L.call("ddfa_sgemm", 0, 0, -1, 1, 1, 1.0, None, 1, None, 1, 0.0, None, 1, 1, None)
     assert L.call("ddfa_gru_step_workspace_bytes", 100, 128, 0) == 4 * 2 * 100 * 384
+    rc = L.raw("ddfa_tuning_set")(_lib.TUNE_FWD_PAIR, 1)      # reserved key: the CTA-pair forward form does not exist on sm_90a
+    assert rc == -1 and "FWD_PAIR" in L.last_error() and L.call("ddfa_tuning_get", _lib.TUNE_FWD_PAIR) == 0
 
 
 def test_header_is_plain_c_and_a_c_host_links_the_library(libpath, tmp_path):

@@ -159,8 +159,10 @@ def test_module_state_dict_matches_the_reference_classes():
     data = torch.load(os.path.join(os.path.dirname(__file__), "golden", "reference_ctrlflow_golden.pt"), weights_only=False)
     for case in data["cases"]:
         m = D.FlowGNNGGNNModule(**case["ctor"])
-        ours, ref = m.state_dict(), case["state_dict"]
+        ours, ref = m.state_dict(), case["state"]["shapes"]
         assert sorted(ours.keys()) == sorted(ref.keys()), case["name"]
         for k in ref:
-            assert ours[k].shape == ref[k].shape, (case["name"], k)
-        m.load_state_dict(ref)                      # a reference checkpoint loads as is
+            assert ours[k].shape == torch.Size(ref[k]), (case["name"], k)
+        for k, v in case["state"]["fixed"].items():     # buffers as the reference classes hold them, e.g. loss_fn.pos_weight
+            assert torch.equal(ours[k], v), (case["name"], k)
+        m.load_state_dict(O.golden_state(case["state"]))     # a reference checkpoint loads as is

@@ -21,11 +21,12 @@ def _build(data, flow, device="cpu", overlap=True):
     from transformers import RobertaConfig, RobertaForSequenceClassification
     config = RobertaConfig(**data["roberta"])
     model = LineVulCombined(RobertaForSequenceClassification(config), flow, config, overlap=overlap)
-    sd = {k: v for k, v in data["state_dict"].items() if not k.startswith(("roberta.", "flowgnn_encoder."))}
+    state = O.golden_state(data["state"])
+    sd = {k: v for k, v in state.items() if not k.startswith(("roberta.", "flowgnn_encoder."))}
     missing, unexpected = model.load_state_dict(sd, strict=False)
     # the reference class inherits an unused second RoBERTa ("roberta.*"); everything else must line up by name
     assert not unexpected and all(k.startswith("flowgnn_encoder.") for k in missing), (missing, unexpected)
-    flow.load_state_dict({k[len("flowgnn_encoder."):]: v for k, v in data["state_dict"].items() if k.startswith("flowgnn_encoder.")})
+    flow.load_state_dict({k[len("flowgnn_encoder."):]: v for k, v in state.items() if k.startswith("flowgnn_encoder.")})
     return model.to(device).eval()
 
 

@@ -496,7 +496,7 @@ def test_module_matches_reference_control_flow_goldens(engine):
         if engine == "tcgen05" and case["ctor"]["hidden_dim"] * (4 if case["ctor"].get("concat_all_absdf") else 1) != 128:
             continue                                                      # the tensor-core engine is the width-128 one
         m = D.FlowGNNGGNNModule(**case["ctor"], engine=engine)
-        m.load_state_dict(case["state_dict"])
+        m.load_state_dict(O.golden_state(case["state"]))
         m.to(DEV)
         with torch.no_grad():
             out = m(g, {})
@@ -510,10 +510,10 @@ def test_module_matches_reference_control_flow_goldens(engine):
             loss.backward()
             assert abs(float(loss) - float(case["train_loss"])) < 1e-4, case["name"]
             for k, p in m.named_parameters():
-                if k in case["grads"]:
-                    ref = case["grads"][k]
-                    tol = 2e-4 if engine == "simt" else 2e-3
-                    assert (p.grad.cpu() - ref).abs().max() < tol * max(1.0, float(ref.abs().max())), (case["name"], k)
+                if k in case["grads"]:      # a fixed, seeded sample of each reference gradient (O.sample_grad)
+                    err, absmax = O.grad_sample_error(p.grad, case["grads"][k])
+                    tol = 2e-4 if engine == "simt" else 2e-3      # relative to the gradient's largest entry (+ fp32 noise floor)
+                    assert err < tol * absmax + 1e-6, (case["name"], k, err, absmax)
             checked_grads += 1
     assert checked_grads >= 1, "no reference-code gradient case ran for this engine"
 
