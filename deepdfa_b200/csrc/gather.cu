@@ -346,7 +346,7 @@ static int launch_d128_variant(int variant, const int32_t *indptr, const int32_t
     case 8: return launch_gather<32, 1, 4, 4, 2, 1, 256>(indptr, indices, h, N, 128, out, accumulate, stream);
     case 9: return launch_gather<32, 1, 2, 4, 2, 1, 128>(indptr, indices, h, N, 128, out, accumulate, stream);
     case 10:      // gather_tma.cu: neighbour rows staged in shared memory by per-row TMA bulk copies
-    case 11:      // gather_tma.cu: ... by tensor-map tile::gather4 copies (four rows per instruction)
+    case 11:      // gather_tma.cu: ... by tensor-map tile copies (one row per copy)
       return launch_gather_tma(variant, indptr, indices, h, N, out, accumulate, stream);
     default:
       set_error("ddfa_gather_sum_variant: unknown variant %d (0..11)", variant);

@@ -12,7 +12,8 @@
 //         memory as the B operand; a CTA owns one output (ds or dh) and one column half (see the comment at the kernel)
 //   (3) wgrad_kernel            dW' += [q_r q_z q_n]^T s ;  dWhh += [q_r q_z q_nr]^T h            K = nodes
 //         both operands are read "MN-major" straight from the images (whole 128-node tiles, three 64 KB slots); a CTA keeps
-//         one [128 x 128] gate block of the fp32 sum in registers over all its tiles and writes it to a private global partial
+//         one [128 x 128] gate block of the fp32 sum in registers over all its tiles (one wgmma accumulation per tile, added to
+//         the running sum with round-to-nearest adds) and writes it to a private global partial
 //         at the end; wgrad_reduce_kernel sums the partials once per backward pass.
 // Precision: bf16x3 everywhere (hi*hi + hi*lo + lo*hi), fp32 accumulate.
 #include <cuda_fp16.h>
@@ -654,9 +655,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const uint8_t *__r
   }
 
   const int wg = warp >> 2;
-  float acc[64];
+  // acc: this tile's wgmma accumulator (restarted every tile); sum: the running sum over the CTA's tiles, in ordinary fp32 adds.
+  // Chaining all tiles inside the wgmma accumulator biased the sum toward zero by about 2e-7 per tile (the tensor core's fp32
+  // accumulation does not round to nearest): -1e-4 of dW' / dWhh at 447 tiles per CTA (C1, T = 8, tests/test_scale_gpu.py).
+  float acc[64], sum[64];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int i = 0; i < 64; ++i) acc[i] = sum[i] = 0.f;
   for (int i = 0; i < my_tiles; ++i) {
     const int cb = 2 * i, ca = 2 * i + 1;
     mbar_wait_bounded(full(cb % kWgSlots), (cb / kWgSlots) & 1);
@@ -672,17 +676,19 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const uint8_t *__r
       const uint32_t koff = (uint32_t)k16 * 2048u;      // 16 nodes = two 8-node groups of 1024 B
       const uint64_t a_hi = gmma_desc(a0 + koff, kChunkBytes), a_lo = gmma_desc(a0 + vs + koff, kChunkBytes);
       const uint64_t b_hi = gmma_desc(b0 + koff, kChunkBytes), b_lo = gmma_desc(b0 + vs + koff, kChunkBytes);
-      wgmma_n128<1, 1>(acc, a_hi, b_hi, 1u);
+      wgmma_n128<1, 1>(acc, a_hi, b_hi, k16 == 0 ? 0u : 1u);
       wgmma_n128<1, 1>(acc, a_lo, b_hi, 1u);
       wgmma_n128<1, 1>(acc, a_hi, b_lo, 1u);
     }
     wgmma_commit();
     if (warp == 0 && lane == 0) trace_stamp(tron, i, 6);
     wgmma_wait<0>();
+    wgmma_fence_regs(acc);
     __syncwarp();
     if (lane == 0) { mbar_arrive(empty(cb % kWgSlots)); mbar_arrive(empty(ca % kWgSlots)); }
+#pragma unroll
+    for (int j = 0; j < 64; ++j) sum[j] += acc[j];
   }
-  wgmma_fence_regs(acc);
   if (warp == 0 && lane == 0) trace_stamp(tron, 0, 8);
   // this CTA's private partial: rows 128 g + (fragment row), 128 columns; every CTA writes its slot (zeros if it owns no tile)
   float *dst = partial + ((size_t)role * gridDim.x + blockIdx.x) * kWgPartialFloats;
@@ -692,7 +698,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const uint8_t *__r
     float *rowp = dst + (size_t)(row0 + 8 * hh) * kD + 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
-      float2 v = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+      float2 v = make_float2(sum[4 * j + 2 * hh], sum[4 * j + 2 * hh + 1]);
       if (!first) {
         const float2 o = *reinterpret_cast<const float2 *>(rowp + 8 * j);
         v.x += o.x;
