@@ -25,10 +25,10 @@ bool chain_take_break() {
 // scripts set them through the C ABI.  They select between equivalent launch configurations of the same kernels.
 static std::atomic<int> g_tuning[DDFA_TUNE__COUNT] = {
     {23},   // DDFA_TUNE_L2_HINTS: measured best on whole-step A/Bs (profiles/r02l-m): 1 + 2 + 4 + 16
-    {15},   // DDFA_TUNE_PDL_MASK: all four chain kernels
+    {15},   // DDFA_TUNE_PDL_MASK: all chain kernels (bit 4: the backward step's first kernel, fused or not; 8: dgrad3 after gate_bwd_image)
     {9},    // DDFA_TUNE_GATHER_VARIANT: r01b sweep — 2 rows/pass, 4 loads in flight, 128-thread CTAs
     {0},    // DDFA_TUNE_FWD_PAIR: reserved, only 0 is accepted (no CTA-pair form of the forward kernel on sm_90a)
-    {2},    // DDFA_TUNE_GATE_BWD_TMA: 0 register loads; 1 TMA-staged streaming operands (packed saved state); 2 = 1 + CSR scalars pipelined
+    {2},    // DDFA_TUNE_GATE_BWD_TMA: 0 gate_bwd_image + dgrad3; 1 bwd_step_fused_kernel (packed saved state); 2 = 1 + CSR scalars pipelined
     {0},    // DDFA_TUNE_GATHER_SRC_GROUPS: image->image gather, row groups per warp (0 = default = 1; 2 / 4 selectable)
 };
 int l2_hints() { return g_tuning[DDFA_TUNE_L2_HINTS].load(std::memory_order_relaxed); }
@@ -70,7 +70,7 @@ int ddfa_tuning_get(int key) {
 
 int ddfa_debug_set(int key, int value) {
   switch (key) {
-    case 2: {   // pipeline timeline stamps of the tensor-core kernels: 0 off, 1 = gru_fwd3 + dgrad3, 2 = gru_fwd3 + wgrad
+    case 2: {   // pipeline timeline stamps of the tensor-core kernels: 0 off, 1 = gru_fwd3 + dgrad3 / bwd_step_fused, 2 = gru_fwd3 + wgrad
       int rc = ddfa::gru_tc3_trace_enable(value);
       return rc != DDFA_OK ? rc : ddfa::gru_tc2b_trace_enable(value);
     }
@@ -81,11 +81,19 @@ int ddfa_debug_set(int key, int value) {
 int ddfa_debug_read(int key, void *host_out, size_t bytes) {
   DDFA_REQUIRE(host_out != nullptr, "ddfa_debug_read: null output");
   switch (key) {   // [132 CTAs][12 tiles][12 events] int64 SM-clock stamps
-    case 2: return ddfa::gru_tc2b_trace_read(host_out, bytes);    // dgrad3_kernel / wgrad_kernel
+    case 2: return ddfa::gru_tc2b_trace_read(host_out, bytes);    // dgrad3_kernel / bwd_step_fused_kernel / wgrad_kernel
     case 3: return ddfa::gru_tc3_trace_read(host_out, bytes);     // gru_fwd3_kernel
     case 4: {                                                     // int32: bounded-wait failures of the TMA-staged gather variants
       DDFA_REQUIRE(bytes >= sizeof(int), "ddfa_debug_read: key 4 needs 4 bytes");
       const int v = ddfa::gather_tma_errors();
+      memcpy(host_out, &v, sizeof(int));
+      return DDFA_OK;
+    }
+    case 5: {                                                     // int32: 4-CTA clusters of bwd_step_fused_kernel resident at once
+      DDFA_REQUIRE(bytes >= sizeof(int), "ddfa_debug_read: key 5 needs 4 bytes");
+      int v = 0;
+      const int rc = ddfa::gru_tc2b_fused_max_clusters(&v);
+      if (rc != DDFA_OK) return rc;
       memcpy(host_out, &v, sizeof(int));
       return DDFA_OK;
     }

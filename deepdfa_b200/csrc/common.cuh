@@ -58,10 +58,11 @@ inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s
 // Both instructions are no-ops in a normal launch.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-int pdl_mask();       // abi.cu: DDFA_TUNE_PDL_MASK — bit mask of the kernels launched programmatically (1 gather_image, 2 gru_fwd3, 4 gate_bwd, 8 dgrad3)
+int pdl_mask();       // abi.cu: DDFA_TUNE_PDL_MASK — bit mask of the kernels launched programmatically (1 gather_image, 2 gru_fwd3,
+                      // 4 the head of the backward step: bwd_step_fused_kernel or gate_bwd_image_kernel, 8 dgrad3 after gate_bwd_image)
 int gather_variant(); // abi.cu: DDFA_TUNE_GATHER_VARIANT
 int gather_src_groups();   // abi.cu: DDFA_TUNE_GATHER_SRC_GROUPS — row groups per warp of the image->image gather (0 = by size)
-int gate_bwd_tma();   // abi.cu: DDFA_TUNE_GATE_BWD_TMA — TMA-staged gate backward kernel (packed saved state)
+int gate_bwd_tma();   // abi.cu: DDFA_TUNE_GATE_BWD_TMA — gate backward fused into dgrad (packed saved state)
 void chain_break();   // abi.cu: the next launch_chain() on this thread is a normal (fully serialised) launch
 bool chain_take_break();
 
@@ -120,6 +121,7 @@ int gru_tc3_trace_enable(int on);   // pipeline timeline of gru_fwd3_kernel (dev
 int gru_tc3_trace_read(void *host, size_t bytes);
 int gru_tc2b_trace_enable(int on);  // pipeline timeline of dgrad3_kernel (value 1) / wgrad_kernel (value 2) — development aid
 int gru_tc2b_trace_read(void *host, size_t bytes);
+int gru_tc2b_fused_max_clusters(int *out);   // 4-CTA clusters of bwd_step_fused_kernel resident at once on this device
 size_t gru_tc2_workspace_bytes();
 int gru_tc2_prepare(const float *w_fold, const float *b_fold, const float *b_ih, const float *w_hh, const float *b_hh,
                     void *workspace, size_t workspace_bytes, cudaStream_t stream);

@@ -10,13 +10,18 @@
 //   (2) dgrad3_kernel           ds = [q_r q_z q_n] W' ;  dh = dh' * z + [q_r q_z q_nr] Whh      K = 3D
 //         wgmma with the q image tiles as the A operand (two 64 KB stages) and 64 columns of the weights resident in shared
 //         memory as the B operand; a CTA owns one output (ds or dh) and one column half (see the comment at the kernel)
-//   (3) wgrad_kernel            dW' += [q_r q_z q_n]^T s ;  dWhh += [q_r q_z q_nr]^T h            K = nodes
+//   (1+2) bwd_step_fused_kernel  (1) and (2) in one 4-CTA cluster kernel, for the packed saved state (the default path):
+//         the gate backward of a tile on TMA-staged operands, the q images handed over through L2, and dh' * z through the
+//         rows of dh instead of a plane of its own; (1) then (2) remain the path of the fp32 saved state and the A/B reference
+//   (3) wgrad_kernel           dW' += [q_r q_z q_n]^T s ;  dWhh += [q_r q_z q_nr]^T h            K = nodes
 //         both operands are read "MN-major" straight from the images (whole 128-node tiles, three 64 KB slots); a CTA keeps
 //         one [128 x 128] gate block of the fp32 sum in registers over all its tiles (one wgmma accumulation per tile, added to
 //         the running sum with round-to-nearest adds) and writes it to a private global partial
 //         at the end; wgrad_reduce_kernel sums the partials once per backward pass.
 // Precision: bf16x3 everywhere (hi*hi + hi*lo + lo*hi), fp32 accumulate.
 #include <cuda_fp16.h>
+
+#include <atomic>
 
 #include "tc_common.cuh"
 
@@ -186,241 +191,6 @@ __global__ void __launch_bounds__(32 * kGbWarps, 2) gate_bwd_image_kernel(const 
   }
 }
 
-// -------------------------------------------------------------------------------------------------
-// (1') gate backward, TMA-staged (packed saved state).  The register-path kernel above is load-latency-bound: ncu on C1
-// (profiles/r03i) shows 170 us for 731 MB = 4.3 TB/s, DRAM 52 %, 85 % of the stall samples on long_scoreboard — 16 warps per SM
-// with ~128 bytes of streaming loads in flight per lane do not cover the loaded DRAM latency, and the register file (128 x 512)
-// admits no more.  Here the three STREAMING operands of a row block — dh (fp32), the packed gates and h (image pieces, or fp32 for
-// step 0) — are contiguous in memory, so a producer warp moves them with TMA bulk copies into a three-stage shared-memory ring
-// (3 x 64 KB in flight per SM, no registers), and 16 consumer warps read them with LDS; only the gathered ds rows of the folded
-// transposed edge gather (data-dependent addresses) remain register loads, and they hit L2 (dgrad wrote them a kernel ago).
-// One CTA per SM, block of 32 consecutive rows per stage, warp w owns rows w and w + 16 of the block, lane = 4 columns as before:
-// same arithmetic, same summation order of the gather, same outputs.
-// -------------------------------------------------------------------------------------------------
-constexpr int kGtRows = 32, kGtStages = 3, kGtConsumers = 16, kGtPre = 2;
-constexpr int kGtOffD = 0, kGtOffG = kGtRows * kD * 4, kGtOffH = kGtOffG + kGtRows * kD * 8;          // 16 KB | 32 KB | 16 KB
-constexpr int kGtStageBytes = kGtOffH + kGtRows * kD * 4;                                              // 64 KB
-constexpr int kGtOffBar = kGtStages * kGtStageBytes;
-constexpr int kGtSmem = kGtOffBar + 2 * kGtStages * 8 + 16;
-constexpr int kGtThreads = 32 * kGtConsumers;
-
-// HF32: h operand as fp32 rows (step 0: h_0 = x) or the activation image.  CSRP: the CSR scalars / neighbour ids of the folded
-// gather pipelined across iterations, one value per lane (DDFA_TUNE_GATE_BWD_TMA = 2, default; 1 = fetched inside the iteration).
-template <bool HF32, bool CSRP>
-__global__ void __launch_bounds__(kGtThreads, 1) gate_bwd_tma_kernel(const float *__restrict__ dh_out, const float *__restrict__ h,
-                                                                     const uint8_t *__restrict__ h_img_src, const uint2 *__restrict__ gates_packed,
-                                                                     const int32_t *__restrict__ indptr, const float *__restrict__ ds_in,
-                                                                     const int32_t *__restrict__ indptr_t, const int32_t *__restrict__ indices_t,
-                                                                     int32_t N, uint8_t *__restrict__ q_img, size_t img_stride,
-                                                                     float *__restrict__ dhz, float *__restrict__ db_fold, float *__restrict__ db_ih,
-                                                                     float *__restrict__ db_hh, int hints) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = sbase + kGtOffBar;
-  auto full = [&](int i) { return bar0 + 8u * i; };
-  auto empty = [&](int i) { return bar0 + 8u * (kGtStages + i); };
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t Npad = ((int64_t)N + kTileM - 1) / kTileM * kTileM;
-  const int num_blocks = (int)(Npad / kGtRows);
-  const int my_blocks = (num_blocks > (int)blockIdx.x) ? (num_blocks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kGtStages; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), kGtConsumers); }
-    mbar_fence_init();
-  }
-  __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();
-  float4 sum[7];
-#pragma unroll
-  for (int i = 0; i < 7; ++i) sum[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-
-  // the copies of block k into its stage: issued by one lane of warp 0 — ahead of the loop for the first kGtStages blocks, then
-  // each time warp 0 has finished a block (a dedicated producer warp would make 17 warps = 640 allocated threads = 96 registers;
-  // 16 warps get 128 and the kernel does not spill)
-  auto fill = [&](int k) {
-    const uint64_t pol_saved = l2_policy((hints & 2) ? 1 : 0), pol_dh = l2_policy((hints & 8) ? 1 : 0);
-    const int stage = k % kGtStages;
-    const int64_t r0 = (int64_t)(blockIdx.x + (int64_t)k * gridDim.x) * kGtRows;
-    const int valid = (int)max((int64_t)0, min((int64_t)kGtRows, (int64_t)N - r0));      // rows that exist in the [N, ...] arrays
-    const uint32_t dst = sbase + stage * kGtStageBytes;
-    const uint32_t bytes = (uint32_t)valid * (kD * 4 + kD * 8) + (HF32 ? (uint32_t)valid * kD * 4 : (uint32_t)kGtRows * kD * 4);
-    mbar_arrive_expect_tx(full(stage), bytes);
-    if (valid > 0) {
-      bulk_g2s_hint(dst + kGtOffD, dh_out + r0 * kD, (uint32_t)valid * kD * 4, full(stage), pol_dh);
-      bulk_g2s_hint(dst + kGtOffG, gates_packed + r0 * kD, (uint32_t)valid * kD * 8, full(stage), pol_saved);
-    }
-    if (HF32) {
-      if (valid > 0) bulk_g2s_hint(dst + kGtOffH, h + r0 * kD, (uint32_t)valid * kD * 4, full(stage), pol_saved);
-    } else {      // the block's 32 rows of each of the four [128 x 64] bf16 chunks: 4 KB pieces (the image is padded to whole tiles)
-      const uint8_t *tile = h_img_src + (size_t)(r0 >> 7) * kImageTileBytes + (size_t)(r0 & 127) * 128;
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) bulk_g2s_hint(dst + kGtOffH + ch * (kGtRows * 128), tile + (size_t)ch * kChunkBytes, kGtRows * 128, full(stage), pol_saved);
-    }
-  };
-  if (warp == 0 && elect_one())
-    for (int k = 0; k < kGtStages && k < my_blocks; ++k) fill(k);
-  __syncwarp();
-  {
-    // ===== consumers =====
-    const int col = lane * 4;
-    const uint64_t pol_tmp = l2_policy((hints & 4) ? 2 : 0);
-    // The CSR data of the warp's two rows — indptr (in-degree), indptr_t and the first kGtPre transposed neighbour ids — is a chain of
-    // dependent global loads (indptr_t -> indices_t -> ds row); fetched inside the iteration that uses it, the chain was 59 % of the
-    // kernel's stall samples (profiles/r03r: long_scoreboard on these lines).  It is warp-uniform, so it is kept ONE VALUE PER LANE
-    // and pipelined across iterations: lanes 0-3 hold indptr[node_r + {0,1}], lanes 4-7 indptr_t[node_r + {0,1}] (r = (lane >> 1) & 1)
-    // of a block, lanes 8-11 its ids id[r][q] (q = lane & 1); iteration k requests the scalars of block k + 2 and the ids of block
-    // k + 1 (from the scalars that arrived during iteration k - 1) and broadcasts block k's values by shuffle — only the ds rows
-    // themselves are still requested in the iteration that adds them.
-    static_assert(kGtPre == 2, "lane slots below assume two prefetched neighbours per row");
-    auto load_scalars = [&](int kk) -> int {
-      int v = 0;
-      if (kk < my_blocks && lane < 8) {
-        const int64_t nd = (int64_t)(blockIdx.x + (int64_t)kk * gridDim.x) * kGtRows + warp + 16 * ((lane >> 1) & 1);
-        const int32_t *base = lane < 4 ? indptr : indptr_t;
-        if (nd < N && base) v = __ldcg(base + nd + (lane & 1));
-      }
-      return v;
-    };
-    auto load_ids = [&](int sc) -> int {
-      const int r_ = (lane >> 1) & 1, q_ = lane & 1;
-      const int tb_ = __shfl_sync(0xffffffffu, sc, 4 + 2 * r_), te_ = __shfl_sync(0xffffffffu, sc, 5 + 2 * r_);
-      int v = -1;
-      if (lane >= 8 && lane < 12 && tb_ + q_ < te_) v = __ldcg(indices_t + tb_ + q_);
-      return v;
-    };
-    int sc_cur = 0, sc_next = 0, id_cur = -1;
-    if constexpr (CSRP) {
-      sc_cur = load_scalars(0); sc_next = load_scalars(1);
-      id_cur = load_ids(sc_cur);
-    }
-    for (int k = 0; k < my_blocks; ++k) {
-      const int stage = k % kGtStages, use = k / kGtStages;
-      const int64_t r0 = (int64_t)(blockIdx.x + (int64_t)k * gridDim.x) * kGtRows;
-      // the two rows of this warp and their CSR data
-      int64_t node[2];
-      bool ok[2];
-      int tb[2], te[2], ip0[2], ip1[2];
-      int id[2][kGtPre];      // the first kGtPre neighbours of both rows (a CFG node has ~2 in-edges); longer lists finish below
-      if constexpr (CSRP) {
-        const int sc_next2 = load_scalars(k + 2);
-        const int id_next = load_ids(sc_next);
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          node[r] = r0 + warp + 16 * r;
-          ok[r] = node[r] < N;
-          ip0[r] = __shfl_sync(0xffffffffu, sc_cur, 2 * r); ip1[r] = __shfl_sync(0xffffffffu, sc_cur, 2 * r + 1);
-          tb[r] = __shfl_sync(0xffffffffu, sc_cur, 4 + 2 * r); te[r] = __shfl_sync(0xffffffffu, sc_cur, 5 + 2 * r);
-#pragma unroll
-          for (int q = 0; q < kGtPre; ++q) id[r][q] = __shfl_sync(0xffffffffu, id_cur, 8 + 2 * r + q);
-        }
-        sc_cur = sc_next; sc_next = sc_next2; id_cur = id_next;
-      } else {      // everything requested inside the iteration (global, independent of the staged operands: before the wait)
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          node[r] = r0 + warp + 16 * r;
-          ok[r] = node[r] < N;
-          tb[r] = te[r] = ip0[r] = ip1[r] = 0;
-          if (ok[r]) {
-            ip0[r] = __ldcg(indptr + node[r]); ip1[r] = __ldcg(indptr + node[r] + 1);
-            if (indptr_t) { tb[r] = __ldcg(indptr_t + node[r]); te[r] = __ldcg(indptr_t + node[r] + 1); }
-          }
-        }
-#pragma unroll
-        for (int r = 0; r < 2; ++r)
-#pragma unroll
-          for (int q = 0; q < kGtPre; ++q) id[r][q] = (tb[r] + q < te[r]) ? __ldcg(indices_t + tb[r] + q) : -1;
-      }
-      float4 gv[2][kGtPre];
-#pragma unroll
-      for (int r = 0; r < 2; ++r)
-#pragma unroll
-        for (int q = 0; q < kGtPre; ++q) gv[r][q] = id[r][q] >= 0 ? ldg_cg_f4(ds_in + (size_t)id[r][q] * kD + col) : make_float4(0.f, 0.f, 0.f, 0.f);
-      mbar_wait(full(stage), use & 1);
-      const uint8_t *st = smem + stage * kGtStageBytes;
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = warp + 16 * r;                   // row inside the block
-        float4 d = make_float4(0.f, 0.f, 0.f, 0.f), hv = d, rr = d, zz = d, nn = d, gh = d;
-        if (ok[r]) {
-          d = *reinterpret_cast<const float4 *>(st + kGtOffD + row * (kD * 4) + col * 4);
-          const uint4 g0 = *reinterpret_cast<const uint4 *>(st + kGtOffG + row * (kD * 8) + col * 8);
-          const uint4 g1 = *reinterpret_cast<const uint4 *>(st + kGtOffG + row * (kD * 8) + col * 8 + 16);
-          unpack_gates(make_uint2(g0.x, g0.y), rr.x, zz.x, nn.x, gh.x);
-          unpack_gates(make_uint2(g0.z, g0.w), rr.y, zz.y, nn.y, gh.y);
-          unpack_gates(make_uint2(g1.x, g1.y), rr.z, zz.z, nn.z, gh.z);
-          unpack_gates(make_uint2(g1.z, g1.w), rr.w, zz.w, nn.w, gh.w);
-          if (HF32) {
-            hv = *reinterpret_cast<const float4 *>(st + kGtOffH + row * (kD * 4) + col * 4);
-          } else {      // piece [v][kb = col / 64] of 32 rows x 128 B; 16-byte units swizzled by (global row) & 7 == row & 7 (blocks start at multiples of 32)
-            const uint32_t off = (uint32_t)((col >> 6) * (kGtRows * 128) + row * 128 + (((((col & 63) >> 3) ^ (row & 7)) & 7) << 4) + (col & 7) * 2);
-            const uint2 hh = *reinterpret_cast<const uint2 *>(st + kGtOffH + off);
-            const uint2 hl = *reinterpret_cast<const uint2 *>(st + kGtOffH + 2 * (kGtRows * 128) + off);
-            const float4 a = bf16x4_to_f4(hh), b = bf16x4_to_f4(hl);
-            hv = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-          }
-#pragma unroll
-          for (int q = 0; q < kGtPre; ++q) f4_add(d, gv[r][q]);
-          for (int j = tb[r] + kGtPre; j < te[r]; ++j) f4_add(d, ldg_cg_f4(ds_in + (size_t)__ldcg(indices_t + j) * kD + col));
-        }
-        float4 qr = make_float4(0.f, 0.f, 0.f, 0.f), qz = qr, qn = qr, qnr = qr;
-        if (ok[r]) {
-          const float deg = (float)(ip1[r] - ip0[r]);
-          st_f4_hint(dhz + (size_t)node[r] * kD + col, make_float4(d.x * zz.x, d.y * zz.y, d.z * zz.z, d.w * zz.w), pol_tmp);
-#define BWDQ2(f)                                         \
-  {                                                      \
-    const float dz_ = d.f * (hv.f - nn.f);               \
-    const float dn_ = d.f * (1.f - zz.f);                \
-    qn.f = dn_ * (1.f - nn.f * nn.f);                    \
-    qz.f = dz_ * zz.f * (1.f - zz.f);                    \
-    qr.f = qn.f * gh.f * rr.f * (1.f - rr.f);            \
-    qnr.f = qn.f * rr.f;                                 \
-  }
-          BWDQ2(x) BWDQ2(y) BWDQ2(z) BWDQ2(w)
-#undef BWDQ2
-          f4_add(sum[0], qr); f4_add(sum[1], qz); f4_add(sum[2], qn); f4_add(sum[3], qnr);
-          f4_fma(sum[4], deg, qr); f4_fma(sum[5], deg, qz); f4_fma(sum[6], deg, qn);
-        }
-        if (node[r] < Npad) {      // rows N .. Npad-1 are written as zeros (the weight-gradient GEMM sums over all 128 rows of a tile)
-          const size_t o_hi = image_offset(node[r], col, 0), o_lo = image_offset(node[r], col, 1);
-          uint2 ph, pl;
-          split4(qr, ph, pl);  *reinterpret_cast<uint2 *>(q_img + 0 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 0 * img_stride + o_lo) = pl;
-          split4(qz, ph, pl);  *reinterpret_cast<uint2 *>(q_img + 1 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 1 * img_stride + o_lo) = pl;
-          split4(qn, ph, pl);  *reinterpret_cast<uint2 *>(q_img + 2 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 2 * img_stride + o_lo) = pl;
-          split4(qnr, ph, pl); *reinterpret_cast<uint2 *>(q_img + 3 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 3 * img_stride + o_lo) = pl;
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty(stage));      // this warp has read its rows of the stage
-      if (warp == 0 && k + kGtStages < my_blocks) {  // refill the stage with block k + kGtStages once all 16 warps have released it
-        if (elect_one()) {
-          mbar_wait(empty(stage), use & 1);
-          fill(k + kGtStages);
-        }
-        __syncwarp();
-      }
-    }
-  }
-  // bias gradients: column sums of the 16 consumer warps, through the (now idle) first stage
-  __syncthreads();
-  float *red = reinterpret_cast<float *>(smem);
-  {
-#pragma unroll
-    for (int i = 0; i < 7; ++i) *reinterpret_cast<float4 *>(&red[(warp * 7 + i) * kD + lane * 4]) = sum[i];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 7 * kD; i += kGtThreads) {
-    float v_ = 0.f;
-#pragma unroll
-    for (int w = 0; w < kGtConsumers; ++w) v_ += red[(w * 7) * kD + i];
-    const int which = i >> 7, c_ = i & 127;
-    if (which == 0) { atomicAdd(db_ih + c_, v_); atomicAdd(db_hh + c_, v_); }
-    else if (which == 1) { atomicAdd(db_ih + kD + c_, v_); atomicAdd(db_hh + kD + c_, v_); }
-    else if (which == 2) atomicAdd(db_ih + 2 * kD + c_, v_);
-    else if (which == 3) atomicAdd(db_hh + 2 * kD + c_, v_);
-    else atomicAdd(db_fold + (which - 4) * kD + c_, v_);
-  }
-}
-
 // =================================================================================================
 // (2) dgrad
 // =================================================================================================
@@ -581,6 +351,362 @@ __global__ void __launch_bounds__(kD3Threads, 1) dgrad3_kernel(const uint8_t *__
       }
     }
     if (tr) trace_stamp(tron, k, 10);
+  }
+}
+
+// =================================================================================================
+// (1+2) gate backward fused into dgrad: one kernel per backward step (packed saved state)
+// =================================================================================================
+// No single CTA can both compute q for a tile and run all of dgrad on it: the dgrad CTA of one (role, column half) keeps 96 KB
+// of weights resident, and both roles take 384 KB.  So the four dgrad CTAs of a 128-node tile form a thread-block cluster:
+//   phase A  CTA rank c (= its (role, half), as in dgrad3_kernel) runs the gate backward on rows 32 c .. 32 c + 31 of the tile:
+//            dh', the packed gates and h (image pieces, or fp32 rows at step 0) arrive by TMA bulk copies in one 64 KB stage;
+//            the transposed edge gather of ds_in is folded in (register loads, data-dependent addresses).  It writes the four q
+//            images (global: the weight-gradient GEMM reads them later; rows N .. Npad-1 as zeros) and dh' * z into the rows
+//            of the dh OUTPUT, which the dh-role CTAs overwrite with acc + dh' * z in phase B — dh' * z never needs a plane of
+//            its own (so dh must alias neither dh_out nor ds_in: other clusters are still in phase A when this one writes dh);
+//   handover every writer fences its generic-proxy stores against the async proxy (the q tiles are read back by TMA), then
+//            the cluster barrier (arrive.release / wait.acquire);
+//   phase B  dgrad3_kernel's MMA loop, unchanged: the three q tiles of the role by bulk copy (L2 hits: written microseconds
+//            earlier), m64n64k16 bf16x3, the same MMA order, so ds and dh are bit-identical to the two-kernel path.
+// The phase-A operands of a tile and the q tiles share the two 64 KB stages as one ring, four uses per tile (A, q0, q1, q2):
+// the next tile's phase-A copy goes into the stage that q1 releases, so it streams from HBM while phase B runs.
+// Persistent over tiles, one cluster per 4 SMs; every CTA of a cluster runs the same tiles (each iteration holds a cluster
+// barrier).  HF32: h as fp32 rows (step 0: h_0 = x) or the activation image.  CSRP: the CSR scalars / first neighbour ids of the
+// folded gather pipelined across tiles, one value per lane (DDFA_TUNE_GATE_BWD_TMA = 2, default; 1 = fetched inside the tile).
+constexpr int kGtRows = 32;                                                                            // phase-A rows per CTA
+constexpr int kGtOffD = 0, kGtOffG = kGtRows * kD * 4, kGtOffH = kGtOffG + kGtRows * kD * 8;          // 16 KB | 32 KB | 16 KB
+static_assert(kGtOffH + kGtRows * kD * 4 == kD3StageBytes, "phase A's operands fill exactly one stage");
+static_assert(4 * kGtRows == kTileM, "four CTAs per tile");
+constexpr int kGtPre = 2;           // neighbour rows of the folded gather requested ahead of the stage wait, per row
+constexpr int kGtRowsPerWarp = kGtRows / kEpiWarps;
+
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+
+template <bool HF32, bool CSRP>
+__global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const float *__restrict__ dh_out, const float *__restrict__ h,
+                                                                       const uint8_t *__restrict__ h_img_src, const uint2 *__restrict__ gates_packed,
+                                                                       const int32_t *__restrict__ indptr, const float *__restrict__ ds_in,
+                                                                       const int32_t *__restrict__ indptr_t, const int32_t *__restrict__ indices_t,
+                                                                       int32_t N, uint8_t *__restrict__ q_img, size_t img_stride,
+                                                                       const uint8_t *__restrict__ packed3, float *__restrict__ ds, float *__restrict__ dh,
+                                                                       float *__restrict__ db_fold, float *__restrict__ db_ih, float *__restrict__ db_hh,
+                                                                       int hints) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t bar0 = sbase + kD3OffBar;
+  auto full = [&](int i) { return bar0 + 8u * i; };
+  auto empty = [&](int i) { return bar0 + 8u * (kD3Stages + i); };
+  const uint32_t w_full = bar0 + 8u * (2 * kD3Stages);
+  const int tron = (g_trace_on == 1);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rh = blockIdx.x & 3, role = rh >> 1, half = rh & 1;      // rh = the CTA's rank in its cluster
+  const int cluster = blockIdx.x >> 2, num_clusters = gridDim.x >> 2;
+  const int num_tiles = (N + kTileM - 1) / kTileM;
+  const int my_tiles = (num_tiles > cluster) ? (num_tiles - 1 - cluster) / num_clusters + 1 : 0;
+  const int tile0 = num_tiles - 1 - cluster;
+  auto tile_of = [&](int k) { return tile0 - k * num_clusters; };      // back to front, as in dgrad3_kernel
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kD3Stages; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), kEpiWarps); }
+    mbar_init(w_full, 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) trace_stamp(tron, 0, 0);
+  pdl_launch_dependents();
+
+  if (warp == kEpiWarps) {
+    // ===== producer: the weights once; per tile the phase-A operands of the CTA's 32 rows, then (after the handover) the
+    // three q tiles of this role.  All 32 lanes run the loop: every thread of the cluster takes part in its barrier. =====
+    const uint64_t pol_saved = l2_policy((hints & 2) ? 1 : 0), pol_dh = l2_policy((hints & 8) ? 1 : 0);
+    const uint64_t pol_q = l2_policy((hints & 64) ? 1 : 0);
+    if (my_tiles > 0 && elect_one()) {
+      mbar_arrive_expect_tx(w_full, kD3WBytes);
+      bulk_g2s(sbase, packed3 + (size_t)rh * kD3WBytes, kD3WBytes, w_full);
+    }
+    __syncwarp();
+    pdl_wait();      // dh_out and ds_in come from the previous kernel of the chain
+    int cc = 0;
+    for (int k = 0; k < my_tiles; ++k, cc += 4) {
+      const int tile = tile_of(k);
+      if (elect_one()) {
+        const int stage = cc % kD3Stages, use = cc / kD3Stages;
+        if (use > 0) mbar_wait_bounded(empty(stage), (use - 1) & 1);
+        const int64_t r0 = (int64_t)tile * kTileM + kGtRows * rh;
+        const int valid = (int)max((int64_t)0, min((int64_t)kGtRows, (int64_t)N - r0));      // rows that exist in the [N, ...] arrays
+        const uint32_t dst = sbase + kD3OffStage + stage * kD3StageBytes;
+        const uint32_t bytes = (uint32_t)valid * (kD * 4 + kD * 8) + (HF32 ? (uint32_t)valid * kD * 4 : (uint32_t)kGtRows * kD * 4);
+        mbar_arrive_expect_tx(full(stage), bytes);
+        if (valid > 0) {
+          bulk_g2s_hint(dst + kGtOffD, dh_out + r0 * kD, (uint32_t)valid * kD * 4, full(stage), pol_dh);
+          bulk_g2s_hint(dst + kGtOffG, gates_packed + r0 * kD, (uint32_t)valid * kD * 8, full(stage), pol_saved);
+        }
+        if (HF32) {
+          if (valid > 0) bulk_g2s_hint(dst + kGtOffH, h + r0 * kD, (uint32_t)valid * kD * 4, full(stage), pol_saved);
+        } else {      // the 32 rows of each of the four [128 x 64] bf16 chunks: 4 KB pieces (the image is padded to whole tiles)
+          const uint8_t *t0 = h_img_src + (size_t)tile * kImageTileBytes + (size_t)(kGtRows * rh) * 128;
+#pragma unroll
+          for (int ch = 0; ch < 4; ++ch) bulk_g2s_hint(dst + kGtOffH + ch * (kGtRows * 128), t0 + (size_t)ch * kChunkBytes, kGtRows * 128, full(stage), pol_saved);
+        }
+      }
+      __syncwarp();
+      cluster_arrive_release();
+      cluster_wait_acquire();
+      if (elect_one()) {
+        fence_proxy_async_global();      // the q tiles the cluster just wrote are read through the async proxy
+        for (int g = 0; g < 3; ++g) {
+          const int m = g < 2 ? g : (role == 0 ? 2 : 3);      // q_r, q_z, then q_n (ds) or q_nr (dh)
+          const int c = cc + 1 + g, stage = c % kD3Stages, use = c / kD3Stages;
+          if (use > 0) mbar_wait_bounded(empty(stage), (use - 1) & 1);
+          mbar_arrive_expect_tx(full(stage), kD3StageBytes);
+          bulk_g2s_hint(sbase + kD3OffStage + stage * kD3StageBytes, q_img + (size_t)m * img_stride + (size_t)tile * kImageTileBytes,
+                        kD3StageBytes, full(stage), pol_q);
+          if (g != 1) trace_stamp(tron, k, g == 0 ? 1 : 2);      // 1: first / 2: last q copy of the tile issued
+        }
+      }
+      __syncwarp();
+    }
+  } else {
+    // ===== consumers: phase A, warp w owns rows w + 8 j (j < 4) of the CTA's 32; phase B, warpgroup wg owns nodes 64 wg .. + 63 =====
+    pdl_wait();
+    const int col = lane * 4;
+    // L2 policies (created where they are used: 64-bit values live across the whole loop made the kernel spill)
+    // pol_tmp: ds / dh / dh' * z die after the next kernel has read them; pol_dhz: the last read of dh' * z
+#define DDFA_POL_TMP l2_policy((hints & 4) ? 2 : 0)
+#define DDFA_POL_DHZ l2_policy((hints & 8) ? 1 : 0)
+    const int wg = warp >> 2;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int col0 = half * 64 + 2 * (lane & 3);
+    const bool tr = (warp == 0 && lane == 0);
+    float4 sum[7];      // the seven column sums (bias gradients) over all the warp's rows, combined once at the end
+#pragma unroll
+    for (int i = 0; i < 7; ++i) sum[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    // The CSR data of the warp's four rows — indptr (in-degree), indptr_t and the first kGtPre transposed neighbour ids — is a
+    // chain of dependent global loads (indptr_t -> indices_t -> ds row), warp-uniform, so with CSRP it is kept ONE VALUE PER LANE
+    // and pipelined across tiles: lanes 0-7 hold indptr[node_r + {0,1}], lanes 8-15 indptr_t[node_r + {0,1}] (r = (lane >> 1) & 3)
+    // of a tile, lanes 16-23 its ids id[r][q] (q = lane & 1); tile k requests the scalars of tile k + 2 and the ids of tile k + 1
+    // and broadcasts its own by shuffle — only the ds rows themselves are requested in the tile that adds them.
+    static_assert(kGtPre == 2 && kGtRowsPerWarp == 4, "lane slots below assume four rows per warp and two prefetched neighbours per row");
+    auto node_of = [&](int tile, int r) { return (int64_t)tile * kTileM + kGtRows * rh + warp + kEpiWarps * r; };
+    auto load_scalars = [&](int kk) -> int {
+      int v = 0;
+      if (kk < my_tiles && lane < 16) {
+        const int64_t nd = node_of(tile_of(kk), (lane >> 1) & 3);
+        const int32_t *base = lane < 8 ? indptr : indptr_t;
+        if (nd < N && base) v = __ldcg(base + nd + (lane & 1));
+      }
+      return v;
+    };
+    auto load_ids = [&](int sc) -> int {
+      const int r_ = (lane >> 1) & 3, q_ = lane & 1;
+      const int tb_ = __shfl_sync(0xffffffffu, sc, 8 + 2 * r_), te_ = __shfl_sync(0xffffffffu, sc, 9 + 2 * r_);
+      int v = -1;
+      if (lane >= 16 && lane < 24 && tb_ + q_ < te_) v = __ldcg(indices_t + tb_ + q_);
+      return v;
+    };
+    int sc_cur = 0, sc_next = 0, id_cur = -1;
+    if constexpr (CSRP) {
+      sc_cur = load_scalars(0); sc_next = load_scalars(1);
+      id_cur = load_ids(sc_cur);
+    }
+    int cc = 0;
+    for (int k = 0; k < my_tiles; ++k) {
+      const int tile = tile_of(k);
+      // ---------------- phase A ----------------
+      {
+        const int stage = cc % kD3Stages, use = cc / kD3Stages;
+        ++cc;
+        const int64_t node0 = node_of(tile, 0);      // row r of the warp is node0 + kEpiWarps r
+        bool ok[kGtRowsPerWarp];
+        int tb[kGtRowsPerWarp], te[kGtRowsPerWarp];
+        float deg[kGtRowsPerWarp];
+        int id[kGtRowsPerWarp][kGtPre];      // the first kGtPre neighbours of each row (a CFG node has ~2 in-edges); longer lists finish below
+        if constexpr (CSRP) {
+          const int sc_next2 = load_scalars(k + 2);
+          const int id_next = load_ids(sc_next);
+#pragma unroll
+          for (int r = 0; r < kGtRowsPerWarp; ++r) {
+            ok[r] = node0 + kEpiWarps * r < N;
+            deg[r] = (float)(__shfl_sync(0xffffffffu, sc_cur, 2 * r + 1) - __shfl_sync(0xffffffffu, sc_cur, 2 * r));
+            tb[r] = __shfl_sync(0xffffffffu, sc_cur, 8 + 2 * r); te[r] = __shfl_sync(0xffffffffu, sc_cur, 9 + 2 * r);
+#pragma unroll
+            for (int q = 0; q < kGtPre; ++q) id[r][q] = __shfl_sync(0xffffffffu, id_cur, 16 + 2 * r + q);
+          }
+          sc_cur = sc_next; sc_next = sc_next2; id_cur = id_next;
+        } else {      // everything requested inside the tile (global, independent of the staged operands: before the wait)
+#pragma unroll
+          for (int r = 0; r < kGtRowsPerWarp; ++r) {
+            const int64_t nd = node0 + kEpiWarps * r;
+            ok[r] = nd < N;
+            tb[r] = te[r] = 0;
+            deg[r] = 0.f;
+            if (ok[r]) {
+              deg[r] = (float)(__ldcg(indptr + nd + 1) - __ldcg(indptr + nd));
+              if (indptr_t) { tb[r] = __ldcg(indptr_t + nd); te[r] = __ldcg(indptr_t + nd + 1); }
+            }
+          }
+#pragma unroll
+          for (int r = 0; r < kGtRowsPerWarp; ++r)
+#pragma unroll
+            for (int q = 0; q < kGtPre; ++q) id[r][q] = (tb[r] + q < te[r]) ? __ldcg(indices_t + tb[r] + q) : -1;
+        }
+        float4 gv[kGtRowsPerWarp][kGtPre];
+#pragma unroll
+        for (int r = 0; r < kGtRowsPerWarp; ++r)
+#pragma unroll
+          for (int q = 0; q < kGtPre; ++q) gv[r][q] = id[r][q] >= 0 ? ldg_cg_f4(ds_in + (size_t)id[r][q] * kD + col) : make_float4(0.f, 0.f, 0.f, 0.f);
+        mbar_wait_bounded(full(stage), use & 1);
+        const uint8_t *st = smem + kD3OffStage + stage * kD3StageBytes;
+#pragma unroll
+        for (int r = 0; r < kGtRowsPerWarp; ++r) {
+          const int row = warp + kEpiWarps * r;             // row inside the CTA's 32
+          float4 d = make_float4(0.f, 0.f, 0.f, 0.f), hv = d, rr = d, zz = d, nn = d, gh = d;
+          if (ok[r]) {
+            d = *reinterpret_cast<const float4 *>(st + kGtOffD + row * (kD * 4) + col * 4);
+            const uint4 g0 = *reinterpret_cast<const uint4 *>(st + kGtOffG + row * (kD * 8) + col * 8);
+            const uint4 g1 = *reinterpret_cast<const uint4 *>(st + kGtOffG + row * (kD * 8) + col * 8 + 16);
+            unpack_gates(make_uint2(g0.x, g0.y), rr.x, zz.x, nn.x, gh.x);
+            unpack_gates(make_uint2(g0.z, g0.w), rr.y, zz.y, nn.y, gh.y);
+            unpack_gates(make_uint2(g1.x, g1.y), rr.z, zz.z, nn.z, gh.z);
+            unpack_gates(make_uint2(g1.z, g1.w), rr.w, zz.w, nn.w, gh.w);
+            if (HF32) {
+              hv = *reinterpret_cast<const float4 *>(st + kGtOffH + row * (kD * 4) + col * 4);
+            } else {      // piece [v][kb = col / 64] of 32 rows x 128 B; 16-byte units swizzled by (tile row) & 7 == row & 7 (32 rh is a multiple of 8)
+              const uint32_t off = (uint32_t)((col >> 6) * (kGtRows * 128) + row * 128 + (((((col & 63) >> 3) ^ (row & 7)) & 7) << 4) + (col & 7) * 2);
+              const uint2 hh = *reinterpret_cast<const uint2 *>(st + kGtOffH + off);
+              const uint2 hl = *reinterpret_cast<const uint2 *>(st + kGtOffH + 2 * (kGtRows * 128) + off);
+              const float4 a = bf16x4_to_f4(hh), b = bf16x4_to_f4(hl);
+              hv = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+            }
+#pragma unroll
+            for (int q = 0; q < kGtPre; ++q) f4_add(d, gv[r][q]);
+            for (int j = tb[r] + kGtPre; j < te[r]; ++j) f4_add(d, ldg_cg_f4(ds_in + (size_t)__ldcg(indices_t + j) * kD + col));
+          }
+          float4 qr = make_float4(0.f, 0.f, 0.f, 0.f), qz = qr, qn = qr, qnr = qr;
+          const int64_t node = node0 + kEpiWarps * r;
+          if (ok[r]) {
+            st_f4_hint(dh + (size_t)node * kD + col, make_float4(d.x * zz.x, d.y * zz.y, d.z * zz.z, d.w * zz.w), DDFA_POL_TMP);
+#define BWDQ2(f)                                         \
+  {                                                      \
+    const float dz_ = d.f * (hv.f - nn.f);               \
+    const float dn_ = d.f * (1.f - zz.f);                \
+    qn.f = dn_ * (1.f - nn.f * nn.f);                    \
+    qz.f = dz_ * zz.f * (1.f - zz.f);                    \
+    qr.f = qn.f * gh.f * rr.f * (1.f - rr.f);            \
+    qnr.f = qn.f * rr.f;                                 \
+  }
+            BWDQ2(x) BWDQ2(y) BWDQ2(z) BWDQ2(w)
+#undef BWDQ2
+            f4_add(sum[0], qr); f4_add(sum[1], qz); f4_add(sum[2], qn); f4_add(sum[3], qnr);
+            f4_fma(sum[4], deg[r], qr); f4_fma(sum[5], deg[r], qz); f4_fma(sum[6], deg[r], qn);
+          }
+          // rows N .. Npad-1 are written as zeros (the weight-gradient GEMM sums over all 128 rows of a tile)
+          const size_t o_hi = image_offset(node, col, 0), o_lo = image_offset(node, col, 1);
+          uint2 ph, pl;
+          split4(qr, ph, pl);  *reinterpret_cast<uint2 *>(q_img + 0 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 0 * img_stride + o_lo) = pl;
+          split4(qz, ph, pl);  *reinterpret_cast<uint2 *>(q_img + 1 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 1 * img_stride + o_lo) = pl;
+          split4(qn, ph, pl);  *reinterpret_cast<uint2 *>(q_img + 2 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 2 * img_stride + o_lo) = pl;
+          split4(qnr, ph, pl); *reinterpret_cast<uint2 *>(q_img + 3 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 3 * img_stride + o_lo) = pl;
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty(stage));      // this warp has read its rows of the stage
+      }
+      // ---------------- handover: q and dh' * z of the whole tile visible to the cluster ----------------
+      fence_proxy_async_global();
+      cluster_arrive_release();
+      cluster_wait_acquire();
+      if (tr) trace_stamp(tron, k, 11);      // 11: handover done
+      // ---------------- phase B: dgrad3_kernel's loop ----------------
+      if (k == 0) mbar_wait_bounded(w_full, 0);
+      float acc[32];
+      int pending = -1;      // the stage whose MMAs were issued last and not yet waited for
+      if (tr) { trace_stamp(tron, k, 7); trace_stamp(tron, k, 3); }
+      for (int g = 0; g < 3; ++g, ++cc) {
+        const int stage = cc % kD3Stages, use = cc / kD3Stages;
+        mbar_wait_bounded(full(stage), use & 1);
+        if (tr && g != 1) trace_stamp(tron, k, g == 0 ? 4 : 5);      // 4: first / 5: last q tile landed
+        wgmma_fence();
+        const uint32_t a0 = sbase + kD3OffStage + stage * kD3StageBytes + wg * 8192;
+        const uint32_t w0 = sbase + g * 4 * kD3WChunkBytes;
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) {
+#pragma unroll
+          for (int k4 = 0; k4 < 4; ++k4) {
+            const uint64_t a_hi = gmma_desc(a0 + kb * kChunkBytes + k4 * 32), a_lo = gmma_desc(a0 + (2 + kb) * kChunkBytes + k4 * 32);
+            const uint64_t b_hi = gmma_desc(w0 + kb * kD3WChunkBytes + k4 * 32), b_lo = gmma_desc(w0 + (2 + kb) * kD3WChunkBytes + k4 * 32);
+            wgmma_n64<0, 0>(acc, a_hi, b_hi, (g == 0 && kb == 0 && k4 == 0) ? 0u : 1u);
+            wgmma_n64<0, 0>(acc, a_hi, b_lo, 1u);
+            wgmma_n64<0, 0>(acc, a_lo, b_hi, 1u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        __syncwarp();
+        if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
+        pending = stage;
+      }
+      // dh = acc + (dh' * z), the elementwise term written into dh's rows in phase A: the first of the thread's two rows is
+      // fetched while the last MMAs run, the second after them (both in flight at once would make the kernel spill)
+      float2 dv[8];
+      auto fetch_dv = [&](int hh) {
+        const uint64_t pol_dhz = DDFA_POL_DHZ;
+        const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          dv[j] = make_float2(0.f, 0.f);
+          if (role == 1 && node < N) {
+            const float *p = dh + node * kD + col0 + 8 * j;
+            dv[j] = make_float2(ldg_cg_f32_hint(p, pol_dhz), ldg_cg_f32_hint(p + 1, pol_dhz));
+          }
+        }
+      };
+      fetch_dv(0);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (tr) { trace_stamp(tron, k, 6); trace_stamp(tron, k, 8); }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(pending));
+      if (tr) trace_stamp(tron, k, 9);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        if (hh == 1) fetch_dv(1);
+        const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
+        if (node < N) {
+          const uint64_t pol_tmp = DDFA_POL_TMP;
+          float *out = role == 0 ? ds : dh;
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            st_f2_hint(out + node * kD + col0 + 8 * j, make_float2(acc[4 * j + 2 * hh] + dv[j].x, acc[4 * j + 2 * hh + 1] + dv[j].y), pol_tmp);
+        }
+      }
+      if (tr) trace_stamp(tron, k, 10);
+    }
+#undef DDFA_POL_TMP
+#undef DDFA_POL_DHZ
+    // bias gradients: the warps' column sums through the stages, once both warpgroups are past their last MMAs
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
+    float *red = reinterpret_cast<float *>(smem + kD3OffStage);
+#pragma unroll
+    for (int i = 0; i < 7; ++i) *reinterpret_cast<float4 *>(&red[(warp * 7 + i) * kD + col]) = sum[i];
+  }
+  __syncthreads();
+  const float *red = reinterpret_cast<const float *>(smem + kD3OffStage);
+  for (int i = threadIdx.x; i < 7 * kD; i += kD3Threads) {
+    float v_ = 0.f;
+#pragma unroll
+    for (int w = 0; w < kEpiWarps; ++w) v_ += red[(w * 7) * kD + i];
+    const int which = i >> 7, c_ = i & 127;
+    // 0:S(q_r) 1:S(q_z) 2:S(q_n) 3:S(q_nr) 4:S(deg q_r) 5:S(deg q_z) 6:S(deg q_n)
+    if (which == 0) { atomicAdd(db_ih + c_, v_); atomicAdd(db_hh + c_, v_); }
+    else if (which == 1) { atomicAdd(db_ih + kD + c_, v_); atomicAdd(db_hh + kD + c_, v_); }
+    else if (which == 2) atomicAdd(db_ih + 2 * kD + c_, v_);
+    else if (which == 3) atomicAdd(db_hh + 2 * kD + c_, v_);
+    else atomicAdd(db_fold + (which - 4) * kD + c_, v_);
   }
 }
 
@@ -775,6 +901,54 @@ int gru_tc2_bwd_finish(int32_t N, float *dw_fold, float *dw_hh, void *workspace,
   return DDFA_OK;
 }
 
+// Clusters of bwd_step_fused_kernel that fit on the device at once (one CTA per SM; queried once per instantiation)
+template <bool HF32, bool CSRP>
+static int bwd_fused_max_clusters(int *out) {
+  static std::atomic<int> cached{0};
+  int v = cached.load(std::memory_order_relaxed);
+  if (v == 0) {
+    DDFA_CUDA(cudaFuncSetAttribute(tc2b::bwd_step_fused_kernel<HF32, CSRP>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(kNumSMs / 4 * 4);
+    cfg.blockDim = dim3(tc2b::kD3Threads);
+    cfg.dynamicSmemBytes = tc2b::kD3SmemAlloc;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 4;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    DDFA_CUDA(cudaOccupancyMaxActiveClusters(&v, tc2b::bwd_step_fused_kernel<HF32, CSRP>, &cfg));
+    if (v < 1) {
+      set_error("tcgen05 engine (bwd): bwd_step_fused_kernel fits no 4-CTA cluster on this device");
+      return DDFA_ERR_CUDA;
+    }
+    cached.store(v, std::memory_order_relaxed);
+  }
+  *out = v;
+  return DDFA_OK;
+}
+int gru_tc2b_fused_max_clusters(int *out) { return bwd_fused_max_clusters<false, true>(out); }
+
+// One cluster of 4 CTAs per 128-node tile, persistent: min(tiles, the clusters that fit) clusters.  Chained (PDL) under bit 4 of
+// DDFA_TUNE_PDL_MASK, the bit of the gate backward whose place it takes at the head of the step.
+template <bool HF32, bool CSRP>
+static int launch_bwd_fused(int tiles, cudaStream_t stream, const float *dh_out, const float *h, const void *h_img_in, const void *gates_packed,
+                            const int32_t *indptr, const float *ds_in, const int32_t *indptr_t, const int32_t *indices_t, int32_t N,
+                            uint8_t *q_img, size_t img, const uint8_t *packed, float *ds, float *dh, float *db_fold, float *db_ih, float *db_hh) {
+  int clusters = 0;
+  const int rc = bwd_fused_max_clusters<HF32, CSRP>(&clusters);
+  if (rc != DDFA_OK) return rc;
+  if (clusters > tiles) clusters = tiles;
+  DDFA_CUDA(cudaFuncSetAttribute(tc2b::bwd_step_fused_kernel<HF32, CSRP>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
+  DDFA_CUDA(launch_chain_cluster(4, 4, tc2b::bwd_step_fused_kernel<HF32, CSRP>, dim3(clusters * 4), dim3(tc2b::kD3Threads), tc2b::kD3SmemAlloc,
+                                 stream, dh_out, h, static_cast<const uint8_t *>(h_img_in), static_cast<const uint2 *>(gates_packed), indptr,
+                                 ds_in, ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, l2_hints()));
+  DDFA_CHECK_LAUNCH("tc2b::bwd_step_fused_kernel");
+  return DDFA_OK;
+}
+
 // wgrad_mode: 0 = immediate (dW += this step's contribution before returning), 1 = first step of a deferred accumulation
 // (partials overwritten), 2 = further deferred step (partials accumulated); deferred passes end with gru_tc2_bwd_finish.
 // wgrad_mode >= 16: keep this step's q images in workspace slot (wgrad_mode - 16) and run no weight-gradient GEMM now —
@@ -796,40 +970,30 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
   uint8_t *packed = static_cast<uint8_t *>(workspace);
   const size_t img = tcc::image_bytes(N);
   uint8_t *h_img_ws = packed + kPackedTotal;
-  float *dhz = reinterpret_cast<float *>(h_img_ws + img);
   float *partial = reinterpret_cast<float *>(h_img_ws + 3 * img);
   uint8_t *q_img = packed + bwd_fixed_bytes(N) + (size_t)q_slot * 4 * img;
   const uint8_t *h_img = h_img_in ? static_cast<const uint8_t *>(h_img_in) : h_img_ws;
-  const int64_t rows = ((int64_t)N + tcc::kTileM - 1) / tcc::kTileM * tcc::kTileM;
-  unsigned gb_grid = 1;
-  {
-    const int64_t want = (rows + tc2b::kGbWarps - 1) / tc2b::kGbWarps;
-    gb_grid = (unsigned)(want < 2 * kNumSMs ? want : 2 * kNumSMs);
-  }
-  if (gates_packed && gate_bwd_tma()) {
-    // TMA-staged form (packed saved state only): one CTA per SM, three 64 KB stages
-    const int blocks32 = (int)(rows / tc2b::kGtRows);
-    const int grid = blocks32 < kNumSMs ? blocks32 : kNumSMs;
-    const bool csrp = gate_bwd_tma() >= 2;
-#define DDFA_GT_LAUNCH(HF32, CSRP)                                                                                                             \
-  do {                                                                                                                                         \
-    DDFA_CUDA(cudaFuncSetAttribute(tc2b::gate_bwd_tma_kernel<HF32, CSRP>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kGtSmem));        \
-    DDFA_CUDA(launch_chain(4, tc2b::gate_bwd_tma_kernel<HF32, CSRP>, dim3(grid), dim3(tc2b::kGtThreads), tc2b::kGtSmem, stream, dh_out, h,     \
-                           static_cast<const uint8_t *>(h_img_in), static_cast<const uint2 *>(gates_packed), indptr, ds_in,                    \
-                           ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, dhz, db_fold, db_ih, db_hh, l2_hints()));                    \
-  } while (0)
-    if (h) { if (csrp) DDFA_GT_LAUNCH(true, true); else DDFA_GT_LAUNCH(true, false); }
-    else   { if (csrp) DDFA_GT_LAUNCH(false, true); else DDFA_GT_LAUNCH(false, false); }
-#undef DDFA_GT_LAUNCH
-  } else
-  DDFA_CUDA(launch_chain(4, tc2b::gate_bwd_image_kernel, dim3(gb_grid), dim3(32 * tc2b::kGbWarps), 0, stream, dh_out, h,
-                         static_cast<const uint8_t *>(h_img_in), gates, static_cast<const uint4 *>(gates_packed), indptr, ds_in,
-                         ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, h_img_in ? nullptr : h_img_ws, dhz, db_fold, db_ih, db_hh,
-                         l2_hints()));
-  DDFA_CHECK_LAUNCH("tc2b::gate_bwd_image_kernel");
-  DDFA_CUDA(cudaFuncSetAttribute(tc2b::wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kWgSmemAlloc));
   const int tiles = (N + tcc::kTileM - 1) / tcc::kTileM;
-  {
+  if (gates_packed && gate_bwd_tma()) {
+    // packed saved state: gate backward and dgrad in one cluster kernel (dh' * z handed over through the rows of dh)
+    const bool csrp = gate_bwd_tma() >= 2;
+    int rc = DDFA_OK;
+    if (h) rc = csrp ? launch_bwd_fused<true, true>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh)
+                     : launch_bwd_fused<true, false>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh);
+    else   rc = csrp ? launch_bwd_fused<false, true>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh)
+                     : launch_bwd_fused<false, false>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh);
+    if (rc != DDFA_OK) return rc;
+  } else {
+    // register-path gate backward, then dgrad3 (the fp32 saved state, and DDFA_TUNE_GATE_BWD_TMA = 0)
+    const int64_t rows = (int64_t)tiles * tcc::kTileM;
+    const int64_t want = (rows + tc2b::kGbWarps - 1) / tc2b::kGbWarps;
+    const unsigned gb_grid = (unsigned)(want < 2 * kNumSMs ? want : 2 * kNumSMs);
+    float *dhz = reinterpret_cast<float *>(h_img_ws + img);
+    DDFA_CUDA(launch_chain(4, tc2b::gate_bwd_image_kernel, dim3(gb_grid), dim3(32 * tc2b::kGbWarps), 0, stream, dh_out, h,
+                           static_cast<const uint8_t *>(h_img_in), gates, static_cast<const uint4 *>(gates_packed), indptr, ds_in,
+                           ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, h_img_in ? nullptr : h_img_ws, dhz, db_fold, db_ih, db_hh,
+                           l2_hints()));
+    DDFA_CHECK_LAUNCH("tc2b::gate_bwd_image_kernel");
     DDFA_CUDA(cudaFuncSetAttribute(tc2b::dgrad3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
     int groups = kNumSMs / 4;
     if (groups > tiles) groups = tiles;
@@ -837,6 +1001,7 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
                            static_cast<const uint8_t *>(packed), N, ds, dh, l2_hints()));
     DDFA_CHECK_LAUNCH("tc2b::dgrad3_kernel");
   }
+  DDFA_CUDA(cudaFuncSetAttribute(tc2b::wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kWgSmemAlloc));
   if (wgrad_mode >= 16) return DDFA_OK;       // q images kept; the batched weight-gradient launch follows the last step
   // every one of the 74 x 2 CTAs writes its partial slot (zeros if it owns no tile), so the reduction can sum all of them
   tc2b::WgBatch one = {};

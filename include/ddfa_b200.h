@@ -52,10 +52,14 @@ int ddfa_engine_available(int engine);
  * the library reads no environment variables).  ddfa_tuning_get returns -1 for an unknown key. */
 enum {
   DDFA_TUNE_L2_HINTS = 0,       /* bit mask of L2 eviction-priority hints, default 23 (csrc/common.cuh) */
-  DDFA_TUNE_PDL_MASK = 1,       /* bit mask of kernels launched with programmatic stream serialization, default 15 */
+  DDFA_TUNE_PDL_MASK = 1,       /* bit mask of kernels launched with programmatic stream serialization, default 15: 1 image gather, 2 forward GRU
+                                   step, 4 the first kernel of a backward GRU step (the fused kernel, or the register-path gate backward),
+                                   8 dgrad after the register-path gate backward */
   DDFA_TUNE_GATHER_VARIANT = 2, /* launch shape of the D = 128 edge gather (ddfa_gather_sum_variant ids), default 9 */
   DDFA_TUNE_FWD_PAIR = 3,       /* reserved: only 0 is accepted (the CTA-pair form of the forward kernel does not exist on sm_90a) */
-  DDFA_TUNE_GATE_BWD_TMA = 4,   /* gate backward: 0 register loads; 1 dh / gates / h stream through a TMA-fed shared-memory ring; 2 (default) = 1 + the folded gather's CSR scalars pipelined across iterations */
+  DDFA_TUNE_GATE_BWD_TMA = 4,   /* backward GRU step with the packed saved state: 0 register-path gate backward, then dgrad (two kernels, and the
+                                   only path of the fp32 saved state); 1 one cluster kernel: gate backward on TMA-staged dh / gates / h, then dgrad;
+                                   2 (default) = 1 + the folded gather's CSR scalars pipelined across tiles */
   DDFA_TUNE_GATHER_SRC_GROUPS = 5, /* image->image edge gather: row groups (of 4 rows) walked per warp with the CSR chain pipelined; 0 (default) = 1 group (2 / 4 measured neutral), or 1 / 2 / 4 */
   DDFA_TUNE__COUNT = 6
 };
@@ -64,7 +68,8 @@ int ddfa_tuning_get(int key);
 /* development aid: in-kernel pipeline timeline of the tensor-core kernels (SM-clock stamps per CTA / tile / event, 132 x 12 x 12).
  * ddfa_debug_set(2, v): v = 0 off, 1 = forward + dgrad kernels, 2 = forward + wgrad kernels;
  * ddfa_debug_read(2 | 3, host, bytes): stamps of the backward (2) or forward (3) kernel's last launch;
- * ddfa_debug_read(4, host, 4): int32 count of timed-out mbarrier waits in the TMA-staged gather variants (0 when healthy). */
+ * ddfa_debug_read(4, host, 4): int32 count of timed-out mbarrier waits in the TMA-staged gather variants (0 when healthy);
+ * ddfa_debug_read(5, host, 4): int32 number of 4-CTA clusters of the fused backward step kernel resident at once on this device. */
 int ddfa_debug_set(int key, int value);
 int ddfa_debug_read(int key, void *host_out, size_t bytes);
 /* number of CUDA kernels this library has launched in this process (monotonic; for bench accounting) */
