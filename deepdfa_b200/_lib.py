@@ -84,6 +84,8 @@ _SIGNATURES = {
     "ddfa_graph_label_bce_valid": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, _f32, _f32, _vp, _vp, _vp, _vp]),
     "ddfa_adam_flat": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _vp]),
     "ddfa_allreduce_adam_p2p": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _vp]),
+    "ddfa_adam_flat_hp": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "ddfa_allreduce_adam_p2p_hp": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
 }
 

@@ -54,7 +54,10 @@ __global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp,
                                                                  float *__restrict__ v, const int32_t *__restrict__ step_count,
                                                                  int64_t numel, int64_t loss_off, float *__restrict__ loss_out,
                                                                  uint32_t *__restrict__ ticket, float lr, float beta1, float beta2,
-                                                                 float eps, float wd) {
+                                                                 float eps, float wd, const float *__restrict__ hyper) {
+  if (hyper) {      // [lr, beta1, beta2, eps, wd] read at run time (ddfa_allreduce_adam_p2p_hp); same arithmetic as the by-value form
+    lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], wd = hyper[4];
+  }
   __shared__ float s_c[2];
   __shared__ int s_last;
   const int32_t t0 = *step_count;
@@ -116,11 +119,13 @@ __global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp,
 }  // namespace p2p
 }  // namespace ddfa
 
-extern "C" int ddfa_allreduce_adam_p2p(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
-                                       int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
-                                       int64_t loss_offset, float *loss_out, uint32_t *ticket, float lr, float beta1, float beta2,
-                                       float eps, float weight_decay, void *stream_) {
-  using namespace ddfa;
+namespace ddfa {
+namespace p2p {
+
+static int launch(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank, int32_t world,
+                  float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel, int64_t loss_offset, float *loss_out,
+                  uint32_t *ticket, float lr, float beta1, float beta2, float eps, float weight_decay, const float *hyper,
+                  void *stream_) {
   DDFA_REQUIRE(world >= 1 && world <= p2p::kMaxRanks && rank >= 0 && rank < world, "ddfa_allreduce_adam_p2p: rank %d / world %d (max %d ranks)", rank,
                world, p2p::kMaxRanks);
   DDFA_REQUIRE(numel >= 0 && numel % 4 == 0, "ddfa_allreduce_adam_p2p: numel (%lld) must be a multiple of 4", (long long)numel);
@@ -139,7 +144,27 @@ extern "C" int ddfa_allreduce_adam_p2p(void *const *peer_params, const void *con
   if (blocks < 1) blocks = 1;
   if (blocks > 64) blocks = 64;        // all CTAs must be co-resident: they spin on flags (64 x 256 threads fit any idle H100)
   p2p::allreduce_adam_p2p_kernel<<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out, ticket,
-                                                             lr, beta1, beta2, eps, weight_decay);
+                                                             lr, beta1, beta2, eps, weight_decay, hyper);
   DDFA_CHECK_LAUNCH("allreduce_adam_p2p_kernel");
   return adam_step_inc_launch(step_count, stream);
+}
+
+}  // namespace p2p
+}  // namespace ddfa
+
+extern "C" int ddfa_allreduce_adam_p2p(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
+                                       int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                                       int64_t loss_offset, float *loss_out, uint32_t *ticket, float lr, float beta1, float beta2,
+                                       float eps, float weight_decay, void *stream_) {
+  return ddfa::p2p::launch(peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out,
+                           ticket, lr, beta1, beta2, eps, weight_decay, nullptr, stream_);
+}
+
+extern "C" int ddfa_allreduce_adam_p2p_hp(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
+                                          int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                                          int64_t loss_offset, float *loss_out, uint32_t *ticket, const float *hyper, void *stream_) {
+  using namespace ddfa;
+  DDFA_REQUIRE(hyper, "ddfa_allreduce_adam_p2p_hp: NULL hyperparameter pointer");
+  return p2p::launch(peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out, ticket,
+                     0.f, 0.f, 0.f, 0.f, 0.f, hyper, stream_);
 }

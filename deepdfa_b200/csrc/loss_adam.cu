@@ -53,9 +53,15 @@ __global__ void __launch_bounds__(256) graph_label_bce_kernel(const float *__res
   }
 }
 
+// hyper: NULL (the by-value lr .. wd are used) or 5 device floats [lr, beta1, beta2, eps, wd] read when the kernel runs, so a
+// captured launch sees values written after the capture.  Either way the update below is the same arithmetic.
 __global__ void __launch_bounds__(256) adam_flat_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
                                                         float *__restrict__ v, const int32_t *__restrict__ step_count, int64_t n,
-                                                        float lr, float beta1, float beta2, float eps, float wd) {
+                                                        float lr, float beta1, float beta2, float eps, float wd,
+                                                        const float *__restrict__ hyper) {
+  if (hyper) {
+    lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], wd = hyper[4];
+  }
   __shared__ float s_c[2];
   if (threadIdx.x == 0) {
     const double t = (double)(*step_count + 1);
@@ -119,7 +125,21 @@ int ddfa_adam_flat(float *params, const float *grads, float *exp_avg, float *exp
   cudaStream_t stream = as_stream(stream_);
   if (numel > 0) {
     adam_flat_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel, lr,
-                                                                         beta1, beta2, eps, weight_decay);
+                                                                         beta1, beta2, eps, weight_decay, nullptr);
+    DDFA_CHECK_LAUNCH("adam_flat_kernel");
+  }
+  return adam_step_inc_launch(step_count, stream);
+}
+
+int ddfa_adam_flat_hp(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                      const float *hyper, void *stream_) {
+  using namespace ddfa;
+  DDFA_REQUIRE(numel >= 0, "ddfa_adam_flat_hp: negative numel");
+  DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && hyper, "ddfa_adam_flat_hp: NULL pointer");
+  cudaStream_t stream = as_stream(stream_);
+  if (numel > 0) {
+    adam_flat_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel, 0.f,
+                                                                         0.f, 0.f, 0.f, 0.f, hyper);
     DDFA_CHECK_LAUNCH("adam_flat_kernel");
   }
   return adam_step_inc_launch(step_count, stream);

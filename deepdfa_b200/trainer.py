@@ -8,6 +8,8 @@ data-path collective (SURVEY.md §8e); the gradient all-reduce is the only excha
 
 Replaces, for the hot path only, Lightning's ``Trainer.fit`` loop around
 ``BaseModule.training_step`` (base_module.py:171-199) + ``torch.optim.Adam`` (config_default.yaml:43-47).
+``FusedTrainer.optimizer`` (:class:`FusedAdam`) is the ``torch.optim.Optimizer`` face of the fused Adam: checkpoints in
+``torch.optim.Adam``'s format and LR schedulers that reach captured steps.
 """
 from __future__ import annotations
 
@@ -24,6 +26,177 @@ from .batched_graph import BatchedCFG, as_batched_cfg
 from .module import FlowGNNGGNNModule, _ENGINES
 
 _ALIGN = 64  # elements; keeps every parameter 256-byte aligned inside the flat buffers
+
+
+def flat_offsets(plist):
+    """Element offset of every tensor of ``plist`` (``module.param_list()`` order) inside the flat buffers, and their length:
+    every slot is rounded up to ``_ALIGN`` elements."""
+    offs, total = [], 0
+    for p in plist:
+        offs.append(total)
+        total += (p.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
+    return offs, total
+
+
+def owned_range(numel: int, rank: int, world: int):
+    """``[lo, hi)``: the elements of the flat buffers whose Adam moments rank ``rank`` of ``world`` keeps up to date under
+    ``exchange="p2p"``.  Mirrors ``allreduce_adam_p2p_kernel``: the buffers are cut into 16-byte units and every rank owns
+    ``per = ceil(numel / 4 / world)`` consecutive units (the last rank fewer, possibly none)."""
+    n4 = numel // 4
+    per = (n4 + world - 1) // world
+    lo = min(n4, rank * per)
+    return 4 * lo, 4 * min(n4, lo + per)
+
+
+_ADAM_FLAGS = dict(amsgrad=False, maximize=False, foreach=None, capturable=False, differentiable=False, fused=None,
+                   decoupled_weight_decay=False)
+_UNSUPPORTED = ("amsgrad", "maximize", "decoupled_weight_decay")
+
+
+class FusedAdam(torch.optim.Optimizer):
+    """The optimizer object of a :class:`FusedTrainer` (``trainer.optimizer``): a ``torch.optim.Optimizer`` whose state is
+    the trainer's flat Adam buffers.  It owns no arithmetic — the update runs inside the trainer's step, in
+    ``ddfa_adam_flat_hp`` / ``ddfa_allreduce_adam_p2p_hp`` — and exists so that the usual tools work on a fused run:
+
+    * ``state_dict()`` / ``load_state_dict()`` in ``torch.optim.Adam``'s format, parameters indexed in
+      ``module.parameters()`` order (what ``torch.optim.Adam(module.parameters())`` and a Lightning checkpoint's
+      ``optimizer_states[0]`` use; the flat buffers hold them in ``module.param_list()`` order);
+    * LR schedulers: ``step()`` copies ``param_groups[0]``'s hyperparameters into a 5-float device word that the Adam
+      kernels read when they run, so a captured CUDA graph picks up a new learning rate on its next replay.
+
+    One parameter group; coupled L2 weight decay (``torch.optim.Adam``, not AdamW); no AMSGrad, no ``maximize``.
+    The buffers may live on any device, so the conversion also runs on CPU tensors."""
+
+    def __init__(self, module, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, step_count: torch.Tensor, hyper: torch.Tensor,
+                 lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0, shard=None):
+        """``exp_avg`` / ``exp_avg_sq``: flat fp32 moment buffers laid out by :func:`flat_offsets`; ``step_count``: int32[1];
+        ``hyper``: fp32[5] ``[lr, beta1, beta2, eps, weight_decay]``.  ``shard = (rank, world, process_group)`` when each rank
+        keeps the moments of its :func:`owned_range` only (``exchange="p2p"``)."""
+        params = list(module.parameters())
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, **_ADAM_FLAGS))
+        plist = module.param_list()
+        offs, total = flat_offsets(plist)
+        where = {id(p): o for p, o in zip(plist, offs)}
+        if len(plist) != len(params) or any(id(p) not in where for p in params):
+            raise ValueError("FusedAdam: module.parameters() and module.param_list() hold different tensors")
+        if exp_avg.numel() != total or exp_avg_sq.numel() != total:
+            raise ValueError(f"FusedAdam: moment buffers of {exp_avg.numel()} / {exp_avg_sq.numel()} elements, layout needs {total}")
+        self._slots = [(where[id(p)], p.numel()) for p in params]      # per module.parameters() index: (flat offset, numel)
+        self._flat = (exp_avg, exp_avg_sq, step_count, hyper)
+        self._shard = shard
+        self._pushed = None
+        self._push()
+
+    def _group(self):
+        if len(self.param_groups) != 1:
+            raise ValueError("FusedAdam supports exactly one parameter group")
+        g = self.param_groups[0]
+        bad = [k for k in _UNSUPPORTED if g.get(k)]
+        if bad:
+            raise ValueError(f"FusedAdam: {bad} are not supported (the fused kernels implement torch.optim.Adam with coupled L2)")
+        return g
+
+    def _push(self):
+        """Writes the hyperparameters that changed since the last push into the device word, by value, in stream order
+        (no staging buffer the host could overwrite while the device lags behind)."""
+        g = self._group()
+        vals = (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))
+        hyper = self._flat[3]
+        for i, x in enumerate(vals):
+            if self._pushed is None or self._pushed[i] != x:
+                hyper[i].fill_(x)
+        self._pushed = vals
+
+    def step(self, closure=None):
+        """Hands ``param_groups[0]``'s lr / betas / eps / weight_decay to the kernels of the NEXT trainer step (the trainer
+        calls this at the start of every step; a value is written only when it changed).  Computes nothing itself."""
+        if closure is not None:
+            raise ValueError("FusedAdam.step takes no closure: FusedTrainer.step runs forward and backward")
+        self._push()
+
+    def _gathered(self, t: torch.Tensor) -> torch.Tensor:
+        if self._shard is None:
+            return t
+        rank, world, group = self._shard
+        lo, hi = owned_range(t.numel(), rank, world)
+        out = torch.zeros_like(t)
+        out[lo:hi].copy_(t[lo:hi])
+        dist.all_reduce(out, op=dist.ReduceOp.SUM, group=group)    # every element is nonzero on its owner only: exact
+        return out
+
+    def state_dict(self):
+        """What ``torch.optim.Adam(module.parameters()).state_dict()`` returns after the same steps: per parameter index
+        ``{"step": float32 CPU tensor, "exp_avg", "exp_avg_sq"}`` (copies, shaped like the parameter, on its device) — empty
+        before the first step — and the one parameter group.  Reads the step counter from the device: one synchronisation.
+        With sharded moments (``exchange="p2p"``) this is a collective: every rank must call it, and every rank gets the
+        full state (each rank's owned slice, all-reduced)."""
+        g = self._group()
+        exp_avg, exp_avg_sq, step_count, _ = self._flat
+        step = int(step_count.item())
+        m, v = self._gathered(exp_avg), self._gathered(exp_avg_sq)
+        state = {}
+        if step > 0:
+            for i, (p, (o, n)) in enumerate(zip(g["params"], self._slots)):
+                state[i] = {"step": torch.tensor(float(step), dtype=torch.float32),
+                            "exp_avg": m[o:o + n].view_as(p).clone(), "exp_avg_sq": v[o:o + n].view_as(p).clone()}
+        packed = {k: val for k, val in g.items() if k != "params"}
+        packed["params"] = list(range(len(g["params"])))
+        return {"state": state, "param_groups": [packed]}
+
+    def load_state_dict(self, state_dict):
+        """Loads ``torch.optim.Adam``'s format (from :meth:`state_dict`, ``torch.optim.Adam.state_dict()`` or a Lightning
+        checkpoint's ``optimizer_states[0]``), older forms included: ``step`` as int or tensor, group keys such as
+        ``foreach`` / ``capturable`` / ``fused`` / ``differentiable`` missing; an empty ``state`` means step 0 and zero
+        moments.  Writes IN PLACE into the flat moment buffers, the step counter and the hyperparameter word, so CUDA
+        graphs captured before the load replay from the loaded state.  Every rank loads the full moments, whatever world
+        size wrote them.  Raises ``ValueError`` for more than one group, a parameter count or shape mismatch, AMSGrad,
+        ``maximize``, ``decoupled_weight_decay`` (AdamW) or per-parameter steps that differ."""
+        groups = state_dict.get("param_groups")
+        if not isinstance(groups, (list, tuple)) or len(groups) != 1:
+            raise ValueError(f"FusedAdam loads exactly one parameter group, got {len(groups) if groups is not None else None}")
+        saved = groups[0]
+        bad = [k for k in _UNSUPPORTED if saved.get(k)]
+        if bad:
+            raise ValueError(f"FusedAdam cannot load an optimizer with {bad} set")
+        cur = self._group()["params"]
+        ids = list(saved.get("params", []))
+        if len(ids) != len(cur):
+            raise ValueError(f"checkpoint has {len(ids)} parameters, the module {len(cur)}")
+        state = state_dict.get("state", {})
+        if set(state) - set(ids):
+            raise ValueError(f"state entries {sorted(set(state) - set(ids))} belong to no parameter of the group")
+        steps, entries = set(), []
+        for i, (pid, p) in enumerate(zip(ids, cur)):
+            st = state.get(pid)
+            if st:
+                for key in ("exp_avg", "exp_avg_sq"):
+                    if key not in st or tuple(st[key].shape) != tuple(p.shape):
+                        raise ValueError(f"parameter {i}: {key} of shape {tuple(st[key].shape) if key in st else None}, "
+                                         f"the parameter has {tuple(p.shape)}")
+                s = st.get("step", 0)
+                s = float(s.item()) if torch.is_tensor(s) else float(s)
+                if s != int(s) or not 0 <= s < 2 ** 31:
+                    raise ValueError(f"parameter {i}: step {s} is not a step count")
+                steps.add(int(s))
+                entries.append(st)
+            else:
+                steps.add(0)                          # no state yet: the parameter has never been updated
+                entries.append(None)
+        if len(steps) > 1:
+            raise ValueError(f"per-parameter steps differ ({sorted(steps)}): the fused optimizer keeps one step counter")
+        step = steps.pop() if steps else 0
+        exp_avg, exp_avg_sq, step_count, _ = self._flat
+        with torch.no_grad():
+            exp_avg.zero_()
+            exp_avg_sq.zero_()
+            for (o, n), st in zip(self._slots, entries):
+                if st is not None:
+                    exp_avg[o:o + n].copy_(st["exp_avg"].reshape(-1))
+                    exp_avg_sq[o:o + n].copy_(st["exp_avg_sq"].reshape(-1))
+            step_count.fill_(step)
+        group = self.param_groups[0]
+        group.update({k: val for k, val in saved.items() if k != "params"})
+        self._push()
 
 
 class FusedTrainer:
@@ -44,7 +217,6 @@ class FusedTrainer:
                                       "label_style='node' / encoder_mode modules through module.training_step + torch.optim")
         self.module = module
         self.device = module.device
-        self.lr, self.betas, self.eps, self.weight_decay = lr, betas, eps, weight_decay
         self.pg = process_group
         self.world = dist.get_world_size(process_group) if (distributed and dist.is_available() and dist.is_initialized()) else 1
         self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes = int(bucket_nodes), int(bucket_edges), int(bucket_min_pad_nodes)
@@ -75,10 +247,7 @@ class FusedTrainer:
         self.max_graph_shapes = max_graph_shapes
         self.max_resident_graphs = max_resident_graphs
         plist = module.param_list()
-        offs, total = [], 0
-        for p in plist:
-            offs.append(total)
-            total += (p.numel() + _ALIGN - 1) // _ALIGN * _ALIGN
+        offs, total = flat_offsets(plist)
         self.numel = total
         ntab = len(module._tables())
         self._gemm_grad_range = (offs[ntab], offs[ntab + 4])     # flat offsets of [w_msg, b_msg, w_ih, w_hh]
@@ -106,6 +275,11 @@ class FusedTrainer:
             self.exp_avg = torch.zeros(total, dtype=torch.float32, device=self.device)
             self.exp_avg_sq = torch.zeros(total, dtype=torch.float32, device=self.device)
             self.step_count = torch.zeros(1, dtype=torch.int32, device=self.device)
+            # [lr, beta1, beta2, eps, weight_decay], read by the Adam kernels when they run; written by self.optimizer.step()
+            self.hyper = torch.zeros(5, dtype=torch.float32, device=self.device)
+            shard = (self._p2p_rank, self.world, self.pg) if self.exchange == "p2p" else None
+            self.optimizer = FusedAdam(module, self.exp_avg, self.exp_avg_sq, self.step_count, self.hyper, lr=lr, betas=betas, eps=eps,
+                                       weight_decay=weight_decay, shard=shard)
         gviews = []
         for p, o in zip(plist, offs):
             view = self.flat_p[o:o + p.numel()].view_as(p)
@@ -124,6 +298,40 @@ class FusedTrainer:
         self._stream_slots = {}
         self._copy_stream = None
         self._warm_shapes = set()
+
+    # The Adam hyperparameters live in self.optimizer.param_groups[0], which is what an LR scheduler changes; the next step
+    # (eager or replayed) uses whatever is there when it starts.
+    @property
+    def lr(self):
+        return self.optimizer.param_groups[0]["lr"]
+
+    @lr.setter
+    def lr(self, value):
+        self.optimizer.param_groups[0]["lr"] = value
+
+    @property
+    def betas(self):
+        return self.optimizer.param_groups[0]["betas"]
+
+    @betas.setter
+    def betas(self, value):
+        self.optimizer.param_groups[0]["betas"] = tuple(value)
+
+    @property
+    def eps(self):
+        return self.optimizer.param_groups[0]["eps"]
+
+    @eps.setter
+    def eps(self, value):
+        self.optimizer.param_groups[0]["eps"] = value
+
+    @property
+    def weight_decay(self):
+        return self.optimizer.param_groups[0]["weight_decay"]
+
+    @weight_decay.setter
+    def weight_decay(self, value):
+        self.optimizer.param_groups[0]["weight_decay"] = value
 
     # ------------------------------------------------------------------------------------
     def _setup_p2p(self, total: int):
@@ -170,10 +378,9 @@ class FusedTrainer:
         if self.exchange == "p2p":
             E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws)
             pp, pg_, pf = self._peer_ptrs
-            _lib.lib().call("ddfa_allreduce_adam_p2p", _lib.ptr_array(pp), _lib.ptr_array(pg_), _lib.ptr_array(pf), self._p2p_rank, self.world,
+            _lib.lib().call("ddfa_allreduce_adam_p2p_hp", _lib.ptr_array(pp), _lib.ptr_array(pg_), _lib.ptr_array(pf), self._p2p_rank, self.world,
                             self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.numel,
-                            self.loss_slot.data_ptr(), self._ticket.data_ptr(), self.lr, self.betas[0], self.betas[1], self.eps,
-                            self.weight_decay, torch.cuda.current_stream().cuda_stream)
+                            self.loss_slot.data_ptr(), self._ticket.data_ptr(), self.hyper.data_ptr(), torch.cuda.current_stream().cuda_stream)
             return
         split = self.world > 1 and self.overlap_allreduce
         E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws,
@@ -185,9 +392,9 @@ class FusedTrainer:
         elif self.world > 1:
             dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
         L = _lib.lib()
-        L.call("ddfa_adam_flat", self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
-               self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.lr, self.betas[0], self.betas[1],
-               self.eps, self.weight_decay, torch.cuda.current_stream().cuda_stream)
+        L.call("ddfa_adam_flat_hp", self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
+               self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.hyper.data_ptr(),
+               torch.cuda.current_stream().cuda_stream)
 
     def _reduce_small_grads(self):
         """All-reduce of the embedding / bias / readout / MLP gradients and the loss slot on a side stream (engine.backward
@@ -341,8 +548,9 @@ class FusedTrainer:
         f1: the batch producer).  With ``use_cuda_graph`` the batch is assembled into static per-shape buffers by
         ``ddfa_arena_batch`` inside one captured graph, so a step costs the H2D copy of the id list plus one graph launch;
         otherwise it is ``step(arena.batch(ids))``."""
+        self.optimizer.step()
         if not self.use_cuda_graph:
-            return self.step(arena.batch(ids), global_batch)
+            return self._step_eager(arena.batch(ids), global_batch)
         import numpy as np
         m = self.module
         ids_np = np.asarray(ids.cpu() if isinstance(ids, torch.Tensor) else ids, dtype=np.int64).reshape(-1)
@@ -398,8 +606,9 @@ class FusedTrainer:
 
     def step(self, batch, global_batch: Optional[int] = None) -> torch.Tensor:
         """One optimisation step on this rank's shard.  Returns the device tensor holding the
-        global mean loss (valid after the step's stream work completes)."""
-        m = self.module
+        global mean loss (valid after the step's stream work completes).  Starts with ``self.optimizer.step()``, which hands
+        the current learning rate etc. to this step's Adam launch (an LR scheduler on ``self.optimizer`` sees that call)."""
+        self.optimizer.step()
         if self.use_cuda_graph:
             gb_ = as_batched_cfg(batch)
             if gb_.device.type == "cpu":

@@ -343,6 +343,12 @@ int ddfa_graph_label_bce_valid(const float *logits, const int32_t *vuln, const i
 int ddfa_adam_flat(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
                    int32_t *step_count, int64_t numel, float lr, float beta1, float beta2, float eps,
                    float weight_decay, void *stream);
+/* Same kernel, hyperparameters from device memory: hyper = 5 device floats [lr, beta1, beta2, eps, weight_decay].
+ * The words are read when the kernel RUNS, not when it is enqueued: a launch captured into a CUDA graph uses whatever
+ * the words hold at each replay, so a learning-rate schedule reaches captured steps (write the words in stream order
+ * before the replay).  Equal values give bit-identical parameters and moments to ddfa_adam_flat. */
+int ddfa_adam_flat_hp(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                      int32_t *step_count, int64_t numel, const float *hyper, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K10'  The data-parallel exchange fused with the optimizer over NVLink peer memory: ONE kernel per rank does
@@ -360,6 +366,14 @@ int ddfa_allreduce_adam_p2p(void *const *peer_params, const void *const *peer_gr
                             int32_t rank, int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count,
                             int64_t numel, int64_t loss_offset, float *loss_out, uint32_t *ticket, float lr,
                             float beta1, float beta2, float eps, float weight_decay, void *stream);
+/* Same protocol, hyperparameters from device memory: hyper = 5 LOCAL device floats [lr, beta1, beta2, eps, weight_decay],
+ * read when the kernel runs (as in ddfa_adam_flat_hp: captured launches see later writes).  Every rank must hold the same
+ * values.  The owner of element i is rank floor(i / 4 / per), per = ceil(numel / 4 / world): only the owner reads and
+ * writes exp_avg / exp_avg_sq there. */
+int ddfa_allreduce_adam_p2p_hp(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags,
+                               int32_t rank, int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count,
+                               int64_t numel, int64_t loss_offset, float *loss_out, uint32_t *ticket,
+                               const float *hyper, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Generic row-major fp32 GEMM on the SIMT engine (building block, exported for tests):
