@@ -52,6 +52,8 @@ _SIGNATURES = {
     "ddfa_embed_concat_fwd": (_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_embed_concat_fwd_image": (_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "ddfa_embed_concat_bwd": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "ddfa_embed_concat_bwd_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
+    "ddfa_embed_concat_bwd_ws": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
     "ddfa_gather_sum": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _int, _vp]),
     "ddfa_gather_sum_variant": (_int, [_int, _vp, _vp, _vp, _i32, _i32, _vp, _int, _vp]),
     "ddfa_fold_weights_fwd": (_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp]),
@@ -80,6 +82,8 @@ _SIGNATURES = {
     "ddfa_readout_mlp_fwd": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32] + [_vp] * 6 + [_vp]),
     "ddfa_mlp_bwd": (_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "ddfa_readout_bwd": (_int, [_vp] * 5 + [_i32, _i32] + [_vp] * 8 + [_vp]),
+    "ddfa_readout_bwd_workspace_bytes": (_sz, [_i32, _i32]),
+    "ddfa_readout_bwd_ws": (_int, [_vp] * 5 + [_i32, _i32] + [_vp] * 8 + [_vp, _sz, _vp]),
     "ddfa_graph_label_bce": (_int, [_vp, _vp, _vp, _i32, _f32, _f32, _f32, _vp, _vp, _vp, _vp]),
     "ddfa_graph_label_bce_valid": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, _f32, _f32, _vp, _vp, _vp, _vp]),
     "ddfa_adam_flat": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _vp]),
@@ -90,10 +94,11 @@ _SIGNATURES = {
 }
 
 TUNE_L2_HINTS, TUNE_PDL_MASK, TUNE_GATHER_VARIANT, TUNE_FWD_PAIR, TUNE_GATE_BWD_TMA, TUNE_GATHER_SRC_GROUPS = 0, 1, 2, 3, 4, 5
+TUNE_DETERMINISTIC = 6
 
 _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_version", "ddfa_last_error", "ddfa_device_supported", "ddfa_launch_count", "ddfa_engine_available",
               "ddfa_build_csr_workspace_bytes", "ddfa_arena_batch_workspace_bytes", "ddfa_gru_step_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes_steps",
-              "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes"}
+              "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes"}
 
 
 class _Lib:
@@ -148,6 +153,28 @@ def lib() -> _Lib:
     if _LIB is None:
         _LIB = _Lib()
     return _LIB
+
+
+def deterministic_requested() -> bool:
+    """The mode the Python layer runs in: DDFA_DETERMINISTIC=0|1 when that is set, else torch.are_deterministic_algorithms_enabled()
+    (also True under warn_only=True: every entry point the Python layer calls has a deterministic form, so there is nothing to warn
+    about — only C hosts can reach the entry points that refuse the mode)."""
+    env = os.environ.get("DDFA_DETERMINISTIC")
+    if env is not None:
+        if env not in ("0", "1"):
+            raise DdfaError(f"DDFA_DETERMINISTIC must be 0 or 1, got {env!r}")
+        return env == "1"
+    import torch
+    return bool(torch.are_deterministic_algorithms_enabled())
+
+
+def apply_deterministic_mode() -> bool:
+    """Sets DDFA_TUNE_DETERMINISTIC to the requested mode (only when it differs from the library's) and returns the mode."""
+    want = deterministic_requested()
+    L = lib()
+    if (L.call("ddfa_tuning_get", TUNE_DETERMINISTIC) == 1) != want:
+        L.call("ddfa_tuning_set", TUNE_DETERMINISTIC, int(want))
+    return want
 
 
 def ptr_array(ptrs):

@@ -30,7 +30,9 @@ static std::atomic<int> g_tuning[DDFA_TUNE__COUNT] = {
     {0},    // DDFA_TUNE_FWD_PAIR: reserved, only 0 is accepted (no CTA-pair form of the forward kernel on sm_90a)
     {2},    // DDFA_TUNE_GATE_BWD_TMA: 0 gate_bwd_image + dgrad3; 1 bwd_step_fused_kernel (packed saved state); 2 = 1 + CSR scalars pipelined
     {0},    // DDFA_TUNE_GATHER_SRC_GROUPS: image->image gather, row groups per warp (0 = default = 1; 2 / 4 selectable)
+    {0},    // DDFA_TUNE_DETERMINISTIC: 0 float atomics where they are fastest; 1 every reduction in a fixed order
 };
+bool deterministic() { return g_tuning[DDFA_TUNE_DETERMINISTIC].load(std::memory_order_relaxed) != 0; }
 int l2_hints() { return g_tuning[DDFA_TUNE_L2_HINTS].load(std::memory_order_relaxed); }
 int pdl_mask() { return g_tuning[DDFA_TUNE_PDL_MASK].load(std::memory_order_relaxed); }
 int gather_variant() { return g_tuning[DDFA_TUNE_GATHER_VARIANT].load(std::memory_order_relaxed); }
@@ -60,6 +62,7 @@ int ddfa_engine_available(int engine) {
 int ddfa_tuning_set(int key, int value) {
   DDFA_REQUIRE(key >= 0 && key < DDFA_TUNE__COUNT, "ddfa_tuning_set: unknown key %d", key);
   DDFA_REQUIRE(key != DDFA_TUNE_FWD_PAIR || value == 0, "ddfa_tuning_set: DDFA_TUNE_FWD_PAIR must be 0 (no CTA-pair forward kernel on sm_90a)");
+  DDFA_REQUIRE(key != DDFA_TUNE_DETERMINISTIC || value == 0 || value == 1, "ddfa_tuning_set: DDFA_TUNE_DETERMINISTIC must be 0 or 1 (got %d)", value);
   ddfa::g_tuning[key].store(value, std::memory_order_relaxed);
   return DDFA_OK;
 }

@@ -63,7 +63,8 @@ int pdl_mask();       // abi.cu: DDFA_TUNE_PDL_MASK — bit mask of the kernels 
 int gather_variant(); // abi.cu: DDFA_TUNE_GATHER_VARIANT
 int gather_src_groups();   // abi.cu: DDFA_TUNE_GATHER_SRC_GROUPS — row groups per warp of the image->image gather (0 = by size)
 int gate_bwd_tma();   // abi.cu: DDFA_TUNE_GATE_BWD_TMA — gate backward fused into dgrad (packed saved state)
-void chain_break();   // abi.cu: the next launch_chain() on this thread is a normal (fully serialised) launch
+bool deterministic(); // abi.cu: DDFA_TUNE_DETERMINISTIC — reductions summed in a fixed order (no float atomics)
+void chain_break();  // abi.cu: the next launch_chain() on this thread is a normal (fully serialised) launch
 bool chain_take_break();
 
 // cluster_x > 1: the grid is launched as thread-block clusters of that many CTAs along x
@@ -108,6 +109,15 @@ constexpr int kNumSMs = 132;  // H100 SXM
 // sgemm.cu — SIMT fp32 GEMM, C = alpha*op(A)op(B) + beta*C (row-major)
 int sgemm(int ta, int tb, int M, int N, int K, float alpha, const float *A, int lda, const float *B, int ldb,
           float beta, float *C, int ldc, int split_k, cudaStream_t stream);
+// C[M,N] += alpha * A^T B with K split over split_k slices whose products go to part (sgemm_splitk_ordered_slices(K, split_k) x M x N
+// floats) and are added to C in slice order: the deterministic form of a split-K accumulation
+int sgemm_splitk_ordered_slices(int K, int split_k);
+int sgemm_splitk_ordered(int M, int N, int K, float alpha, const float *A, int lda, const float *B, int ldb, float *C, int ldc,
+                         int split_k, float *part, cudaStream_t stream);
+// csr_build.cu — in-place inclusive scan of a[1..n] (a[0] stays 0) for one or two int32 arrays (a1 may be NULL); s0 / s1 hold
+// the block sums of the multi-CTA form, scan_block_sums_len(n) ints each (NULL: single-CTA form)
+int32_t scan_block_sums_len(int32_t n);
+int scan_counts(int32_t *a0, int32_t *a1, int32_t n, int32_t *s0, int32_t *s1, cudaStream_t stream);
 // gru_tc_fwd3.cu — tensor-core engine, forward (D == 128): activation images
 size_t act_image_bytes(int64_t n);
 int act_to_image(const float *x, int32_t N, void *image, cudaStream_t stream);

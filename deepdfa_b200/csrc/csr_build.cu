@@ -206,6 +206,25 @@ __global__ void graph_ptr_kernel(const int64_t *__restrict__ bnn, int32_t B, int
   }
 }
 
+int32_t scan_block_sums_len(int32_t n) { return (n + kScanBlock - 1) / kScanBlock + 1; }
+
+int scan_counts(int32_t *a0, int32_t *a1, int32_t n, int32_t *s0, int32_t *s1, cudaStream_t stream) {
+  if (n <= 0) return DDFA_OK;
+  const int nb = (n + kScanBlock - 1) / kScanBlock;
+  if (n > 4 * kScanBlock && s0 != nullptr && (a1 == nullptr || s1 != nullptr)) {
+    csr_block_sum_kernel<<<dim3(nb, 2), 256, 0, stream>>>(a0, a1, n, s0, s1);
+    DDFA_CHECK_LAUNCH("csr_block_sum_kernel");
+    csr_scan_kernel<<<2, 1024, 0, stream>>>(a0 ? s0 : nullptr, a1 ? s1 : nullptr, nb);
+    DDFA_CHECK_LAUNCH("csr_scan_kernel(block sums)");
+    csr_block_scan_kernel<<<dim3(nb, 2), 256, 0, stream>>>(a0, a1, n, s0, s1);
+    DDFA_CHECK_LAUNCH("csr_block_scan_kernel");
+  } else {
+    csr_scan_kernel<<<2, 1024, 0, stream>>>(a0, a1, n);
+    DDFA_CHECK_LAUNCH("csr_scan_kernel");
+  }
+  return DDFA_OK;
+}
+
 }  // namespace ddfa
 
 extern "C" {
@@ -247,19 +266,10 @@ int ddfa_build_csr(const void *src, const void *dst, int idx_bytes, int64_t E, i
     DDFA_CHECK_LAUNCH("csr_count_kernel");
   }
   if (N > 0) {
-    const int nb = (N + kScanBlock - 1) / kScanBlock;
     // block sums live in the (not yet used) tmp / tmp_t regions: 1 + nb ints each
-    if (N > 4 * kScanBlock && (int64_t)nb + 1 <= E) {
-      csr_block_sum_kernel<<<dim3(nb, 2), 256, 0, stream>>>(indptr, indptr_t, N, tmp, tmp_t);
-      DDFA_CHECK_LAUNCH("csr_block_sum_kernel");
-      csr_scan_kernel<<<2, 1024, 0, stream>>>(indptr ? tmp : nullptr, indptr_t ? tmp_t : nullptr, nb);
-      DDFA_CHECK_LAUNCH("csr_scan_kernel(block sums)");
-      csr_block_scan_kernel<<<dim3(nb, 2), 256, 0, stream>>>(indptr, indptr_t, N, tmp, tmp_t);
-      DDFA_CHECK_LAUNCH("csr_block_scan_kernel");
-    } else {
-      csr_scan_kernel<<<2, 1024, 0, stream>>>(indptr, indptr_t, N);
-      DDFA_CHECK_LAUNCH("csr_scan_kernel");
-    }
+    const bool multi = (int64_t)scan_block_sums_len(N) <= E;
+    const int rc = scan_counts(indptr, indptr_t, N, multi ? tmp : nullptr, multi ? tmp_t : nullptr, stream);
+    if (rc != DDFA_OK) return rc;
   }
   if (E > 0) {
     const int threads = 256;

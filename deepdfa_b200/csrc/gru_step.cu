@@ -60,13 +60,15 @@ __global__ void __launch_bounds__(256) gru_gate_fwd_kernel(const float *__restri
 
 // ---- gate math, backward -----------------------------------------------------------------
 // dgi, dgh: [N,3D] (inputs of the dgrad/wgrad GEMMs).  dh_part = dh_out * z.
-// Bias grads accumulated with one RED per column per CTA.
+// Bias grads accumulated with one RED per column per CTA, or (bias_slots != NULL, deterministic mode) written to the CTA's slot
+// [7][D] and added in CTA order by bias_slots_sum_kernel.
 constexpr int kGateBwdRows = 128;
 __global__ void __launch_bounds__(256) gru_gate_bwd_kernel(const float *__restrict__ dh_out, const float *__restrict__ h,
                                                            const float *__restrict__ gates, const int32_t *__restrict__ indptr,
                                                            int32_t N, int32_t D, float *__restrict__ dgi, float *__restrict__ dgh,
                                                            float *__restrict__ dh_part, float *__restrict__ db_fold,
-                                                           float *__restrict__ db_ih, float *__restrict__ db_hh) {
+                                                           float *__restrict__ db_ih, float *__restrict__ db_hh,
+                                                           float *__restrict__ bias_slots) {
   extern __shared__ float red[];  // [blockDim.y][7][D]
   const int c = threadIdx.x * 4;
   const int64_t plane = (int64_t)N * D;
@@ -120,12 +122,40 @@ __global__ void __launch_bounds__(256) gru_gate_bwd_kernel(const float *__restri
       for (int y = 1; y < blockDim.y; ++y) f4_add(sum, *reinterpret_cast<const float4 *>(&red[((int64_t)y * 7 + i) * D + c]));
       acc[i] = sum;
     }
+    if (bias_slots) {
+#pragma unroll
+      for (int i = 0; i < 7; ++i) *reinterpret_cast<float4 *>(bias_slots + ((int64_t)blockIdx.x * 7 + i) * D + c) = acc[i];
+      return;
+    }
 #define RED4(ptr, v) atomicAdd((ptr) + 0, (v).x); atomicAdd((ptr) + 1, (v).y); atomicAdd((ptr) + 2, (v).z); atomicAdd((ptr) + 3, (v).w);
     RED4(db_ih + c, acc[0]) RED4(db_ih + D + c, acc[1]) RED4(db_ih + 2 * D + c, acc[2])
     RED4(db_hh + c, acc[0]) RED4(db_hh + D + c, acc[1]) RED4(db_hh + 2 * D + c, acc[3])
     RED4(db_fold + c, acc[4]) RED4(db_fold + D + c, acc[5]) RED4(db_fold + 2 * D + c, acc[6])
 #undef RED4
   }
+}
+
+// one thread per bias-gradient element (7 x D): the CTAs' slots added in CTA order, then into db_ih / db_hh / db_fold as above
+__global__ void __launch_bounds__(256) bias_slots_sum_kernel(const float *__restrict__ slots, int ctas, int32_t D, float *__restrict__ db_fold,
+                                                             float *__restrict__ db_ih, float *__restrict__ db_hh) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 7 * D) return;
+  float v = 0.f;
+  for (int c = 0; c < ctas; ++c) v += slots[(int64_t)c * 7 * D + i];
+  const int which = i / D, col = i - which * D;
+  if (which < 3) db_ih[which * D + col] += v;
+  if (which < 2) db_hh[which * D + col] += v;
+  if (which == 3) db_hh[2 * D + col] += v;
+  if (which >= 4) db_fold[(which - 4) * D + col] += v;
+}
+
+// split of the SIMT weight-gradient GEMMs (K = N nodes) over the SMs
+static int simt_wgrad_split(int32_t N, int32_t D) {
+  const int tiles = ((3 * D + 127) / 128) * ((D + 127) / 128);
+  int split = (2 * kNumSMs + tiles - 1) / tiles;
+  const int k_tiles = (N + 15) / 16;
+  if (split > k_tiles / 8) split = k_tiles / 8 > 0 ? k_tiles / 8 : 1;
+  return split;
 }
 
 // ---- fold helpers --------------------------------------------------------------------------
@@ -311,7 +341,11 @@ size_t ddfa_gru_step_bwd_workspace_bytes(int32_t N, int32_t D, int engine) {
 size_t ddfa_gru_step_bwd_workspace_bytes_steps(int32_t N, int32_t D, int engine, int32_t steps) {
   if (N < 0 || D <= 0) return 0;
   if (engine == DDFA_ENGINE_TCGEN05) return D == 128 ? ddfa::gru_tc2_bwd_workspace_bytes(N, steps) : 16;   // layout: gru_tc_bwd.cu
-  return sizeof(float) * 2 * (size_t)N * 3 * (size_t)D;  // dgi | dgh
+  // dgi | dgh | bias slots of the gate-backward CTAs | split-K slices of one weight gradient (the last two: deterministic mode,
+  // reserved in both modes)
+  const size_t slots = (size_t)((N + ddfa::kGateBwdRows - 1) / ddfa::kGateBwdRows) * 7 * D;
+  const size_t part = (size_t)ddfa::sgemm_splitk_ordered_slices(N, ddfa::simt_wgrad_split(N, D)) * 3 * D * D;
+  return sizeof(float) * (2 * (size_t)N * 3 * (size_t)D + slots + part);
 }
 
 int ddfa_gru_bwd_wgrad_batched(const void *const *s_images, const void *const *h_images, int32_t steps, int32_t N, int32_t D,
@@ -407,21 +441,31 @@ int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const
   }
   float *dgi = static_cast<float *>(workspace);
   float *dgh = dgi + (size_t)N * 3 * D;
+  const bool det = deterministic();
+  const int ctas = (N + kGateBwdRows - 1) / kGateBwdRows;
+  float *bias_slots = dgh + (size_t)N * 3 * D;
+  float *wg_part = bias_slots + (size_t)ctas * 7 * D;
   dim3 block(D / 4, 256 / (D / 4) > 0 ? 256 / (D / 4) : 1);
   const size_t smem = sizeof(float) * block.y * 7 * D;
-  gru_gate_bwd_kernel<<<(N + kGateBwdRows - 1) / kGateBwdRows, block, smem, stream>>>(dh_out, h, gates, indptr, N, D, dgi, dgh, dh,
-                                                                                     db_fold, db_ih, db_hh);
+  gru_gate_bwd_kernel<<<ctas, block, smem, stream>>>(dh_out, h, gates, indptr, N, D, dgi, dgh, dh, db_fold, db_ih, db_hh,
+                                                     det ? bias_slots : nullptr);
   DDFA_CHECK_LAUNCH("gru_gate_bwd_kernel");
+  if (det) {
+    bias_slots_sum_kernel<<<(7 * D + 255) / 256, 256, 0, stream>>>(bias_slots, ctas, D, db_fold, db_ih, db_hh);
+    DDFA_CHECK_LAUNCH("bias_slots_sum_kernel");
+  }
   // ds = dgi @ w_fold ; dh = dh_out*z + dgh @ w_hh
   rc = sgemm(0, 0, N, D, 3 * D, 1.f, dgi, 3 * D, w_fold, D, 0.f, ds, D, 1, stream);
   if (rc) return rc;
   rc = sgemm(0, 0, N, D, 3 * D, 1.f, dgh, 3 * D, w_hh, D, 1.f, dh, D, 1, stream);
   if (rc) return rc;
-  // dw_fold += dgi^T @ s ; dw_hh += dgh^T @ h   (K = N nodes -> split-K over the SMs)
-  const int tiles = ((3 * D + 127) / 128) * ((D + 127) / 128);
-  int split = (2 * kNumSMs + tiles - 1) / tiles;
-  const int k_tiles = (N + 15) / 16;
-  if (split > k_tiles / 8) split = k_tiles / 8 > 0 ? k_tiles / 8 : 1;
+  // dw_fold += dgi^T @ s ; dw_hh += dgh^T @ h   (K = N nodes -> split-K over the SMs; deterministic mode: slices added in order)
+  const int split = simt_wgrad_split(N, D);
+  if (det) {
+    rc = sgemm_splitk_ordered(3 * D, D, N, 1.f, dgi, 3 * D, s, D, dw_fold, D, split, wg_part, stream);
+    if (rc) return rc;
+    return sgemm_splitk_ordered(3 * D, D, N, 1.f, dgh, 3 * D, h, D, dw_hh, D, split, wg_part, stream);
+  }
   rc = sgemm(1, 0, 3 * D, D, N, 1.f, dgi, 3 * D, s, D, 1.f, dw_fold, D, split, stream);
   if (rc) return rc;
   rc = sgemm(1, 0, 3 * D, D, N, 1.f, dgh, 3 * D, h, D, 1.f, dw_hh, D, split, stream);

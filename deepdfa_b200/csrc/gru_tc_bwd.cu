@@ -100,7 +100,8 @@ __global__ void __launch_bounds__(32 * kGbWarps, 2) gate_bwd_image_kernel(const 
                                                                           int32_t N, uint8_t *__restrict__ q_img, size_t img_stride,
                                                                           uint8_t *__restrict__ h_img, float *__restrict__ dhz,
                                                                           float *__restrict__ db_fold,
-                                                                          float *__restrict__ db_ih, float *__restrict__ db_hh, int hints) {
+                                                                          float *__restrict__ db_ih, float *__restrict__ db_hh, float *__restrict__ bias_slots,
+                                                                          int hints) {
   __shared__ float red[kGbWarps][7 * kD];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int col = lane * 4;
@@ -181,6 +182,7 @@ __global__ void __launch_bounds__(32 * kGbWarps, 2) gate_bwd_image_kernel(const 
     float v_ = 0.f;
 #pragma unroll
     for (int w = 0; w < kGbWarps; ++w) v_ += red[w][i];
+    if (bias_slots) { bias_slots[(size_t)blockIdx.x * 7 * kD + i] = v_; continue; }      // deterministic mode: bias_slots_reduce_kernel
     const int which = i >> 7, c_ = i & 127;
     // 0:S(q_r) 1:S(q_z) 2:S(q_n) 3:S(q_nr) 4:S(deg q_r) 5:S(deg q_z) 6:S(deg q_n)
     if (which == 0) { atomicAdd(db_ih + c_, v_); atomicAdd(db_hh + c_, v_); }
@@ -393,7 +395,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
                                                                        int32_t N, uint8_t *__restrict__ q_img, size_t img_stride,
                                                                        const uint8_t *__restrict__ packed3, float *__restrict__ ds, float *__restrict__ dh,
                                                                        float *__restrict__ db_fold, float *__restrict__ db_ih, float *__restrict__ db_hh,
-                                                                       int hints) {
+                                                                       float *__restrict__ bias_slots, int hints) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
@@ -700,6 +702,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
     float v_ = 0.f;
 #pragma unroll
     for (int w = 0; w < kEpiWarps; ++w) v_ += red[(w * 7) * kD + i];
+    if (bias_slots) { bias_slots[(size_t)blockIdx.x * 7 * kD + i] = v_; continue; }      // deterministic mode: bias_slots_reduce_kernel
     const int which = i >> 7, c_ = i & 127;
     // 0:S(q_r) 1:S(q_z) 2:S(q_n) 3:S(q_nr) 4:S(deg q_r) 5:S(deg q_z) 6:S(deg q_n)
     if (which == 0) { atomicAdd(db_ih + c_, v_); atomicAdd(db_hh + c_, v_); }
@@ -851,6 +854,22 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float *__restri
   *dst = d;
 }
 
+// Deterministic mode: the bias-gradient column sums of the step's CTAs (slot c = CTA c, 7 x 128 floats, the order of the epilogues
+// above), added in CTA order — one thread per column.
+constexpr int kBiasSlots = 2 * kNumSMs;      // the largest grid of the step's first kernel (gate_bwd_image_kernel)
+__global__ void __launch_bounds__(128) bias_slots_reduce_kernel(const float *__restrict__ slots, int ctas, float *__restrict__ db_fold,
+                                                                float *__restrict__ db_ih, float *__restrict__ db_hh) {
+  const int i = blockIdx.x * 128 + threadIdx.x;
+  const int which = i >> 7, c_ = i & 127;
+  float v_ = 0.f;
+  for (int c = 0; c < ctas; ++c) v_ += slots[(size_t)c * 7 * kD + i];
+  if (which == 0) { db_ih[c_] += v_; db_hh[c_] += v_; }
+  else if (which == 1) { db_ih[kD + c_] += v_; db_hh[kD + c_] += v_; }
+  else if (which == 2) db_ih[2 * kD + c_] += v_;
+  else if (which == 3) db_hh[2 * kD + c_] += v_;
+  else db_fold[(which - 4) * kD + c_] += v_;
+}
+
 }  // namespace tc2b
 
 // workspace = [dgrad per-slice transposed weight images (384 KB)][q images x4][h image][wgrad partial sums: 2 x 74 x 384 x 128 fp32]
@@ -866,10 +885,11 @@ int gru_tc2b_trace_read(void *host, size_t bytes) {
   return DDFA_OK;
 }
 // workspace: [dgrad3 packed weights 384 KB][h image][dh' * z plane (image-sized)][s image (fp32-s entry only)]
-//            [wgrad partial sums][q images x 4] x slots   (one slot, or one per time step when the weight-gradient GEMM of a
+//            [wgrad partial sums][bias-gradient slots (deterministic mode; reserved in both modes)][q images x 4] x slots   (one slot, or one per time step when the weight-gradient GEMM of a
 //            whole backward pass is batched into one launch)
 static constexpr size_t kPackedTotal = tc2b::kD3PackedBytes;
-static size_t bwd_fixed_bytes(int32_t N) { return kPackedTotal + 3 * tcc::image_bytes(N) + wg_partial_bytes(); }
+static constexpr size_t kBiasSlotBytes = (size_t)tc2b::kBiasSlots * 7 * tcc::kD * sizeof(float);
+static size_t bwd_fixed_bytes(int32_t N) { return kPackedTotal + 3 * tcc::image_bytes(N) + wg_partial_bytes() + kBiasSlotBytes; }
 void *gru_tc2_bwd_s_image_scratch(void *workspace, int32_t N) { return static_cast<uint8_t *>(workspace) + kPackedTotal + 2 * tcc::image_bytes(N); }
 size_t gru_tc2_bwd_workspace_bytes(int32_t N, int32_t slots) {
   return bwd_fixed_bytes(N) + (size_t)(slots < 1 ? 1 : slots) * 4 * tcc::image_bytes(N);
@@ -936,15 +956,20 @@ int gru_tc2b_fused_max_clusters(int *out) { return bwd_fused_max_clusters<false,
 template <bool HF32, bool CSRP>
 static int launch_bwd_fused(int tiles, cudaStream_t stream, const float *dh_out, const float *h, const void *h_img_in, const void *gates_packed,
                             const int32_t *indptr, const float *ds_in, const int32_t *indptr_t, const int32_t *indices_t, int32_t N,
-                            uint8_t *q_img, size_t img, const uint8_t *packed, float *ds, float *dh, float *db_fold, float *db_ih, float *db_hh) {
+                            uint8_t *q_img, size_t img, const uint8_t *packed, float *ds, float *dh, float *db_fold, float *db_ih, float *db_hh,
+                            float *bias_slots, int *ctas) {
   int clusters = 0;
   const int rc = bwd_fused_max_clusters<HF32, CSRP>(&clusters);
   if (rc != DDFA_OK) return rc;
   if (clusters > tiles) clusters = tiles;
+  *ctas = clusters * 4;
+  DDFA_REQUIRE(bias_slots == nullptr || *ctas <= tc2b::kBiasSlots, "tcgen05 engine (bwd): %d CTAs exceed the %d bias-gradient slots",
+               *ctas, tc2b::kBiasSlots);
   DDFA_CUDA(cudaFuncSetAttribute(tc2b::bwd_step_fused_kernel<HF32, CSRP>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
   DDFA_CUDA(launch_chain_cluster(4, 4, tc2b::bwd_step_fused_kernel<HF32, CSRP>, dim3(clusters * 4), dim3(tc2b::kD3Threads), tc2b::kD3SmemAlloc,
                                  stream, dh_out, h, static_cast<const uint8_t *>(h_img_in), static_cast<const uint2 *>(gates_packed), indptr,
-                                 ds_in, ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, l2_hints()));
+                                 ds_in, ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, bias_slots,
+                                 l2_hints()));
   DDFA_CHECK_LAUNCH("tc2b::bwd_step_fused_kernel");
   return DDFA_OK;
 }
@@ -971,6 +996,8 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
   const size_t img = tcc::image_bytes(N);
   uint8_t *h_img_ws = packed + kPackedTotal;
   float *partial = reinterpret_cast<float *>(h_img_ws + 3 * img);
+  float *bias_slots = deterministic() ? reinterpret_cast<float *>(h_img_ws + 3 * img + wg_partial_bytes()) : nullptr;
+  int ctas = 0;      // CTAs of the step's first kernel (one bias slot each)
   uint8_t *q_img = packed + bwd_fixed_bytes(N) + (size_t)q_slot * 4 * img;
   const uint8_t *h_img = h_img_in ? static_cast<const uint8_t *>(h_img_in) : h_img_ws;
   const int tiles = (N + tcc::kTileM - 1) / tcc::kTileM;
@@ -978,21 +1005,22 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
     // packed saved state: gate backward and dgrad in one cluster kernel (dh' * z handed over through the rows of dh)
     const bool csrp = gate_bwd_tma() >= 2;
     int rc = DDFA_OK;
-    if (h) rc = csrp ? launch_bwd_fused<true, true>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh)
-                     : launch_bwd_fused<true, false>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh);
-    else   rc = csrp ? launch_bwd_fused<false, true>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh)
-                     : launch_bwd_fused<false, false>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh);
+    if (h) rc = csrp ? launch_bwd_fused<true, true>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, bias_slots, &ctas)
+                     : launch_bwd_fused<true, false>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, bias_slots, &ctas);
+    else   rc = csrp ? launch_bwd_fused<false, true>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, bias_slots, &ctas)
+                     : launch_bwd_fused<false, false>(tiles, stream, dh_out, h, h_img_in, gates_packed, indptr, ds_in, indptr_t, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, bias_slots, &ctas);
     if (rc != DDFA_OK) return rc;
   } else {
     // register-path gate backward, then dgrad3 (the fp32 saved state, and DDFA_TUNE_GATE_BWD_TMA = 0)
     const int64_t rows = (int64_t)tiles * tcc::kTileM;
     const int64_t want = (rows + tc2b::kGbWarps - 1) / tc2b::kGbWarps;
-    const unsigned gb_grid = (unsigned)(want < 2 * kNumSMs ? want : 2 * kNumSMs);
+    const unsigned gb_grid = (unsigned)(want < tc2b::kBiasSlots ? want : tc2b::kBiasSlots);
+    ctas = (int)gb_grid;
     float *dhz = reinterpret_cast<float *>(h_img_ws + img);
     DDFA_CUDA(launch_chain(4, tc2b::gate_bwd_image_kernel, dim3(gb_grid), dim3(32 * tc2b::kGbWarps), 0, stream, dh_out, h,
                            static_cast<const uint8_t *>(h_img_in), gates, static_cast<const uint4 *>(gates_packed), indptr, ds_in,
                            ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, h_img_in ? nullptr : h_img_ws, dhz, db_fold, db_ih, db_hh,
-                           l2_hints()));
+                           bias_slots, l2_hints()));
     DDFA_CHECK_LAUNCH("tc2b::gate_bwd_image_kernel");
     DDFA_CUDA(cudaFuncSetAttribute(tc2b::dgrad3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
     int groups = kNumSMs / 4;
@@ -1000,6 +1028,10 @@ int gru_tc2_step_bwd(const float *dh_out, const float *ds_in, const int32_t *ind
     DDFA_CUDA(launch_chain(8, tc2b::dgrad3_kernel, dim3(groups * 4), dim3(tc2b::kD3Threads), tc2b::kD3SmemAlloc, stream, q_img, img, dhz,
                            static_cast<const uint8_t *>(packed), N, ds, dh, l2_hints()));
     DDFA_CHECK_LAUNCH("tc2b::dgrad3_kernel");
+  }
+  if (bias_slots) {
+    tc2b::bias_slots_reduce_kernel<<<7, 128, 0, stream>>>(bias_slots, ctas, db_fold, db_ih, db_hh);
+    DDFA_CHECK_LAUNCH("tc2b::bias_slots_reduce_kernel");
   }
   DDFA_CUDA(cudaFuncSetAttribute(tc2b::wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kWgSmemAlloc));
   if (wgrad_mode >= 16) return DDFA_OK;       // q images kept; the batched weight-gradient launch follows the last step

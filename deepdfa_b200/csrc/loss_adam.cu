@@ -53,6 +53,25 @@ __global__ void __launch_bounds__(256) graph_label_bce_kernel(const float *__res
   }
 }
 
+// deterministic mode: the loss as one CTA's sum of the graphs' terms in a fixed order, from the labels graph_label_bce_kernel wrote
+__global__ void __launch_bounds__(256) bce_loss_sum_kernel(const float *__restrict__ logits, const float *__restrict__ labels, int32_t B_valid,
+                                                           float pos_weight, float loss_scale, float *__restrict__ loss_out) {
+  __shared__ float s_t[256];
+  float acc = 0.f;
+  for (int32_t b = threadIdx.x; b < B_valid; b += 256) {
+    const float x = logits[b], y = labels[b];
+    const float lw = 1.f + (pos_weight - 1.f) * y;
+    acc += (1.f - y) * x + lw * (log1pf(expf(-fabsf(x))) + fmaxf(-x, 0.f));
+  }
+  s_t[threadIdx.x] = acc;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) s_t[threadIdx.x] += s_t[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *loss_out = loss_scale * s_t[0];
+}
+
 // hyper: NULL (the by-value lr .. wd are used) or 5 device floats [lr, beta1, beta2, eps, wd] read when the kernel runs, so a
 // captured launch sees values written after the capture.  Either way the update below is the same arithmetic.
 __global__ void __launch_bounds__(256) adam_flat_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
@@ -104,11 +123,17 @@ int ddfa_graph_label_bce_valid(const float *logits, const int32_t *vuln, const i
   if (B == 0) return DDFA_OK;
   DDFA_REQUIRE(vuln && graph_ptr, "ddfa_graph_label_bce: NULL pointer");
   DDFA_REQUIRE(logits || (!loss_out && !dlogits), "ddfa_graph_label_bce: loss requested without logits");
+  const bool det = deterministic() && loss_out != nullptr;      // the loss summed in a second, single-CTA pass over the labels
+  DDFA_REQUIRE(!det || labels, "ddfa_graph_label_bce: in deterministic mode (DDFA_TUNE_DETERMINISTIC = 1) the loss needs the labels output");
   cudaStream_t stream = as_stream(stream_);
   if (loss_out) DDFA_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), stream));
   graph_label_bce_kernel<<<(B + 7) / 8, 256, 0, stream>>>(logits, vuln, graph_ptr, B, B_valid, pos_weight, loss_scale, grad_scale, labels,
-                                                         loss_out, dlogits);
+                                                         det ? nullptr : loss_out, dlogits);
   DDFA_CHECK_LAUNCH("graph_label_bce_kernel");
+  if (det) {
+    bce_loss_sum_kernel<<<1, 256, 0, stream>>>(logits, labels, B_valid, pos_weight, loss_scale, loss_out);
+    DDFA_CHECK_LAUNCH("bce_loss_sum_kernel");
+  }
   return DDFA_OK;
 }
 

@@ -220,7 +220,10 @@ __global__ void __launch_bounds__(kReadoutWarps * 32) readout_bwd_kernel(
     const float *__restrict__ dpooled, const float *__restrict__ pooled, const float *__restrict__ h,
     const float *__restrict__ x, const int32_t *__restrict__ graph_ptr, int32_t D, const float *__restrict__ w_gate,
     const float *__restrict__ gate_logit, const float *__restrict__ seg_max, const float *__restrict__ seg_sum,
-    float *__restrict__ dh, float *__restrict__ dx, float *__restrict__ dw_gate, float *__restrict__ db_gate) {
+    float *__restrict__ dh, float *__restrict__ dx, float *__restrict__ dw_gate, float *__restrict__ db_gate,
+    float *__restrict__ partial) {
+  // partial == NULL: the graph's dw_gate / db_gate terms are added with atomics; else they go to row b of partial [B][2D] and to
+  // partial[B * 2D + b], and the caller sums the rows in graph order (deterministic mode)
   extern __shared__ __align__(16) float sm[];
   const int D2 = 2 * D;
   float *s_dw = sm;  // [warps][2D]
@@ -278,13 +281,15 @@ __global__ void __launch_bounds__(kReadoutWarps * 32) readout_bwd_kernel(
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < kReadoutWarps; ++w) v += s_dw[w * D2 + j];
-    atomicAdd(dw_gate + j, v);
+    if (partial) partial[(int64_t)b * D2 + j] = v;
+    else atomicAdd(dw_gate + j, v);
   }
   if (threadIdx.x == 0) {
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < kReadoutWarps; ++w) v += s_db[w];
-    atomicAdd(db_gate, v);
+    if (partial) partial[(int64_t)gridDim.x * D2 + b] = v;
+    else atomicAdd(db_gate, v);
   }
 }
 
@@ -318,7 +323,7 @@ __global__ void __launch_bounds__(256) mlp_out_kernel(const float *__restrict__ 
 
 // out[n] += sum_m X[m,n]   (one thread per column, coalesced across threads)
 // block = (32 columns) x (8 row partitions); gridDim.y slices the rows (a single row slice owns its columns: plain +=; several
-// slices — long M, e.g. the MLP head's bias gradients over a batch of 1024 — accumulate with RED.ADD)
+// slices — long M, e.g. the MLP head's bias gradients over a batch of 1024 — accumulate with RED.ADD, except in deterministic mode)
 __global__ void __launch_bounds__(256) colsum_accum_kernel(const float *__restrict__ X, int32_t M, int32_t N, float *__restrict__ out) {
   __shared__ float red[8][33];
   const int n = blockIdx.x * 32 + threadIdx.x;
@@ -415,7 +420,7 @@ int ddfa_mlp_bwd(const float *dlogits, const float *pooled, const float *mlp_act
     // dW_i[out,2D] += dOut^T[out,B] @ in[B,2D]
     int rc = sgemm(1, 0, out_dim, D2, B, 1.f, dout, out_dim, in, D2, 1.f, dmlp_w[i], D2, 1, stream);
     if (rc) return rc;
-    colsum_accum_kernel<<<dim3((out_dim + 31) / 32, B >= 256 ? (B + 63) / 64 : 1), dim3(32, 8), 0, stream>>>(dout, B, out_dim, dmlp_b[i]);
+    colsum_accum_kernel<<<dim3((out_dim + 31) / 32, B >= 256 && !deterministic() ? (B + 63) / 64 : 1), dim3(32, 8), 0, stream>>>(dout, B, out_dim, dmlp_b[i]);
     DDFA_CHECK_LAUNCH("colsum_accum_kernel");
     // dIn[B,2D] = dOut[B,out] @ W_i[out,2D]
     float *din = (i == 0) ? dpooled : (dout == buf0 ? buf1 : buf0);
@@ -432,27 +437,64 @@ int ddfa_mlp_bwd(const float *dlogits, const float *pooled, const float *mlp_act
   return DDFA_OK;
 }
 
-int ddfa_readout_bwd(const float *dpooled, const float *pooled, const float *h_final, const float *x,
-                     const int32_t *graph_ptr, int32_t B, int32_t D, const float *w_gate, const float *gate_logit,
-                     const float *seg_max, const float *seg_sum, float *dh_final, float *dx, float *dw_gate,
-                     float *db_gate, void *stream_) {
+size_t ddfa_readout_bwd_workspace_bytes(int32_t B, int32_t D) {
+  if (B < 0 || D < 0) return 0;
+  return sizeof(float) * (size_t)B * (2 * (size_t)D + 1);
+}
+
+static int readout_bwd_impl(const char *who, const float *dpooled, const float *pooled, const float *h_final, const float *x,
+                            const int32_t *graph_ptr, int32_t B, int32_t D, const float *w_gate, const float *gate_logit,
+                            const float *seg_max, const float *seg_sum, float *dh_final, float *dx, float *dw_gate,
+                            float *db_gate, void *workspace, size_t workspace_bytes, bool has_ws, void *stream_) {
   using namespace ddfa;
-  DDFA_REQUIRE(B >= 0 && D > 0 && D % 4 == 0 && D <= 128 * kMaxChunks, "ddfa_readout_bwd: unsupported shape B=%d D=%d", B, D);
+  DDFA_REQUIRE(B >= 0 && D > 0 && D % 4 == 0 && D <= 128 * kMaxChunks, "%s: unsupported shape B=%d D=%d", who, B, D);
+  DDFA_REQUIRE(has_ws || !deterministic(),
+               "ddfa_readout_bwd has no deterministic form (DDFA_TUNE_DETERMINISTIC = 1): use ddfa_readout_bwd_ws");
   if (B == 0) return DDFA_OK;
   DDFA_REQUIRE(dpooled && pooled && h_final && x && graph_ptr && w_gate && gate_logit && seg_max && seg_sum && dh_final && dx && dw_gate && db_gate,
-               "ddfa_readout_bwd: NULL pointer");
+               "%s: NULL pointer", who);
+  float *partial = nullptr;
+  if (deterministic()) {
+    if (workspace == nullptr || workspace_bytes < ddfa_readout_bwd_workspace_bytes(B, D)) {
+      set_error("%s: workspace too small (%zu < %zu)", who, workspace_bytes, ddfa_readout_bwd_workspace_bytes(B, D));
+      return DDFA_ERR_WORKSPACE;
+    }
+    partial = static_cast<float *>(workspace);
+  }
   cudaStream_t stream = as_stream(stream_);
   const size_t smem = sizeof(float) * (size_t)kReadoutWarps * 2 * D;
   const int ch = (D / 4 + 31) / 32;
 #define LAUNCH(CH)                                                                                                    \
   readout_bwd_kernel<CH><<<B, kReadoutWarps * 32, smem, stream>>>(dpooled, pooled, h_final, x, graph_ptr, D, w_gate, gate_logit, \
-                                                                  seg_max, seg_sum, dh_final, dx, dw_gate, db_gate)
+                                                                  seg_max, seg_sum, dh_final, dx, dw_gate, db_gate, partial)
   if (ch == 1) LAUNCH(1);
   else if (ch == 2) LAUNCH(2);
   else LAUNCH(4);
 #undef LAUNCH
   DDFA_CHECK_LAUNCH("readout_bwd_kernel");
+  if (partial) {      // the graphs' terms, added in graph order
+    colsum_accum_kernel<<<dim3((2 * D + 31) / 32, 1), dim3(32, 8), 0, stream>>>(partial, B, 2 * D, dw_gate);
+    DDFA_CHECK_LAUNCH("colsum_accum_kernel");
+    colsum_accum_kernel<<<dim3(1, 1), dim3(32, 8), 0, stream>>>(partial + (size_t)B * 2 * D, B, 1, db_gate);
+    DDFA_CHECK_LAUNCH("colsum_accum_kernel");
+  }
   return DDFA_OK;
+}
+
+int ddfa_readout_bwd(const float *dpooled, const float *pooled, const float *h_final, const float *x,
+                     const int32_t *graph_ptr, int32_t B, int32_t D, const float *w_gate, const float *gate_logit,
+                     const float *seg_max, const float *seg_sum, float *dh_final, float *dx, float *dw_gate,
+                     float *db_gate, void *stream_) {
+  return readout_bwd_impl("ddfa_readout_bwd", dpooled, pooled, h_final, x, graph_ptr, B, D, w_gate, gate_logit, seg_max, seg_sum,
+                          dh_final, dx, dw_gate, db_gate, nullptr, 0, false, stream_);
+}
+
+int ddfa_readout_bwd_ws(const float *dpooled, const float *pooled, const float *h_final, const float *x,
+                        const int32_t *graph_ptr, int32_t B, int32_t D, const float *w_gate, const float *gate_logit,
+                        const float *seg_max, const float *seg_sum, float *dh_final, float *dx, float *dw_gate,
+                        float *db_gate, void *workspace, size_t workspace_bytes, void *stream_) {
+  return readout_bwd_impl("ddfa_readout_bwd_ws", dpooled, pooled, h_final, x, graph_ptr, B, D, w_gate, gate_logit, seg_max, seg_sum,
+                          dh_final, dx, dw_gate, db_gate, workspace, workspace_bytes, true, stream_);
 }
 
 }  // extern "C"

@@ -67,11 +67,14 @@ __device__ __forceinline__ void store_tile(float (*s)[BM + LDS_PAD], const float
   }
 }
 
-template <bool TA, bool TB>
+// ZSLICE: split-K slice z writes its own [M x ldc] block at C + z * M * ldc (deterministic split-K: the slices are added in z
+// order by splitk_reduce_kernel instead of with atomics)
+template <bool TA, bool TB, bool ZSLICE = false>
 __global__ void __launch_bounds__(256) sgemm_kernel(int M, int N, int K, float alpha, const float *__restrict__ A,
                                                     int lda, const float *__restrict__ B, int ldb, float beta,
                                                     float *__restrict__ C, int ldc, int k_per_split, int use_atomic,
                                                     int vec_a, int vec_b) {
+  if constexpr (ZSLICE) C += (int64_t)blockIdx.z * M * ldc;
   __shared__ __align__(16) float As[2][BK][BM + LDS_PAD];
   __shared__ __align__(16) float Bs[2][BK][BN + LDS_PAD];
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
@@ -240,6 +243,43 @@ __global__ void __launch_bounds__(64) sgemm_small_kernel(int M, int N, int K, fl
     }
 }
 
+// C[i] += sum over z of part[z][i], z in order (one thread per element of the dense [M x N] C block)
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float *__restrict__ part, int nz, int M, int N, float *__restrict__ C,
+                                                            int ldc) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)M * N) return;
+  float s = 0.f;
+  for (int z = 0; z < nz; ++z) s += part[(int64_t)z * M * N + i];
+  float *c = C + (i / N) * ldc + i % N;
+  *c += s;
+}
+
+int sgemm_splitk_ordered_slices(int K, int split_k) {
+  const int k_tiles = (K + BK - 1) / BK;
+  if (split_k > k_tiles) split_k = k_tiles > 0 ? k_tiles : 1;
+  if (split_k < 1) split_k = 1;
+  const int kps = ((k_tiles + split_k - 1) / split_k) * BK;
+  return K > 0 ? (K + kps - 1) / kps : 1;
+}
+
+int sgemm_splitk_ordered(int M, int N, int K, float alpha, const float *A, int lda, const float *B, int ldb, float *C, int ldc,
+                         int split_k, float *part, cudaStream_t stream) {
+  if (M == 0 || N == 0 || K == 0) return DDFA_OK;
+  const int k_tiles = (K + BK - 1) / BK;
+  if (split_k > k_tiles) split_k = k_tiles;
+  if (split_k < 1) split_k = 1;
+  const int kps = ((k_tiles + split_k - 1) / split_k) * BK;
+  const int nz = sgemm_splitk_ordered_slices(K, split_k);
+  const int vec_a = aligned16(A) && (lda % 4 == 0), vec_b = aligned16(B) && (ldb % 4 == 0);
+  dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, nz);
+  sgemm_kernel<true, false, true><<<grid, 256, 0, stream>>>(M, N, K, alpha, A, lda, B, ldb, 0.f, part, N, kps, 0, vec_a, vec_b);
+  DDFA_CHECK_LAUNCH("sgemm_kernel(z slices)");
+  const int64_t tot = (int64_t)M * N;
+  splitk_reduce_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(part, nz, M, N, C, ldc);
+  DDFA_CHECK_LAUNCH("splitk_reduce_kernel");
+  return DDFA_OK;
+}
+
 int sgemm(int ta, int tb, int M, int N, int K, float alpha, const float *A, int lda, const float *B, int ldb,
           float beta, float *C, int ldc, int split_k, cudaStream_t stream) {
   if (M == 0 || N == 0) return DDFA_OK;
@@ -247,10 +287,11 @@ int sgemm(int ta, int tb, int M, int N, int K, float alpha, const float *A, int 
   if (split_k == 1 && (int64_t)M * N <= 512 * 512 && K <= 4096) {
     dim3 grid((N + 31) / 32, (M + 31) / 32);
     // An accumulating product (beta == 1) with a long K and few output tiles — the MLP head's weight gradients, K = batch size —
-    // is a chain of K/32 load latencies on a handful of SMs: slice K over gridDim.z and accumulate with RED.ADD instead.
+    // is a chain of K/32 load latencies on a handful of SMs: slice K over gridDim.z and accumulate with RED.ADD instead (not in
+    // deterministic mode: each output element is then one CTA's sum over all of K).
     int split = 1;
     const int tiles = (int)(grid.x * grid.y);
-    if (beta == 1.f && K >= 256 && tiles < kNumSMs) {
+    if (beta == 1.f && K >= 256 && tiles < kNumSMs && !deterministic()) {
       split = (2 * kNumSMs + tiles - 1) / tiles;
       if (split > K / 64) split = K / 64;
       if (split < 1) split = 1;
@@ -273,6 +314,10 @@ int sgemm(int ta, int tb, int M, int N, int K, float alpha, const float *A, int 
   if (split_k > k_tiles) split_k = k_tiles > 0 ? k_tiles : 1;
   const int k_per_split = ((k_tiles + split_k - 1) / split_k) * BK;
   const int use_atomic = split_k > 1;
+  if (use_atomic && deterministic()) {
+    set_error("sgemm: split_k > 1 accumulates with atomics; deterministic mode needs sgemm_splitk_ordered");
+    return DDFA_ERR_UNSUPPORTED;
+  }
   if (use_atomic && beta != 1.f) {
     set_error("ddfa_sgemm: split_k > 1 requires beta == 1 (atomic accumulation into C)");
     return DDFA_ERR_INVALID_ARG;
@@ -301,6 +346,8 @@ extern "C" int ddfa_sgemm(int trans_a, int trans_b, int32_t m, int32_t n, int32_
                           int32_t split_k, void *stream) {
   using namespace ddfa;
   DDFA_REQUIRE(m >= 0 && n >= 0 && k >= 0, "ddfa_sgemm: negative dimension");
+  DDFA_REQUIRE(split_k <= 1 || !deterministic(),
+               "ddfa_sgemm: split_k > 1 has no deterministic form (DDFA_TUNE_DETERMINISTIC = 1): use split_k = 1");
   DDFA_REQUIRE((m == 0 || n == 0) || (a && b && c) || k == 0, "ddfa_sgemm: NULL pointer");
   return sgemm(trans_a, trans_b, m, n, k, alpha, a, lda, b, ldb, beta, c, ldc, split_k, as_stream(stream));
 }

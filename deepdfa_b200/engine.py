@@ -280,6 +280,7 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     """Returns (pooled [B,2D], logits [B] or None, Saved or None)."""
     _require_cuda(*params.flat_list(), dg.indptr, *idx)
     L = _lib.lib()
+    _lib.apply_deterministic_mode()
     dev = dg.device
     alloc = alloc or _FreshAlloc(dev)
     K = len(params.tables)
@@ -390,6 +391,7 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     b_msg, w_ih, w_hh) is final — with the tcgen05 engine that is before the batched weight-gradient launch, so a data-parallel
     trainer can start reducing them while that launch runs."""
     L = _lib.lib()
+    det = _lib.apply_deterministic_mode()
     dev = dg.device
     alloc = alloc or _FreshAlloc(dev)
     K = len(params.tables)
@@ -416,9 +418,11 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     dh = alloc.get("dh_a", (N, D))
     dh_alt = alloc.get("dh_b", (N, D))
     dx_direct = alloc.get("dx_direct", (N, D))
-    _call("ddfa_readout_bwd", _p(dpooled), _p(saved.pooled), _p(saved.h[T]), _p(saved.x), _p(dg.graph_ptr), B, D,
+    ro_bytes = L.call("ddfa_readout_bwd_workspace_bytes", B, D)
+    ro_ws = alloc.get("readout_bwd_ws", (max(ro_bytes, 16),), torch.uint8)
+    _call("ddfa_readout_bwd_ws", _p(dpooled), _p(saved.pooled), _p(saved.h[T]), _p(saved.x), _p(dg.graph_ptr), B, D,
            _p(params.w_gate), _p(saved.gate_logit), _p(saved.seg_max), _p(saved.seg_sum), _p(dh), _p(dx_direct),
-           _p(grads.w_gate), _p(grads.b_gate), st)
+           _p(grads.w_gate), _p(grads.b_gate), _p(ro_ws), ro_bytes, st, tag="ddfa_readout_bwd")
 
     dw_fold = alloc.get("dw_fold", (3 * D, D))
     db_fold = alloc.get("db_fold", (3 * D,))
@@ -453,8 +457,11 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
         dh, dh_alt = dh_alt, dh
     if engine == ENGINE_TCGEN05 and T > 0 and fuse_gather:     # the gather of the last ds (step 0) has no following step to ride on
         _call("ddfa_gather_sum", _p(dg.indptr_t), _p(dg.indices_t), _p(ds_prev), N, D, _p(dh), 1, st, tag="gather_bwd")
-    _call("ddfa_embed_concat_bwd", ptr_array([_p(t) for t in saved.idx]), _p(dh), _p(dx_direct), K, V, H, N,
-           ptr_array([_p(t) for t in grads.tables]), st)
+    # the deterministic form's scratch (sort keys and partial sums): allocated only in that mode, the default form does not read it
+    emb_bytes = L.call("ddfa_embed_concat_bwd_workspace_bytes", K, V, H, N) if det else 0
+    emb_ws = alloc.get("embed_bwd_ws", (emb_bytes,), torch.uint8) if emb_bytes else None
+    _call("ddfa_embed_concat_bwd_ws", ptr_array([_p(t) for t in saved.idx]), _p(dh), _p(dx_direct), K, V, H, N,
+          ptr_array([_p(t) for t in grads.tables]), _p(emb_ws), emb_bytes, st, tag="ddfa_embed_concat_bwd")
     if on_small_grads_ready is not None:
         on_small_grads_ready()
     if engine == ENGINE_TCGEN05 and T > 0:
@@ -472,6 +479,7 @@ def graph_label_bce(dg: DeviceGraph, vuln: torch.Tensor, logits: Optional[torch.
     """Labels (segment max of _VULN) + BCE-with-logits sum (+ dlogits). Returns (labels, loss[1], dlogits).
     ``num_valid``: graphs [num_valid, B) are bucket padding (no loss term, zero gradient)."""
     L = _lib.lib()
+    _lib.apply_deterministic_mode()
     alloc = alloc or _FreshAlloc(dg.device)
     B = dg.batch_size
     labels = alloc.get("labels", (B,))

@@ -426,7 +426,9 @@ class FusedTrainer:
         N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
         gb = self._global_batch(global_batch, B)
         bucket = self._bucket_shape(N, Eg)
-        key = ("bucket", bucket[0], bucket[1], B, gb) if bucket else ("exact", N, Eg, B, gb)
+        # keyed by the deterministic mode too: a captured graph keeps the kernels of the mode it was captured in
+        det = _lib.deterministic_requested()
+        key = ("bucket", bucket[0], bucket[1], B, gb, det) if bucket else ("exact", N, Eg, B, gb, det)
         slot = self._stream_slots.get(key)
         if slot is None:
             if len(self._stream_slots) >= self.max_graph_shapes:
@@ -560,7 +562,7 @@ class FusedTrainer:
         N = int(arena.nodes_per_graph[ids_np].sum())
         Eg = int(arena.edges_per_graph[ids_np].sum())
         gb = self._global_batch(global_batch, B)
-        key = ("arena", id(arena), N, Eg, B, gb)
+        key = ("arena", id(arena), N, Eg, B, gb, _lib.deterministic_requested())
         slot = self._stream_slots.get(key)
         with torch.cuda.device(self.device):
             if slot is None:
@@ -629,23 +631,25 @@ class FusedTrainer:
             vuln = cached
         global_batch = self._global_batch(global_batch, dg.batch_size)
         with torch.cuda.device(self.device):
-            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size)
+            det = _lib.deterministic_requested()
+            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size, det)
+            graph_key = (id(g), det)
             capturable = self.use_cuda_graph and as_batched_cfg(batch).device.type == "cuda" and \
-                (id(g) in self._graphs or len(self._graphs) < self.max_resident_graphs)
+                (graph_key in self._graphs or len(self._graphs) < self.max_resident_graphs)
             if not capturable or shape_key not in self._warm_shapes:
                 # eager step; also the warm-up (workspace growth, lazy CUDA module init) before any capture
                 self._enqueue(g, dg, idx, vuln, global_batch)
                 self._warm_shapes.add(shape_key)
             else:
                 # one captured CUDA graph per resident batch object (its device pointers are baked in)
-                entry = self._graphs.get(id(g))
+                entry = self._graphs.get(graph_key)
                 if entry is None:
                     torch.cuda.synchronize(self.device)
                     cg = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(cg):
                         self._enqueue(g, dg, idx, vuln, global_batch)
                     entry = (cg, g, idx, vuln)     # keep the captured tensors alive
-                    self._graphs[id(g)] = entry
+                    self._graphs[graph_key] = entry
                 entry[0].replay()
         return self.loss_slot
 

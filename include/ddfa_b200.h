@@ -61,7 +61,13 @@ enum {
                                    only path of the fp32 saved state); 1 one cluster kernel: gate backward on TMA-staged dh / gates / h, then dgrad;
                                    2 (default) = 1 + the folded gather's CSR scalars pipelined across tiles */
   DDFA_TUNE_GATHER_SRC_GROUPS = 5, /* image->image edge gather: row groups (of 4 rows) walked per warp with the CSR chain pipelined; 0 (default) = 1 group (2 / 4 measured neutral), or 1 / 2 / 4 */
-  DDFA_TUNE__COUNT = 6
+  DDFA_TUNE_DETERMINISTIC = 6,  /* 0 (default): reductions may add float partial sums with atomics; 1: every reduction adds in a fixed order, so
+                                   two runs with the same inputs, build, GPU model, shapes and tuning give bit-identical results.  Entry points
+                                   without a deterministic form then fail with DDFA_ERR_INVALID_ARG / _UNSUPPORTED and a message naming the
+                                   replacement: ddfa_embed_concat_bwd (use _ws), ddfa_readout_bwd (use _ws), ddfa_sgemm with split_k > 1.  ddfa_graph_label_bce[_valid] then needs
+                                   `labels` whenever it computes the loss.  Like every key it is read when a call ENQUEUES its kernels: a
+                                   captured CUDA graph keeps the kernels of the mode in force at capture time. */
+  DDFA_TUNE__COUNT = 7
 };
 int ddfa_tuning_set(int key, int value);
 int ddfa_tuning_get(int key);
@@ -137,6 +143,13 @@ int ddfa_embed_concat_fwd_image(const int64_t *const *idx, const float *const *t
 int ddfa_embed_concat_bwd(const int64_t *const *idx, const float *dx, const float *dx2,
                           int32_t num_tables, int32_t vocab, int32_t width, int32_t num_nodes,
                           float *const *dtables, void *stream);
+/* Same, with scratch for the deterministic form (DDFA_TUNE_DETERMINISTIC = 1: the nodes are sorted by index with a stable counting
+ * sort and every table row is summed in node order, in fixed chunks).  workspace: ddfa_embed_concat_bwd_workspace_bytes(...)
+ * bytes, 16-byte aligned; unused in the default mode. */
+size_t ddfa_embed_concat_bwd_workspace_bytes(int32_t num_tables, int32_t vocab, int32_t width, int32_t num_nodes);
+int ddfa_embed_concat_bwd_ws(const int64_t *const *idx, const float *dx, const float *dx2,
+                             int32_t num_tables, int32_t vocab, int32_t width, int32_t num_nodes,
+                             float *const *dtables, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K3  CSR edge gather-sum: out[v,:] = (accumulate ? out[v,:] : 0) + sum_{e in row v} h[indices[e],:]
@@ -316,6 +329,14 @@ int ddfa_readout_bwd(const float *dpooled, const float *pooled, const float *h_f
                      const int32_t *graph_ptr, int32_t num_graphs, int32_t dim, const float *w_gate,
                      const float *gate_logit, const float *seg_max, const float *seg_sum,
                      float *dh_final, float *dx, float *dw_gate, float *db_gate, void *stream);
+/* Same, with scratch for the deterministic form (the graphs' dw_gate / db_gate terms added in graph order):
+ * ddfa_readout_bwd_workspace_bytes(B, D) bytes; unused in the default mode. */
+size_t ddfa_readout_bwd_workspace_bytes(int32_t num_graphs, int32_t dim);
+int ddfa_readout_bwd_ws(const float *dpooled, const float *pooled, const float *h_final, const float *x,
+                        const int32_t *graph_ptr, int32_t num_graphs, int32_t dim, const float *w_gate,
+                        const float *gate_logit, const float *seg_max, const float *seg_sum,
+                        float *dh_final, float *dx, float *dw_gate, float *db_gate, void *workspace,
+                        size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K8  graph labels + loss.  Replaces BaseModule.get_label (base_module.py:83-95: dgl.unbatch +
@@ -378,7 +399,7 @@ int ddfa_allreduce_adam_p2p_hp(void *const *peer_params, const void *const *peer
 /* ---------------------------------------------------------------------------------------
  * Generic row-major fp32 GEMM on the SIMT engine (building block, exported for tests):
  *   C[M,N] = alpha * op(A) op(B) + beta * C,  op(X) = X or X^T per trans flag.
- * split_k > 1 accumulates partial products with atomics (requires beta == 1, C pre-initialised).
+ * split_k > 1 accumulates partial products with atomics (requires beta == 1, C pre-initialised; rejected in deterministic mode).
  * ------------------------------------------------------------------------------------- */
 int ddfa_sgemm(int trans_a, int trans_b, int32_t m, int32_t n, int32_t k, float alpha, const float *a,
                int32_t lda, const float *b, int32_t ldb, float beta, float *c, int32_t ldc,
