@@ -197,8 +197,12 @@ class Workspace:
     it reads, so the retired block needs no content).  Growth is geometric (x1.25) to bound the number of retired blocks;
     ``generation`` counts reallocations (tests)."""
 
-    def __init__(self, device):
+    def __init__(self, device, scrub_image_tails: bool = False):
+        """``scrub_image_tails``: clear, on every request, the last tile of each image whose producer leaves padding rows
+        unwritten (``get_image(..., tail_unwritten=True)``).  A trainer that skips non-finite steps and carries on needs this: a
+        skipped step can leave NaN in rows that a later, smaller batch treats as padding."""
         self.device = device
+        self.scrub_image_tails = bool(scrub_image_tails)
         self._bufs = {}
         self._retired = []
         self.generation = 0
@@ -227,11 +231,16 @@ class Workspace:
         """Like get(), but the backing store is zero-filled when it is (re)allocated."""
         return self._get(name, shape, dtype, True)
 
-    def get_image(self, name, nbytes):
-        """An activation image (tile-major, 64 KB per 128-node tile).  Only the padding rows of the last tile are never written
-        by the producing kernel; they are multiplied by zeros in the weight-gradient GEMM, so they must be finite — here the
-        backing store is zero-filled when it is (re)allocated and only ever holds finite values afterwards."""
-        return self._get(name, (nbytes,), torch.uint8, True)
+    def get_image(self, name, nbytes, tail_unwritten: bool = False):
+        """An activation image (tile-major, 64 KB per 128-node tile).  Only the padding rows of the last tile may be left
+        unwritten by the producing kernel (``tail_unwritten``: ddfa_embed_concat_fwd_image; the gathers and the forward GRU step
+        write zeros there); they are multiplied by zeros in the weight-gradient GEMM, so they must be finite — here the
+        backing store is zero-filled when it is (re)allocated, and holds only finite values afterwards as long as every step
+        is finite.  With ``scrub_image_tails`` the last tile of a ``tail_unwritten`` image is also cleared on every request."""
+        buf = self._get(name, (nbytes,), torch.uint8, True)
+        if tail_unwritten and self.scrub_image_tails and nbytes > 0:
+            buf[max(0, nbytes - 65536):].zero_()
+        return buf
 
     def retired_bytes(self) -> int:
         return sum(b.numel() * b.element_size() for b in self._retired)
@@ -249,7 +258,7 @@ class _FreshAlloc:
     def get_zeroed(self, name, shape, dtype=torch.float32):
         return torch.zeros(*shape, dtype=dtype, device=self.device)
 
-    def get_image(self, name, nbytes):
+    def get_image(self, name, nbytes, tail_unwritten: bool = False):
         """A fresh activation image: every row below N is written by the producing kernel, so only the last 64 KB tile (the one
         that can hold padding rows) is cleared — not the whole image (16 images x 78.6 MB per C1 train step otherwise)."""
         buf = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
@@ -297,7 +306,7 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
         # the embedding kernel writes h_0 = x as fp32 rows AND as its activation image (one pass instead of embed + ddfa_act_to_image)
         img_bytes = L.call("ddfa_act_image_bytes", N)
         n_img = T if training else 2          # training keeps the image of every h_t (the weight-gradient GEMM reads it)
-        h_imgs = [alloc.get_image(f"h_img{i}", img_bytes) for i in range(max(n_img, 1))]
+        h_imgs = [alloc.get_image(f"h_img{i}", img_bytes, tail_unwritten=i == 0) for i in range(max(n_img, 1))]
         _call("ddfa_embed_concat_fwd_image", ptr_array([_p(t) for t in idx]), ptr_array([_p(t) for t in params.tables]),
               K, V, H, N, _p(x), _p(h_imgs[0]), _p(oob_counter), st)
     else:

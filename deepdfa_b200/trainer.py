@@ -203,13 +203,21 @@ class FusedTrainer:
     def __init__(self, module: FlowGNNGGNNModule, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 1e-2, process_group=None, use_cuda_graph: bool = False, max_graph_shapes: int = 8,
                  max_resident_graphs: int = 64, distributed: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
-                 bucket_min_pad_nodes: int = 64, overlap_allreduce: bool = True, exchange: str = "auto"):
+                 bucket_min_pad_nodes: int = 64, overlap_allreduce: bool = True, exchange: str = "auto",
+                 max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False):
         """``distributed=False`` makes this a single-rank trainer even inside an initialised process group (no all-reduce).
         ``bucket_nodes`` / ``bucket_edges`` > 0 switch on shape bucketing for HOST batches under ``use_cuda_graph``: every batch
         is padded with ONE dummy graph of isolated nodes up to the next multiple of ``bucket_nodes`` nodes (at least
         ``bucket_min_pad_nodes`` of them, which also carry the padding edges as self loops) and ``bucket_edges`` edges, so that a
         shuffled stream of ever-new ``(N, E)`` (the reference reshuffles every epoch, datamodule.py:123-129) replays a handful of
-        captured graphs.  The dummy graph has zero loss weight (``ddfa_graph_label_bce_valid``): no gradient comes from it."""
+        captured graphs.  The dummy graph has zero loss weight (``ddfa_graph_label_bce_valid``): no gradient comes from it.
+
+        Gradient guard (opt-in; with both arguments at their defaults the step enqueues exactly what it did without them):
+        ``max_grad_norm`` clips the total L2 norm of the exchanged gradients as ``torch.nn.utils.clip_grad_norm_(params,
+        max_grad_norm)`` would, between the exchange and Adam, inside the (captured) step; ``float("inf")`` measures the norm
+        without clipping.  ``skip_nonfinite=True`` makes a step whose norm is not finite leave parameters, moments and the Adam
+        step count bit-unchanged (GradScaler's rule) and count it in ``skipped_steps``.  ``grad_norm`` holds the last step's
+        pre-clip norm; ``max_grad_norm`` can be changed later, also after capture."""
         if module.device.type != "cuda":
             raise _lib.DdfaError("FusedTrainer needs the module on a CUDA device (no CPU fallback)")
         if module.hparams.label_style != "graph" or module.hparams.encoder_mode:
@@ -218,6 +226,9 @@ class FusedTrainer:
         self.module = module
         self.device = module.device
         self.pg = process_group
+        self._guard = max_grad_norm is not None or bool(skip_nonfinite)
+        self.skip_nonfinite = bool(skip_nonfinite)
+        self._max_grad_norm = float("inf") if max_grad_norm is None else self._check_max_norm(max_grad_norm)
         self.world = dist.get_world_size(process_group) if (distributed and dist.is_available() and dist.is_initialized()) else 1
         self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes = int(bucket_nodes), int(bucket_edges), int(bucket_min_pad_nodes)
         # The gradient exchange is split in two: everything except the four GGNN weight matrices' gradients is final before the
@@ -280,6 +291,17 @@ class FusedTrainer:
             shard = (self._p2p_rank, self.world, self.pg) if self.exchange == "p2p" else None
             self.optimizer = FusedAdam(module, self.exp_avg, self.exp_avg_sq, self.step_count, self.hyper, lr=lr, betas=betas, eps=eps,
                                        weight_decay=weight_decay, shard=shard)
+            if self._guard:
+                # the bound (a device word of its own, read when the step runs: not a param_groups key, so state_dict() stays
+                # torch.optim.Adam's), [norm, coef, nonfinite] of the last step, the skip counter and the norm's scratch
+                self._max_norm_dev = torch.full((1,), self._max_grad_norm, dtype=torch.float32, device=self.device)
+                self._gstate = torch.zeros(4, dtype=torch.float32, device=self.device)
+                self._skipped = torch.zeros(1, dtype=torch.int32, device=self.device)
+                L = _lib.lib()
+                if self.exchange == "p2p":
+                    self._guard_ws = torch.zeros(L.call("ddfa_p2p_guard_state_bytes"), dtype=torch.uint8, device=self.device)
+                else:
+                    self._guard_ws = torch.empty(L.call("ddfa_grad_norm_workspace_bytes", total), dtype=torch.uint8, device=self.device)
         gviews = []
         for p, o in zip(plist, offs):
             view = self.flat_p[o:o + p.numel()].view_as(p)
@@ -293,7 +315,9 @@ class FusedTrainer:
         if self.exchange == "p2p":                                # ... and the global loss into a local word (peers read the slot above)
             self._loss_local = self.loss_slot
             self.loss_slot = torch.zeros(1, dtype=torch.float32, device=self.device)
-        self.ws = E.Workspace(self.device)
+        # with the guard a step may go non-finite and the run continues: images whose padding rows a producer leaves unwritten
+        # get their last tile cleared every step, so no NaN of a skipped step can sit in rows a later, smaller batch pads with
+        self.ws = E.Workspace(self.device, scrub_image_tails=self._guard)
         self._graphs = {}
         self._stream_slots = {}
         self._copy_stream = None
@@ -333,6 +357,42 @@ class FusedTrainer:
     def weight_decay(self, value):
         self.optimizer.param_groups[0]["weight_decay"] = value
 
+    # ---- gradient guard ----------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _check_max_norm(value) -> float:
+        v = float(value)
+        if not v >= 0.0:
+            raise ValueError(f"max_grad_norm must be >= 0 (float('inf') measures without clipping), got {value!r}")
+        return v
+
+    @property
+    def max_grad_norm(self) -> Optional[float]:
+        """The clipping bound (``float('inf')``: measure, don't clip); None when the trainer was built without the guard."""
+        return self._max_grad_norm if self._guard else None
+
+    @max_grad_norm.setter
+    def max_grad_norm(self, value):
+        """Written by value into the bound's device word in stream order, so the next step — eager or a replayed graph —
+        uses it.  ``None`` means ``inf``.  Turning the guard on or off is a construction-time choice."""
+        if not self._guard:
+            raise ValueError("this FusedTrainer was built without a gradient guard: pass max_grad_norm= (float('inf') to start "
+                             "unclipped) or skip_nonfinite=True to FusedTrainer(...)")
+        v = float("inf") if value is None else self._check_max_norm(value)
+        if v != self._max_grad_norm:
+            self._max_norm_dev.fill_(v)
+        self._max_grad_norm = v
+
+    @property
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """fp32[1] device tensor: the last step's total gradient L2 norm before clipping (after the data-parallel exchange;
+        ``clip_grad_norm_``'s return value).  Valid once that step's stream work has completed; None without the guard."""
+        return self._gstate[0:1] if self._guard else None
+
+    @property
+    def skipped_steps(self) -> int:
+        """Steps skipped because their gradient norm was not finite (reads the device counter: one synchronisation)."""
+        return int(self._skipped.item()) if self._guard else 0
+
     # ------------------------------------------------------------------------------------
     def _setup_p2p(self, total: int):
         """Symmetric allocations + rendezvous (torch.distributed._symmetric_memory): every rank gets device pointers to every
@@ -342,7 +402,8 @@ class FusedTrainer:
             group = self.pg if self.pg is not None else dist.group.WORLD
             self.flat_p = symm.empty(total, dtype=torch.float32, device=self.device)
             self.flat_g = symm.empty(total + _ALIGN, dtype=torch.float32, device=self.device)
-            self._flags = symm.empty(64, dtype=torch.int32, device=self.device)
+            # 2 * world words for the barriers; the guarded kernel also needs world norm epochs and 16 fp64 slice sums
+            self._flags = symm.empty(128, dtype=torch.int32, device=self.device)      # >= DDFA_P2P_GUARD_FLAG_WORDS
             self.flat_p.zero_(); self.flat_g.zero_(); self._flags.zero_()
             torch.cuda.synchronize(self.device)
             hp, hg, hf = (symm.rendezvous(t, group) for t in (self.flat_p, self.flat_g, self._flags))
@@ -378,6 +439,13 @@ class FusedTrainer:
         if self.exchange == "p2p":
             E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws)
             pp, pg_, pf = self._peer_ptrs
+            if self._guard:
+                _lib.lib().call("ddfa_allreduce_adam_p2p_guarded", _lib.ptr_array(pp), _lib.ptr_array(pg_), _lib.ptr_array(pf), self._p2p_rank,
+                                self.world, self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel,
+                                self.numel, self.loss_slot.data_ptr(), self.hyper.data_ptr(), self._max_norm_dev.data_ptr(),
+                                self._gstate.data_ptr(), self._skipped.data_ptr() if self.skip_nonfinite else None,
+                                self._guard_ws.data_ptr(), torch.cuda.current_stream().cuda_stream)
+                return
             _lib.lib().call("ddfa_allreduce_adam_p2p_hp", _lib.ptr_array(pp), _lib.ptr_array(pg_), _lib.ptr_array(pf), self._p2p_rank, self.world,
                             self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.numel,
                             self.loss_slot.data_ptr(), self._ticket.data_ptr(), self.hyper.data_ptr(), torch.cuda.current_stream().cuda_stream)
@@ -392,6 +460,14 @@ class FusedTrainer:
         elif self.world > 1:
             dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
         L = _lib.lib()
+        if self._guard:      # the norm of the exchanged gradients (both all-reduce halves are in: the wait above), then clipped Adam
+            stream = torch.cuda.current_stream().cuda_stream
+            L.call("ddfa_grad_norm", self.flat_g.data_ptr(), self.numel, self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
+                   self._guard_ws.data_ptr(), self._guard_ws.numel(), stream)
+            L.call("ddfa_adam_flat_guarded", self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
+                   self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.hyper.data_ptr(), self._gstate.data_ptr(),
+                   self._skipped.data_ptr() if self.skip_nonfinite else None, stream)
+            return
         L.call("ddfa_adam_flat_hp", self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
                self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.hyper.data_ptr(),
                torch.cuda.current_stream().cuda_stream)

@@ -397,6 +397,48 @@ int ddfa_allreduce_adam_p2p_hp(void *const *peer_params, const void *const *peer
                                const float *hyper, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Gradient guard: torch.nn.utils.clip_grad_norm_(params, max_norm, norm_type=2) between the gradient exchange and Adam,
+ * and GradScaler's rule for a non-finite step (optimizer.step() is not called), inside the (capturable) optimizer step.
+ *   norm = sqrt(sum g^2): squares summed in fp64 in a fixed order (the same in both DDFA_TUNE_DETERMINISTIC modes), rounded
+ *          once to fp32.  torch sums in fp32 and returns inf once an element exceeds ~1e19; here every finite gradient gives a
+ *          finite norm unless the norm itself exceeds FLT_MAX.
+ *   coef = min(1, max_norm / (norm + 1e-6)) in fp32, as torch computes it; Adam uses g * coef where it used g (before the
+ *          coupled L2 term).  coef == 1 (max_norm = +inf, or a norm below the bound) gives results bit-identical to the
+ *          unguarded entry points.
+ *   skip: with `skipped` != NULL, a step whose norm is not finite writes no parameter, no moment and not the step counter,
+ *          and adds 1 to *skipped (int32 device counter).  With skipped == NULL a non-finite norm is not special: coef is
+ *          then NaN or 0 and flows into the update, as in torch.
+ * gstate: 3 device floats [norm, coef, nonfinite (1.0f / 0.0f)], written by the norm computation.
+ * max_norm: NULL (no clipping) or ONE device float read when the kernel runs, so a captured launch sees later writes; +inf
+ * measures without clipping.
+ * ------------------------------------------------------------------------------------- */
+size_t ddfa_grad_norm_workspace_bytes(int64_t numel);
+/* The norm of grads[0, numel) (a fixed grid of fp64 per-CTA partials, added in CTA order by a second launch) -> gstate.
+ * workspace: ddfa_grad_norm_workspace_bytes(numel) bytes, 8-byte aligned, scratch. */
+int ddfa_grad_norm(const float *grads, int64_t numel, const float *max_norm, float *gstate, void *workspace,
+                   size_t workspace_bytes, void *stream);
+/* ddfa_adam_flat_hp with the clipped gradient g * gstate[1]; skipped as above (the step-counter increment reads the flag too). */
+int ddfa_adam_flat_guarded(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                           int32_t *step_count, int64_t numel, const float *hyper, const float *gstate,
+                           int32_t *skipped, void *stream);
+/* ddfa_allreduce_adam_p2p_hp with the guard.  A rank reduces only its own 1/R slice, so a norm phase sits between the two
+ * barriers: every rank sums the squares of its reduced slice (per-CTA fp64 partials, added in CTA order by the last CTA), writes
+ * that slice sum into every peer's flag area with a release, and every CTA adds the R slice sums in rank order — norm,
+ * coefficient and skip decision are bit-identical on every rank.  A skipped step still sums the loss and runs the second barrier.
+ *   peer_flags: >= DDFA_P2P_GUARD_FLAG_WORDS uint32 per rank (8-byte aligned), zero-initialised once;
+ *   guard_state: ddfa_p2p_guard_state_bytes() LOCAL bytes, 16-byte aligned, zero-initialised once and kept between launches —
+ *   two tickets, the per-CTA partials and the launch counter the barrier epochs come from (a skipped step does not advance
+ *   step_count, so epochs cannot come from it).  The guarded and unguarded forms must not alternate on the same flag words.
+ * gstate is written on every rank.  The step count is incremented by the kernel itself (one launch per step). */
+#define DDFA_P2P_GUARD_FLAG_WORDS 96
+size_t ddfa_p2p_guard_state_bytes(void);
+int ddfa_allreduce_adam_p2p_guarded(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags,
+                                    int32_t rank, int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count,
+                                    int64_t numel, int64_t loss_offset, float *loss_out, const float *hyper,
+                                    const float *max_norm, float *gstate, int32_t *skipped, void *guard_state,
+                                    void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Generic row-major fp32 GEMM on the SIMT engine (building block, exported for tests):
  *   C[M,N] = alpha * op(A) op(B) + beta * C,  op(X) = X or X^T per trans flag.
  * split_k > 1 accumulates partial products with atomics (requires beta == 1, C pre-initialised; rejected in deterministic mode).
