@@ -16,11 +16,26 @@
 //            word — so when the kernel completes, (a) every rank has finished READING this rank's gradients (they may be zeroed for
 //            the next step) and (b) every owner has finished WRITING this rank's parameters (the next forward may read them).
 // The loss (one fp32 per rank after the gradients) is summed by every rank into a local output word.
-// Flags are epochs (step count + 1, identical on all ranks, read from device memory: the launch is CUDA-graph capturable);
-// every wait is bounded and traps instead of hanging the device.
-// ddfa_allreduce_adam_p2p_guarded adds a norm phase for gradient clipping and skipping (below the first kernel).
+// Flags are epochs (identical on all ranks, read from device memory: the launch is CUDA-graph capturable); every wait is bounded
+// and traps instead of hanging the device.
+//
+// ddfa_allreduce_adam_p2p[_hp] and ddfa_allreduce_adam_p2p_guarded run one kernel, allreduce_adam_p2p_kernel<Guarded>.  The
+// guarded form (gradient clipping and skipping of non-finite steps, adam.cuh) differs in four places:
+//   norm     a rank reduces only its own 1/R slice, but the norm needs all of them, so a norm phase sits between phase 1 and the
+//            update: every CTA sums the squares of its part of the reduced slice in fp64 (a fixed tree) into a per-CTA partial;
+//            the last CTA by ticket adds the partials in CTA order and writes the slice sum into EVERY peer's flag area (slot
+//            `rank` of the fp64 words), then releases an epoch word there.  Every CTA waits for the R epoch words and adds the R
+//            slice sums in RANK order, so norm, coefficient and skip decision are bit-identical on every rank.  The update then
+//            reads the peer gradients again (the same rank-order sum) and runs on g * coef; a skipped step writes no parameter
+//            or moment, but still sums the loss and runs phase 2.
+//   epochs   step count + 1 unguarded.  Guarded, the launch counter in GuardState + 1: a skipped step does not advance the step
+//            count, and an epoch that repeats would let the next launch through the barriers unsynchronised.
+//   tickets  the caller's ticket word unguarded; GuardState's two tickets (norm phase, phase 2) guarded.
+//   counters unguarded, a separate 1-thread launch increments the step count; guarded, the last CTA of phase 2 advances the
+//            launch counter and the step or the skip counter (every CTA has read them by then).
+// Flag words per rank: [0, R) phase 1, [R, 2R) phase 2; guarded also [2R, 3R) norm epochs, fp64 slice sums from word kSumWord.
 #include "common.cuh"
-#include "grad_guard.cuh"
+#include "adam.cuh"
 
 namespace ddfa {
 namespace p2p {
@@ -52,86 +67,10 @@ __device__ __forceinline__ void wait_epoch(const uint32_t *p, uint32_t epoch) {
   __trap();
 }
 
-__global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp, int rank, int world, float *__restrict__ m,
-                                                                 float *__restrict__ v, const int32_t *__restrict__ step_count,
-                                                                 int64_t numel, int64_t loss_off, float *__restrict__ loss_out,
-                                                                 uint32_t *__restrict__ ticket, float lr, float beta1, float beta2,
-                                                                 float eps, float wd, const float *__restrict__ hyper) {
-  if (hyper) {      // [lr, beta1, beta2, eps, wd] read at run time (ddfa_allreduce_adam_p2p_hp); same arithmetic as the by-value form
-    lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], wd = hyper[4];
-  }
-  __shared__ float s_c[2];
-  __shared__ int s_last;
-  const int32_t t0 = *step_count;
-  const uint32_t epoch = (uint32_t)t0 + 1u;
-  if (threadIdx.x == 0) {
-    const double t = (double)(t0 + 1);
-    s_c[0] = (float)((double)lr / (1.0 - pow((double)beta1, t)));   // step_size
-    s_c[1] = (float)sqrt(1.0 - pow((double)beta2, t));              // bias_correction2_sqrt
-  }
-  // ---- phase 1
-  __threadfence_system();
-  if (blockIdx.x == 0 && threadIdx.x < world) st_release_sys(pp.flags[threadIdx.x] + rank, epoch);
-  if (threadIdx.x < world) wait_epoch(pp.flags[rank] + threadIdx.x, epoch);
-  __syncthreads();
-  const float step_size = s_c[0], bc2s = s_c[1];
-  // ---- this rank's slice, in 16-byte units (numel is a multiple of 4: the trainer aligns every parameter to 64 elements)
-  const int64_t n4 = numel >> 2;
-  const int64_t per = (n4 + world - 1) / world;
-  const int64_t lo = (int64_t)rank * per, hi = min(n4, lo + per);
-  for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int p = 0; p < world; ++p) f4_add(g, ld_sys_f4(pp.grads[p] + 4 * i));     // rank order: the same sum on every run
-    float4 w = *reinterpret_cast<const float4 *>(pp.params[rank] + 4 * i);
-    float4 mi = *reinterpret_cast<const float4 *>(m + 4 * i), vi = *reinterpret_cast<const float4 *>(v + 4 * i);
-#define DDFA_ADAM1(f)                                        \
-  {                                                          \
-    const float gi = fmaf(wd, w.f, g.f);                     \
-    mi.f = fmaf(beta1, mi.f, (1.f - beta1) * gi);            \
-    vi.f = fmaf(beta2, vi.f, (1.f - beta2) * gi * gi);       \
-    w.f = w.f - step_size * (mi.f / (sqrtf(vi.f) / bc2s + eps)); \
-  }
-    DDFA_ADAM1(x) DDFA_ADAM1(y) DDFA_ADAM1(z) DDFA_ADAM1(w)
-#undef DDFA_ADAM1
-    *reinterpret_cast<float4 *>(m + 4 * i) = mi;
-    *reinterpret_cast<float4 *>(v + 4 * i) = vi;
-    for (int p = 0; p < world; ++p) *reinterpret_cast<float4 *>(pp.params[p] + 4 * i) = w;
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && loss_out) {
-    float s = 0.f;
-    for (int p = 0; p < world; ++p) {
-      float x;
-      asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(x) : "l"(pp.grads[p] + loss_off) : "memory");
-      s += x;
-    }
-    *loss_out = s;
-  }
-  // ---- phase 2
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1) ? 1 : 0;
-  __syncthreads();
-  if (!s_last) return;
-  if (threadIdx.x == 0) *ticket = 0u;
-  __threadfence_system();
-  if (threadIdx.x < world) st_release_sys(pp.flags[threadIdx.x] + world + rank, epoch);
-  if (threadIdx.x < world) wait_epoch(pp.flags[rank] + world + threadIdx.x, epoch);
-}
-
-// ---- guarded form: gradient-norm clipping and skipping of non-finite steps (grad_guard.cuh) ------------------------------------
-// A rank reduces only its own 1/R slice, but the norm needs all of them, so a norm phase sits between phase 1 and the update:
-//   norm     every CTA sums the squares of its part of the reduced slice in fp64 (a fixed tree) into a per-CTA partial; the last CTA
-//            by ticket adds the partials in CTA order and writes the slice sum into EVERY peer's flag area (slot `rank` of the fp64
-//            words), then releases an epoch word there.  Every CTA waits for the R epoch words and adds the R slice sums in RANK
-//            order, so norm, coefficient and skip decision are bit-identical on every rank.
-//   update   the peer gradients are read again (the same rank-order sum) and Adam runs on g * coef; a skipped step writes no
-//            parameter or moment and leaves the step counter alone, but still sums the loss and runs phase 2.
-// Epochs come from the launch counter in GuardState, not from the step count: a skipped step does not advance the step count, and
-// an epoch that repeats would let the next launch through the barriers unsynchronised.
-// Flag words per rank: [0, R) phase 1, [R, 2R) phase 2, [2R, 3R) norm epochs, fp64 slice sums from word kSumWord (8-byte aligned).
+// Flag words per rank as listed above; the fp64 slice sums are 8-byte aligned.
 constexpr int kSumWord = 64, kGuardFlagWords = kSumWord + 2 * kMaxRanks;     // 96 >= 3 * kMaxRanks
 static_assert(kGuardFlagWords == DDFA_P2P_GUARD_FLAG_WORDS && 3 * kMaxRanks <= kSumWord, "guarded flag layout");
-constexpr int kMaxCtas = 64;
+constexpr int kMaxCtas = 64;     // all CTAs must be co-resident: they spin on flags (64 x 256 threads fit any idle H100)
 struct GuardState {
   uint32_t ticket[2];      // norm phase, phase 2: each returns to 0 within the launch
   uint32_t launches;       // launches completed: the next epoch is launches + 1
@@ -148,38 +87,79 @@ __device__ __forceinline__ double ld_relaxed_sys_f64(const uint32_t *p) {
   return v;
 }
 
-__global__ void __launch_bounds__(256) allreduce_adam_p2p_guarded_kernel(const Peers pp, int rank, int world, float *__restrict__ m,
-                                                                         float *__restrict__ v, int32_t *__restrict__ step_count,
-                                                                         int64_t numel, int64_t loss_off, float *__restrict__ loss_out,
-                                                                         GuardState *__restrict__ gs, const float *__restrict__ hyper,
-                                                                         const float *__restrict__ max_norm, float *__restrict__ gstate,
-                                                                         int32_t *__restrict__ skipped) {
-  const float lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], wd = hyper[4];
-  __shared__ float s_c[2];
-  __shared__ double s_red[256];
-  __shared__ float s_coef;
-  __shared__ int s_last, s_skip;
-  const int32_t t0 = *step_count;
-  const uint32_t epoch = *reinterpret_cast<volatile uint32_t *>(&gs->launches) + 1u;
-  if (threadIdx.x == 0) {
-    const double t = (double)(t0 + 1);
-    s_c[0] = (float)((double)lr / (1.0 - pow((double)beta1, t)));   // step_size
-    s_c[1] = (float)sqrt(1.0 - pow((double)beta2, t));              // bias_correction2_sqrt
-  }
-  // ---- phase 1
+// ---- the protocol's steps, shared by both forms of the kernel
+
+// phase 1 "gradients complete": CTA 0 tells every peer, every CTA waits for every peer
+__device__ __forceinline__ void phase1(const Peers &pp, int rank, int world, uint32_t epoch) {
   __threadfence_system();
   if (blockIdx.x == 0 && threadIdx.x < world) st_release_sys(pp.flags[threadIdx.x] + rank, epoch);
   if (threadIdx.x < world) wait_epoch(pp.flags[rank] + threadIdx.x, epoch);
   __syncthreads();
-  const float step_size = s_c[0], bc2s = s_c[1];
-  const int64_t n4 = numel >> 2;
-  const int64_t per = (n4 + world - 1) / world;
-  const int64_t lo = (int64_t)rank * per, hi = min(n4, lo + per);
-  // ---- norm: this CTA's part of the reduced slice
+}
+
+// the reduced gradient of 16-byte unit i, summed in rank order: the same sum on every run and in every pass
+__device__ __forceinline__ float4 reduced_grad(const Peers &pp, int world, int64_t i) {
+  float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int p = 0; p < world; ++p) f4_add(g, ld_sys_f4(pp.grads[p] + 4 * i));
+  return g;
+}
+
+// Adam on this rank's units [lo, hi) (guarded: on g * coef); the new parameters go to every rank
+template <bool Guarded>
+__device__ __forceinline__ void update_slice(const Peers &pp, int rank, int world, float *__restrict__ m, float *__restrict__ v, int64_t lo,
+                                             int64_t hi, const adam::Hyper &h, const adam::Bias &c, float coef) {
+  for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 g = reduced_grad(pp, world, i);
+    if constexpr (Guarded) g = make_float4(g.x * coef, g.y * coef, g.z * coef, g.w * coef);
+    float4 w = *reinterpret_cast<const float4 *>(pp.params[rank] + 4 * i);
+    float4 mi = *reinterpret_cast<const float4 *>(m + 4 * i), vi = *reinterpret_cast<const float4 *>(v + 4 * i);
+    adam::update(g, w, mi, vi, h, c);
+    *reinterpret_cast<float4 *>(m + 4 * i) = mi;
+    *reinterpret_cast<float4 *>(v + 4 * i) = vi;
+    for (int p = 0; p < world; ++p) *reinterpret_cast<float4 *>(pp.params[p] + 4 * i) = w;
+  }
+}
+
+// the loss words of all ranks, added in rank order into the local word
+__device__ __forceinline__ void sum_loss(const Peers &pp, int world, int64_t loss_off, float *loss_out) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && loss_out) {
+    float s = 0.f;
+    for (int p = 0; p < world; ++p) {
+      float x;
+      asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(x) : "l"(pp.grads[p] + loss_off) : "memory");
+      s += x;
+    }
+    *loss_out = s;
+  }
+}
+
+// phase 2 "parameters complete": every CTA but the last by ticket returns; the last resets the ticket, runs last_cta() on thread
+// 0 (every other CTA has finished reading the counters by then), tells every peer and waits for every peer
+template <typename LastCta>
+__device__ __forceinline__ void phase2(const Peers &pp, int rank, int world, uint32_t epoch, uint32_t *ticket, int &s_last,
+                                       LastCta last_cta) {
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1) ? 1 : 0;
+  __syncthreads();
+  if (!s_last) return;
+  if (threadIdx.x == 0) {
+    *ticket = 0u;
+    last_cta();
+  }
+  __threadfence_system();
+  if (threadIdx.x < world) st_release_sys(pp.flags[threadIdx.x] + world + rank, epoch);
+  if (threadIdx.x < world) wait_epoch(pp.flags[rank] + world + threadIdx.x, epoch);
+}
+
+// guarded: the norm of the reduced gradients over all ranks (see the top of the file) -> gstate, *coef, *skip (thread 0)
+__device__ __forceinline__ void norm_phase(const Peers &pp, int rank, int world, uint32_t epoch, int64_t lo, int64_t hi,
+                                          GuardState *__restrict__ gs, const float *__restrict__ max_norm, float *__restrict__ gstate,
+                                          const int32_t *skipped, int &s_last, float *coef, int *skip) {
+  __shared__ double s_red[256];
   double acc = 0.0;
   for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int p = 0; p < world; ++p) f4_add(g, ld_sys_f4(pp.grads[p] + 4 * i));     // rank order, as in the update below
+    const float4 g = reduced_grad(pp, world, i);
     acc += guard::sq(g.x);
     acc += guard::sq(g.y);
     acc += guard::sq(g.z);
@@ -216,98 +196,81 @@ __global__ void __launch_bounds__(256) allreduce_adam_p2p_guarded_kernel(const P
   if (threadIdx.x == 0) {
     double total = 0.0;
     for (int p = 0; p < world; ++p) total += ld_relaxed_sys_f64(pp.flags[rank] + kSumWord + 2 * p);
-    float norm, coef;
+    float norm, c;
     bool nonfinite;
-    guard::finish(total, max_norm, &norm, &coef, &nonfinite);
-    s_coef = coef;
-    s_skip = (skipped != nullptr && nonfinite) ? 1 : 0;
+    guard::finish(total, max_norm, &norm, &c, &nonfinite);
+    *coef = c;
+    *skip = (skipped != nullptr && nonfinite) ? 1 : 0;
     if (blockIdx.x == 0) {
       gstate[guard::kNorm] = norm;
-      gstate[guard::kCoef] = coef;
+      gstate[guard::kCoef] = c;
       gstate[guard::kNonFinite] = nonfinite ? 1.f : 0.f;
     }
   }
   __syncthreads();
-  // ---- update (allreduce_adam_p2p_kernel's arithmetic on g * coef; coef == 1 leaves g bit-unchanged)
-  const float coef = s_coef;
-  if (!s_skip) {
-    for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (int64_t)gridDim.x * blockDim.x) {
-      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int p = 0; p < world; ++p) f4_add(g, ld_sys_f4(pp.grads[p] + 4 * i));
-      float4 w = *reinterpret_cast<const float4 *>(pp.params[rank] + 4 * i);
-      float4 mi = *reinterpret_cast<const float4 *>(m + 4 * i), vi = *reinterpret_cast<const float4 *>(v + 4 * i);
-#define DDFA_ADAM1(f)                                        \
-  {                                                          \
-    const float gi = fmaf(wd, w.f, g.f * coef);              \
-    mi.f = fmaf(beta1, mi.f, (1.f - beta1) * gi);            \
-    vi.f = fmaf(beta2, vi.f, (1.f - beta2) * gi * gi);       \
-    w.f = w.f - step_size * (mi.f / (sqrtf(vi.f) / bc2s + eps)); \
-  }
-      DDFA_ADAM1(x) DDFA_ADAM1(y) DDFA_ADAM1(z) DDFA_ADAM1(w)
-#undef DDFA_ADAM1
-      *reinterpret_cast<float4 *>(m + 4 * i) = mi;
-      *reinterpret_cast<float4 *>(v + 4 * i) = vi;
-      for (int p = 0; p < world; ++p) *reinterpret_cast<float4 *>(pp.params[p] + 4 * i) = w;
-    }
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && loss_out) {
-    float s = 0.f;
-    for (int p = 0; p < world; ++p) {
-      float x;
-      asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(x) : "l"(pp.grads[p] + loss_off) : "memory");
-      s += x;
-    }
-    *loss_out = s;
-  }
-  // ---- phase 2; the last CTA also advances the counters (every CTA has read them by now)
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(&gs->ticket[1], 1u) == gridDim.x - 1) ? 1 : 0;
-  __syncthreads();
-  if (!s_last) return;
-  if (threadIdx.x == 0) {
-    gs->ticket[1] = 0u;
-    gs->launches = epoch;
-    if (s_skip)
-      *skipped += 1;
-    else
-      *step_count = t0 + 1;
-  }
-  __threadfence_system();
-  if (threadIdx.x < world) st_release_sys(pp.flags[threadIdx.x] + world + rank, epoch);
-  if (threadIdx.x < world) wait_epoch(pp.flags[rank] + world + threadIdx.x, epoch);
 }
 
-}  // namespace p2p
-}  // namespace ddfa
+// Unguarded: ticket is the caller's word, gs .. skipped are NULL.  Guarded: ticket is NULL.
+template <bool Guarded>
+__global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp, int rank, int world, float *__restrict__ m,
+                                                                 float *__restrict__ v, int32_t *__restrict__ step_count, int64_t numel,
+                                                                 int64_t loss_off, float *__restrict__ loss_out, uint32_t *__restrict__ ticket,
+                                                                 adam::Hyper h, const float *__restrict__ hyper, GuardState *__restrict__ gs,
+                                                                 const float *__restrict__ max_norm, float *__restrict__ gstate,
+                                                                 int32_t *__restrict__ skipped) {
+  h = adam::load(h, hyper);
+  __shared__ adam::Bias s_c;
+  __shared__ float s_coef;
+  __shared__ int s_last, s_skip;
+  const int32_t t0 = *step_count;
+  const uint32_t epoch = (Guarded ? *reinterpret_cast<volatile uint32_t *>(&gs->launches) : (uint32_t)t0) + 1u;
+  if (threadIdx.x == 0) s_c = adam::bias_correction(h.lr, h.beta1, h.beta2, t0);
+  phase1(pp, rank, world, epoch);
+  const adam::Bias c = s_c;
+  // this rank's slice, in 16-byte units (numel is a multiple of 4: the trainer aligns every parameter to 64 elements)
+  const int64_t n4 = numel >> 2;
+  const int64_t per = (n4 + world - 1) / world;
+  const int64_t lo = (int64_t)rank * per, hi = min(n4, lo + per);
+  if constexpr (Guarded) {
+    norm_phase(pp, rank, world, epoch, lo, hi, gs, max_norm, gstate, skipped, s_last, &s_coef, &s_skip);
+    if (!s_skip) update_slice<true>(pp, rank, world, m, v, lo, hi, h, c, s_coef);
+  } else {
+    update_slice<false>(pp, rank, world, m, v, lo, hi, h, c, 1.f);
+  }
+  sum_loss(pp, world, loss_off, loss_out);
+  if constexpr (Guarded) {
+    phase2(pp, rank, world, epoch, &gs->ticket[1], s_last, [&] {
+      gs->launches = epoch;
+      if (s_skip)
+        *skipped += 1;
+      else
+        *step_count = t0 + 1;
+    });
+  } else {
+    phase2(pp, rank, world, epoch, ticket, s_last, [] {});
+  }
+}
 
-namespace ddfa {
-namespace p2p {
-
-static int fill_peers(Peers &pp, void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int world) {
+// Argument checks (`name` is the entry point), Peers, the grid, the launch.  Unguarded, the step-count increment follows as a
+// launch of its own; guarded, the kernel advances the counters itself.
+template <bool Guarded>
+static int launch(const char *name, void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
+                  int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel, int64_t loss_offset, float *loss_out,
+                  uint32_t *ticket, adam::Hyper h, const float *hyper, void *guard_state, const float *max_norm, float *gstate,
+                  int32_t *skipped, void *stream_) {
+  DDFA_REQUIRE(world >= 1 && world <= kMaxRanks && rank >= 0 && rank < world, "%s: rank %d / world %d (max %d ranks)", name, rank, world,
+               kMaxRanks);
+  DDFA_REQUIRE(numel >= 0 && numel % 4 == 0, "%s: numel (%lld) must be a multiple of 4", name, (long long)numel);
+  DDFA_REQUIRE(peer_params && peer_grads && peer_flags && exp_avg && exp_avg_sq && step_count &&
+                   (Guarded ? hyper && gstate && guard_state : ticket != nullptr),
+               "%s: NULL pointer", name);
+  DDFA_REQUIRE(!Guarded || aligned16(guard_state), "%s: guard_state must be 16-byte aligned", name);
+  Peers pp = {};
   for (int p = 0; p < world; ++p) {
+    // the guarded kernel's fp64 slice sums live in the flag words
     DDFA_REQUIRE(peer_params[p] && peer_grads[p] && peer_flags[p] && aligned16(peer_params[p]) && aligned16(peer_grads[p]) &&
-                     aligned16(peer_flags[p]),
-                 "ddfa_allreduce_adam_p2p_guarded: peer %d pointer NULL or unaligned", p);
-    pp.params[p] = static_cast<float *>(peer_params[p]);
-    pp.grads[p] = static_cast<const float *>(peer_grads[p]);
-    pp.flags[p] = static_cast<uint32_t *>(peer_flags[p]);
-  }
-  return DDFA_OK;
-}
-
-static int launch(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank, int32_t world,
-                  float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel, int64_t loss_offset, float *loss_out,
-                  uint32_t *ticket, float lr, float beta1, float beta2, float eps, float weight_decay, const float *hyper,
-                  void *stream_) {
-  DDFA_REQUIRE(world >= 1 && world <= p2p::kMaxRanks && rank >= 0 && rank < world, "ddfa_allreduce_adam_p2p: rank %d / world %d (max %d ranks)", rank,
-               world, p2p::kMaxRanks);
-  DDFA_REQUIRE(numel >= 0 && numel % 4 == 0, "ddfa_allreduce_adam_p2p: numel (%lld) must be a multiple of 4", (long long)numel);
-  DDFA_REQUIRE(peer_params && peer_grads && peer_flags && exp_avg && exp_avg_sq && step_count && ticket, "ddfa_allreduce_adam_p2p: NULL pointer");
-  p2p::Peers pp = {};
-  for (int p = 0; p < world; ++p) {
-    DDFA_REQUIRE(peer_params[p] && peer_grads[p] && peer_flags[p] && aligned16(peer_params[p]) && aligned16(peer_grads[p]),
-                 "ddfa_allreduce_adam_p2p: peer %d pointer NULL or unaligned", p);
+                     (!Guarded || aligned16(peer_flags[p])),
+                 "%s: peer %d pointer NULL or unaligned", name, p);
     pp.params[p] = static_cast<float *>(peer_params[p]);
     pp.grads[p] = static_cast<const float *>(peer_grads[p]);
     pp.flags[p] = static_cast<uint32_t *>(peer_flags[p]);
@@ -316,11 +279,12 @@ static int launch(void *const *peer_params, const void *const *peer_grads, void 
   const int64_t per = ((numel >> 2) + world - 1) / world;
   int blocks = (int)((per + 255) / 256);
   if (blocks < 1) blocks = 1;
-  if (blocks > 64) blocks = 64;        // all CTAs must be co-resident: they spin on flags (64 x 256 threads fit any idle H100)
-  p2p::allreduce_adam_p2p_kernel<<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out, ticket,
-                                                             lr, beta1, beta2, eps, weight_decay, hyper);
+  if (blocks > kMaxCtas) blocks = kMaxCtas;     // co-resident, and one partial slot each
+  allreduce_adam_p2p_kernel<Guarded><<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out,
+                                                                 ticket, h, hyper, static_cast<GuardState *>(guard_state), max_norm, gstate,
+                                                                 skipped);
   DDFA_CHECK_LAUNCH("allreduce_adam_p2p_kernel");
-  return adam_step_inc_launch(step_count, stream);
+  return Guarded ? DDFA_OK : adam_step_inc_launch(step_count, nullptr, nullptr, stream);
 }
 
 }  // namespace p2p
@@ -330,8 +294,10 @@ extern "C" int ddfa_allreduce_adam_p2p(void *const *peer_params, const void *con
                                        int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
                                        int64_t loss_offset, float *loss_out, uint32_t *ticket, float lr, float beta1, float beta2,
                                        float eps, float weight_decay, void *stream_) {
-  return ddfa::p2p::launch(peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out,
-                           ticket, lr, beta1, beta2, eps, weight_decay, nullptr, stream_);
+  using namespace ddfa;
+  return p2p::launch<false>("ddfa_allreduce_adam_p2p", peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq, step_count,
+                            numel, loss_offset, loss_out, ticket, adam::Hyper{lr, beta1, beta2, eps, weight_decay}, nullptr, nullptr,
+                            nullptr, nullptr, nullptr, stream_);
 }
 
 extern "C" int ddfa_allreduce_adam_p2p_hp(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
@@ -339,8 +305,8 @@ extern "C" int ddfa_allreduce_adam_p2p_hp(void *const *peer_params, const void *
                                           int64_t loss_offset, float *loss_out, uint32_t *ticket, const float *hyper, void *stream_) {
   using namespace ddfa;
   DDFA_REQUIRE(hyper, "ddfa_allreduce_adam_p2p_hp: NULL hyperparameter pointer");
-  return p2p::launch(peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out, ticket,
-                     0.f, 0.f, 0.f, 0.f, 0.f, hyper, stream_);
+  return p2p::launch<false>("ddfa_allreduce_adam_p2p_hp", peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq, step_count,
+                            numel, loss_offset, loss_out, ticket, adam::Hyper{}, hyper, nullptr, nullptr, nullptr, nullptr, stream_);
 }
 
 extern "C" size_t ddfa_p2p_guard_state_bytes(void) { return sizeof(ddfa::p2p::GuardState); }
@@ -351,23 +317,7 @@ extern "C" int ddfa_allreduce_adam_p2p_guarded(void *const *peer_params, const v
                                                const float *max_norm, float *gstate, int32_t *skipped, void *guard_state,
                                                void *stream_) {
   using namespace ddfa;
-  DDFA_REQUIRE(world >= 1 && world <= p2p::kMaxRanks && rank >= 0 && rank < world, "ddfa_allreduce_adam_p2p_guarded: rank %d / world %d (max %d ranks)",
-               rank, world, p2p::kMaxRanks);
-  DDFA_REQUIRE(numel >= 0 && numel % 4 == 0, "ddfa_allreduce_adam_p2p_guarded: numel (%lld) must be a multiple of 4", (long long)numel);
-  DDFA_REQUIRE(peer_params && peer_grads && peer_flags && exp_avg && exp_avg_sq && step_count && hyper && gstate && guard_state,
-               "ddfa_allreduce_adam_p2p_guarded: NULL pointer");
-  DDFA_REQUIRE(aligned16(guard_state), "ddfa_allreduce_adam_p2p_guarded: guard_state must be 16-byte aligned");
-  p2p::Peers pp = {};
-  const int rc = p2p::fill_peers(pp, peer_params, peer_grads, peer_flags, world);
-  if (rc != DDFA_OK) return rc;
-  cudaStream_t stream = as_stream(stream_);
-  const int64_t per = ((numel >> 2) + world - 1) / world;
-  int blocks = (int)((per + 255) / 256);
-  if (blocks < 1) blocks = 1;
-  if (blocks > p2p::kMaxCtas) blocks = p2p::kMaxCtas;     // co-resident (they spin on flags), and one partial slot each
-  p2p::allreduce_adam_p2p_guarded_kernel<<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset,
-                                                                     loss_out, static_cast<p2p::GuardState *>(guard_state), hyper,
-                                                                     max_norm, gstate, skipped);
-  DDFA_CHECK_LAUNCH("allreduce_adam_p2p_guarded_kernel");
-  return DDFA_OK;
+  return p2p::launch<true>("ddfa_allreduce_adam_p2p_guarded", peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq,
+                           step_count, numel, loss_offset, loss_out, nullptr, adam::Hyper{}, hyper, guard_state, max_norm, gstate, skipped,
+                           stream_);
 }

@@ -100,7 +100,8 @@ inline cudaError_t launch_chain(int which, void (*kernel)(KArgs...), dim3 grid, 
   return launch_chain_cluster(which, 1, kernel, grid, block, smem, stream, args...);
 }
 
-int adam_step_inc_launch(int32_t *step_count, cudaStream_t stream);   // loss_adam.cu
+// loss_adam.cu: the 1-thread step-count increment after the Adam update (gstate / skipped: the guard's skip rule, or NULL)
+int adam_step_inc_launch(int32_t *step_count, const float *gstate, int32_t *skipped, cudaStream_t stream);
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 

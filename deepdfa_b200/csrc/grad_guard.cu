@@ -1,9 +1,9 @@
-// Gradient guard for the fused optimizer step: the total L2 norm of the flat gradient buffer, gradient-norm clipping and
-// skipping of non-finite steps (torch.nn.utils.clip_grad_norm_ + GradScaler's skip rule, grad_guard.cuh), as two launches
-// before a guarded form of K10's Adam.  Everything is read from device memory when it runs, so the whole sequence is
-// CUDA-graph capturable and a captured step sees later writes of max_norm.
+// Gradient guard for the fused optimizer step: the total L2 norm of the flat gradient buffer and the clipping coefficient and
+// skip flag derived from it (torch.nn.utils.clip_grad_norm_ + GradScaler's skip rule, adam.cuh), as two launches before the
+// guarded form of K10's Adam (ddfa_adam_flat_guarded, loss_adam.cu), which reads them.  Everything is read from device memory
+// when it runs, so the whole sequence is CUDA-graph capturable and a captured step sees later writes of max_norm.
 #include "common.cuh"
-#include "grad_guard.cuh"
+#include "adam.cuh"
 
 namespace ddfa {
 namespace guard {
@@ -48,46 +48,6 @@ __global__ void sumsq_finish_kernel(const double *__restrict__ partials, const f
   gstate[kNonFinite] = nonfinite ? 1.f : 0.f;
 }
 
-// adam_flat_kernel (loss_adam.cu) with g * coef in place of g.  skipped != NULL and a non-finite norm: the CTA writes nothing.
-// coef == 1 gives g * 1 == g, so the update is then bit-identical to adam_flat_kernel's.
-__global__ void __launch_bounds__(256) adam_flat_guarded_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
-                                                                float *__restrict__ v, const int32_t *__restrict__ step_count, int64_t n,
-                                                                const float *__restrict__ hyper, const float *__restrict__ gstate,
-                                                                const int32_t *__restrict__ skipped) {
-  if (skipped && gstate[kNonFinite] != 0.f) return;
-  const float lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], wd = hyper[4];
-  const float coef = gstate[kCoef];
-  __shared__ float s_c[2];
-  if (threadIdx.x == 0) {
-    const double t = (double)(*step_count + 1);
-    const double bc1 = 1.0 - pow((double)beta1, t);
-    const double bc2 = 1.0 - pow((double)beta2, t);
-    s_c[0] = (float)((double)lr / bc1);   // step_size
-    s_c[1] = (float)sqrt(bc2);            // bias_correction2_sqrt
-  }
-  __syncthreads();
-  const float step_size = s_c[0], bc2s = s_c[1];
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float gi = g[i] * coef;                              // clip_grad_norm_: grad.mul_(clip_coef_clamped)
-  const float pi = p[i];
-  gi = fmaf(wd, pi, gi);                               // grad = grad + wd * param  (coupled L2)
-  const float mi = fmaf(beta1, m[i], (1.f - beta1) * gi);  // exp_avg.lerp_(grad, 1-beta1)
-  const float vi = fmaf(beta2, v[i], (1.f - beta2) * gi * gi);
-  m[i] = mi;
-  v[i] = vi;
-  const float denom = sqrtf(vi) / bc2s + eps;
-  p[i] = pi - step_size * (mi / denom);
-}
-
-// a skipped step leaves the Adam step counter alone (torch counts the optimizer.step() calls that happened) and counts the skip
-__global__ void adam_step_inc_guarded_kernel(int32_t *step_count, const float *gstate, int32_t *skipped) {
-  if (skipped && gstate[kNonFinite] != 0.f)
-    *skipped += 1;
-  else
-    *step_count += 1;
-}
-
 }  // namespace guard
 }  // namespace ddfa
 
@@ -113,22 +73,6 @@ int ddfa_grad_norm(const float *grads, int64_t numel, const float *max_norm, flo
   DDFA_CHECK_LAUNCH("sumsq_partials_kernel");
   guard::sumsq_finish_kernel<<<1, 1, 0, stream>>>(partials, max_norm, gstate);
   DDFA_CHECK_LAUNCH("sumsq_finish_kernel");
-  return DDFA_OK;
-}
-
-int ddfa_adam_flat_guarded(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
-                           const float *hyper, const float *gstate, int32_t *skipped, void *stream_) {
-  using namespace ddfa;
-  DDFA_REQUIRE(numel >= 0, "ddfa_adam_flat_guarded: negative numel");
-  DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && hyper && gstate, "ddfa_adam_flat_guarded: NULL pointer");
-  cudaStream_t stream = as_stream(stream_);
-  if (numel > 0) {
-    guard::adam_flat_guarded_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count,
-                                                                                        numel, hyper, gstate, skipped);
-    DDFA_CHECK_LAUNCH("adam_flat_guarded_kernel");
-  }
-  guard::adam_step_inc_guarded_kernel<<<1, 1, 0, stream>>>(step_count, gstate, skipped);
-  DDFA_CHECK_LAUNCH("adam_step_inc_guarded_kernel");
   return DDFA_OK;
 }
 

@@ -3,10 +3,13 @@
 // K8 replaces BaseModule.get_label (base_module.py:83-95: dgl.unbatch + a Python loop taking
 // max(_VULN) per graph) and torch.nn.BCEWithLogitsLoss(pos_weight) (base_module.py:72-74,183).
 // K10 replaces torch.optim.Adam(lr=1e-3, weight_decay=1e-2) — coupled L2, not AdamW
-// (DDFA/configs/config_default.yaml:43-47) — over one flat parameter buffer.
+// (DDFA/configs/config_default.yaml:43-47) — over one flat parameter buffer, with the hyperparameters by value
+// (ddfa_adam_flat) or from a device word (ddfa_adam_flat_hp); ddfa_adam_flat_guarded is the same update on the clipped
+// gradient, after ddfa_grad_norm (grad_guard.cu).  The arithmetic is adam.cuh's.
 #include <math.h>
 
 #include "common.cuh"
+#include "adam.cuh"
 
 namespace ddfa {
 
@@ -72,43 +75,57 @@ __global__ void __launch_bounds__(256) bce_loss_sum_kernel(const float *__restri
   if (threadIdx.x == 0) *loss_out = loss_scale * s_t[0];
 }
 
-// hyper: NULL (the by-value lr .. wd are used) or 5 device floats [lr, beta1, beta2, eps, wd] read when the kernel runs, so a
-// captured launch sees values written after the capture.  Either way the update below is the same arithmetic.
+// Guarded: Adam on g * gstate[kCoef] (grad_guard.cu computed it); with skipped != NULL and a non-finite norm the CTA writes nothing.
+template <bool Guarded>
 __global__ void __launch_bounds__(256) adam_flat_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
                                                         float *__restrict__ v, const int32_t *__restrict__ step_count, int64_t n,
-                                                        float lr, float beta1, float beta2, float eps, float wd,
-                                                        const float *__restrict__ hyper) {
-  if (hyper) {
-    lr = hyper[0], beta1 = hyper[1], beta2 = hyper[2], eps = hyper[3], wd = hyper[4];
+                                                        adam::Hyper h, const float *__restrict__ hyper, const float *__restrict__ gstate,
+                                                        const int32_t *__restrict__ skipped) {
+  if constexpr (Guarded) {
+    if (skipped && gstate[guard::kNonFinite] != 0.f) return;
   }
-  __shared__ float s_c[2];
-  if (threadIdx.x == 0) {
-    const double t = (double)(*step_count + 1);
-    const double bc1 = 1.0 - pow((double)beta1, t);
-    const double bc2 = 1.0 - pow((double)beta2, t);
-    s_c[0] = (float)((double)lr / bc1);   // step_size
-    s_c[1] = (float)sqrt(bc2);            // bias_correction2_sqrt
-  }
+  h = adam::load(h, hyper);
+  __shared__ adam::Bias s_c;
+  if (threadIdx.x == 0) s_c = adam::bias_correction(h.lr, h.beta1, h.beta2, *step_count);
   __syncthreads();
-  const float step_size = s_c[0], bc2s = s_c[1];
+  const adam::Bias c = s_c;
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   float gi = g[i];
-  const float pi = p[i];
-  gi = fmaf(wd, pi, gi);                               // grad = grad + wd * param  (coupled L2)
-  const float mi = fmaf(beta1, m[i], (1.f - beta1) * gi);  // exp_avg.lerp_(grad, 1-beta1)
-  const float vi = fmaf(beta2, v[i], (1.f - beta2) * gi * gi);
+  if constexpr (Guarded) gi = gi * gstate[guard::kCoef];     // clip_grad_norm_: grad.mul_(clip_coef_clamped)
+  float pi = p[i], mi = m[i], vi = v[i];
+  adam::update(gi, pi, mi, vi, h, c);
   m[i] = mi;
   v[i] = vi;
-  const float denom = sqrtf(vi) / bc2s + eps;
-  p[i] = pi - step_size * (mi / denom);
+  p[i] = pi;
 }
-__global__ void adam_step_inc_kernel(int32_t *step_count) { *step_count += 1; }
 
-int adam_step_inc_launch(int32_t *step_count, cudaStream_t stream) {
-  adam_step_inc_kernel<<<1, 1, 0, stream>>>(step_count);
+// gstate == NULL: the step.  Otherwise, with skipped != NULL and a non-finite norm, the skip counter instead: a skipped step
+// leaves the Adam step count alone (torch counts the optimizer.step() calls that happened).
+__global__ void adam_step_inc_kernel(int32_t *step_count, const float *gstate, int32_t *skipped) {
+  if (gstate && skipped && gstate[guard::kNonFinite] != 0.f)
+    *skipped += 1;
+  else
+    *step_count += 1;
+}
+
+int adam_step_inc_launch(int32_t *step_count, const float *gstate, int32_t *skipped, cudaStream_t stream) {
+  adam_step_inc_kernel<<<1, 1, 0, stream>>>(step_count, gstate, skipped);
   DDFA_CHECK_LAUNCH("adam_step_inc_kernel");
   return DDFA_OK;
+}
+
+// the flat update and its step-count increment: two launches (none for the update when numel == 0)
+template <bool Guarded>
+static int adam_flat_launch(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                            adam::Hyper h, const float *hyper, const float *gstate, int32_t *skipped, void *stream_) {
+  cudaStream_t stream = as_stream(stream_);
+  if (numel > 0) {
+    adam_flat_kernel<Guarded><<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel,
+                                                                                  h, hyper, gstate, skipped);
+    DDFA_CHECK_LAUNCH("adam_flat_kernel");
+  }
+  return adam_step_inc_launch(step_count, gstate, skipped, stream);
 }
 
 }  // namespace ddfa
@@ -147,13 +164,8 @@ int ddfa_adam_flat(float *params, const float *grads, float *exp_avg, float *exp
   using namespace ddfa;
   DDFA_REQUIRE(numel >= 0, "ddfa_adam_flat: negative numel");
   DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count, "ddfa_adam_flat: NULL pointer");
-  cudaStream_t stream = as_stream(stream_);
-  if (numel > 0) {
-    adam_flat_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel, lr,
-                                                                         beta1, beta2, eps, weight_decay, nullptr);
-    DDFA_CHECK_LAUNCH("adam_flat_kernel");
-  }
-  return adam_step_inc_launch(step_count, stream);
+  return adam_flat_launch<false>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{lr, beta1, beta2, eps, weight_decay},
+                                 nullptr, nullptr, nullptr, stream_);
 }
 
 int ddfa_adam_flat_hp(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
@@ -161,13 +173,15 @@ int ddfa_adam_flat_hp(float *params, const float *grads, float *exp_avg, float *
   using namespace ddfa;
   DDFA_REQUIRE(numel >= 0, "ddfa_adam_flat_hp: negative numel");
   DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && hyper, "ddfa_adam_flat_hp: NULL pointer");
-  cudaStream_t stream = as_stream(stream_);
-  if (numel > 0) {
-    adam_flat_kernel<<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel, 0.f,
-                                                                         0.f, 0.f, 0.f, 0.f, hyper);
-    DDFA_CHECK_LAUNCH("adam_flat_kernel");
-  }
-  return adam_step_inc_launch(step_count, stream);
+  return adam_flat_launch<false>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{}, hyper, nullptr, nullptr, stream_);
+}
+
+int ddfa_adam_flat_guarded(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                           const float *hyper, const float *gstate, int32_t *skipped, void *stream_) {
+  using namespace ddfa;
+  DDFA_REQUIRE(numel >= 0, "ddfa_adam_flat_guarded: negative numel");
+  DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && hyper && gstate, "ddfa_adam_flat_guarded: NULL pointer");
+  return adam_flat_launch<true>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{}, hyper, gstate, skipped, stream_);
 }
 
 }  // extern "C"

@@ -199,6 +199,16 @@ class FusedAdam(torch.optim.Optimizer):
         self._push()
 
 
+def _group_property(key, convert=None):
+    """A :class:`FusedTrainer` attribute that reads and writes ``optimizer.param_groups[0][key]``."""
+    def get(self):
+        return self.optimizer.param_groups[0][key]
+
+    def set(self, value):
+        self.optimizer.param_groups[0][key] = value if convert is None else convert(value)
+    return property(get, set)
+
+
 class FusedTrainer:
     def __init__(self, module: FlowGNNGGNNModule, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 1e-2, process_group=None, use_cuda_graph: bool = False, max_graph_shapes: int = 8,
@@ -318,6 +328,7 @@ class FusedTrainer:
         # with the guard a step may go non-finite and the run continues: images whose padding rows a producer leaves unwritten
         # get their last tile cleared every step, so no NaN of a skipped step can sit in rows a later, smaller batch pads with
         self.ws = E.Workspace(self.device, scrub_image_tails=self._guard)
+        self._update = self._update_calls()
         self._graphs = {}
         self._stream_slots = {}
         self._copy_stream = None
@@ -325,37 +336,10 @@ class FusedTrainer:
 
     # The Adam hyperparameters live in self.optimizer.param_groups[0], which is what an LR scheduler changes; the next step
     # (eager or replayed) uses whatever is there when it starts.
-    @property
-    def lr(self):
-        return self.optimizer.param_groups[0]["lr"]
-
-    @lr.setter
-    def lr(self, value):
-        self.optimizer.param_groups[0]["lr"] = value
-
-    @property
-    def betas(self):
-        return self.optimizer.param_groups[0]["betas"]
-
-    @betas.setter
-    def betas(self, value):
-        self.optimizer.param_groups[0]["betas"] = tuple(value)
-
-    @property
-    def eps(self):
-        return self.optimizer.param_groups[0]["eps"]
-
-    @eps.setter
-    def eps(self, value):
-        self.optimizer.param_groups[0]["eps"] = value
-
-    @property
-    def weight_decay(self):
-        return self.optimizer.param_groups[0]["weight_decay"]
-
-    @weight_decay.setter
-    def weight_decay(self, value):
-        self.optimizer.param_groups[0]["weight_decay"] = value
+    lr = _group_property("lr")
+    betas = _group_property("betas", tuple)
+    eps = _group_property("eps")
+    weight_decay = _group_property("weight_decay")
 
     # ---- gradient guard ----------------------------------------------------------------------------------------------------
     @staticmethod
@@ -417,6 +401,26 @@ class FusedTrainer:
         self._ticket = torch.zeros(1, dtype=torch.int32, device=self.device)
         dist.barrier(group)            # every rank's flag words are zero before anyone's first kernel can write one
 
+    def _update_calls(self):
+        """``[(entry point, arguments but the stream)]``: the optimizer update that ends every step.  None of its buffers ever
+        moves (``load_state_dict`` writes in place), so the calls are fixed when the trainer is built.  With the guard and
+        without peer memory, the norm of the exchanged gradients comes first."""
+        skipped = self._skipped.data_ptr() if self.skip_nonfinite else None      # skip_nonfinite implies the guard
+        adam = (self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr())
+        if self.exchange == "p2p":
+            self._peer_arrays = tuple(_lib.ptr_array(p) for p in self._peer_ptrs)      # host arrays the calls point into
+            head = (*self._peer_arrays, self._p2p_rank, self.world, *adam, self.numel, self.numel, self.loss_slot.data_ptr())
+            if self._guard:
+                return [("ddfa_allreduce_adam_p2p_guarded", head + (self.hyper.data_ptr(), self._max_norm_dev.data_ptr(),
+                                                                    self._gstate.data_ptr(), skipped, self._guard_ws.data_ptr()))]
+            return [("ddfa_allreduce_adam_p2p_hp", head + (self._ticket.data_ptr(), self.hyper.data_ptr()))]
+        flat = (self.flat_p.data_ptr(), self.flat_g.data_ptr(), *adam, self.numel, self.hyper.data_ptr())
+        if self._guard:
+            return [("ddfa_grad_norm", (self.flat_g.data_ptr(), self.numel, self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
+                                        self._guard_ws.data_ptr(), self._guard_ws.numel())),
+                    ("ddfa_adam_flat_guarded", flat + (self._gstate.data_ptr(), skipped))]
+        return [("ddfa_adam_flat_hp", flat)]
+
     def _global_batch(self, global_batch: Optional[int], local_graphs: int) -> int:
         """The divisor of the mean BCE (base_module.py:74,183).  Ranks generally hold different numbers of graphs
         (batched_graph.split_batch balances by nodes), so with more than one rank the caller must say what the global batch is."""
@@ -436,41 +440,21 @@ class FusedTrainer:
         _, _, dlogits = E.graph_label_bce(dg, vuln, logits, pw, 1.0 / global_batch, 1.0 / global_batch, True,
                                           alloc=self.ws, loss_out=self._loss_local if self.exchange == "p2p" else self.loss_slot,
                                           num_valid=num_valid)
-        if self.exchange == "p2p":
+        if self.exchange == "p2p":       # the exchange is the update kernel itself
             E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws)
-            pp, pg_, pf = self._peer_ptrs
-            if self._guard:
-                _lib.lib().call("ddfa_allreduce_adam_p2p_guarded", _lib.ptr_array(pp), _lib.ptr_array(pg_), _lib.ptr_array(pf), self._p2p_rank,
-                                self.world, self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel,
-                                self.numel, self.loss_slot.data_ptr(), self.hyper.data_ptr(), self._max_norm_dev.data_ptr(),
-                                self._gstate.data_ptr(), self._skipped.data_ptr() if self.skip_nonfinite else None,
-                                self._guard_ws.data_ptr(), torch.cuda.current_stream().cuda_stream)
-                return
-            _lib.lib().call("ddfa_allreduce_adam_p2p_hp", _lib.ptr_array(pp), _lib.ptr_array(pg_), _lib.ptr_array(pf), self._p2p_rank, self.world,
-                            self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.numel,
-                            self.loss_slot.data_ptr(), self._ticket.data_ptr(), self.hyper.data_ptr(), torch.cuda.current_stream().cuda_stream)
-            return
-        split = self.world > 1 and self.overlap_allreduce
-        E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws,
-                   on_small_grads_ready=self._reduce_small_grads if split else None)
-        if split:
-            lo, hi = self._gemm_grad_range
-            dist.all_reduce(self.flat_g[lo:hi], op=dist.ReduceOp.SUM, group=self.pg)
-            torch.cuda.current_stream().wait_stream(self._ar_stream)
-        elif self.world > 1:
-            dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
-        L = _lib.lib()
-        if self._guard:      # the norm of the exchanged gradients (both all-reduce halves are in: the wait above), then clipped Adam
-            stream = torch.cuda.current_stream().cuda_stream
-            L.call("ddfa_grad_norm", self.flat_g.data_ptr(), self.numel, self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
-                   self._guard_ws.data_ptr(), self._guard_ws.numel(), stream)
-            L.call("ddfa_adam_flat_guarded", self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
-                   self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.hyper.data_ptr(), self._gstate.data_ptr(),
-                   self._skipped.data_ptr() if self.skip_nonfinite else None, stream)
-            return
-        L.call("ddfa_adam_flat_hp", self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
-               self.exp_avg_sq.data_ptr(), self.step_count.data_ptr(), self.numel, self.hyper.data_ptr(),
-               torch.cuda.current_stream().cuda_stream)
+        else:
+            split = self.world > 1 and self.overlap_allreduce
+            E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws,
+                       on_small_grads_ready=self._reduce_small_grads if split else None)
+            if split:
+                lo, hi = self._gemm_grad_range
+                dist.all_reduce(self.flat_g[lo:hi], op=dist.ReduceOp.SUM, group=self.pg)
+                torch.cuda.current_stream().wait_stream(self._ar_stream)     # both halves are in before the norm and Adam
+            elif self.world > 1:
+                dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
+        L, stream = _lib.lib(), torch.cuda.current_stream().cuda_stream
+        for name, args in self._update:
+            L.call(name, *args, stream)
 
     def _reduce_small_grads(self):
         """All-reduce of the embedding / bias / readout / MLP gradients and the loss slot on a side stream (engine.backward
@@ -486,6 +470,21 @@ class FusedTrainer:
 
     # ------------------------------------------------------------------------------------
     # ---- host batches through per-shape static buffers + captured graphs -------------------------------------------------
+    def _graph_step(self, graph, warm: bool, enqueue):
+        """One step through a cached CUDA graph: ``enqueue()`` runs eagerly while the shape is not ``warm`` (its first visit
+        grows the workspace and loads modules outside any capture); after that ``graph`` is replayed, captured first, after a
+        device synchronise, when it is None.  Returns the graph (None when the step ran eagerly)."""
+        if not warm:
+            enqueue()
+            return None
+        if graph is None:
+            torch.cuda.synchronize(self.device)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                enqueue()
+        graph.replay()
+        return graph
+
     def _bucket_shape(self, N: int, Eg: int):
         """Padded (nodes, edges) of a batch under shape bucketing, or None when bucketing is off."""
         if self.bucket_nodes <= 0:
@@ -603,19 +602,10 @@ class FusedTrainer:
                 if vuln.dtype != torch.int32:
                     vuln = vuln.to(torch.int32)
                 self._enqueue(g_, dg, idx, vuln.contiguous(), gb, num_valid=slot["valid"])
-                return (gs, dg, idx, vuln)
+                st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
 
-            if not slot["warm"]:
-                st["keep"] = enqueue()
-                slot["warm"] = True
-            else:
-                if st["graph"] is None:
-                    torch.cuda.synchronize(self.device)
-                    cg = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(cg):
-                        st["keep"] = enqueue()            # tensors allocated during capture live in the graph's pool
-                    st["graph"] = cg
-                st["graph"].replay()
+            st["graph"] = self._graph_step(st["graph"], slot["warm"], enqueue)
+            slot["warm"] = True
             ev = torch.cuda.Event()
             ev.record(main)
             st["free"] = ev
@@ -667,19 +657,10 @@ class FusedTrainer:
                 g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
                 g_, dg, idx = m._prepare(g)
                 self._enqueue(g_, dg, idx, g.ndata["_VULN"], gb)
-                return (g, dg, idx)
+                slot["keep"] = (g, dg, idx)
 
-            if not slot["warm"]:
-                slot["keep"] = enqueue()
-                slot["warm"] = True
-            else:
-                if slot["graph"] is None:
-                    torch.cuda.synchronize(self.device)
-                    cg = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(cg):
-                        slot["keep"] = enqueue()
-                    slot["graph"] = cg
-                slot["graph"].replay()
+            slot["graph"] = self._graph_step(slot["graph"], slot["warm"], enqueue)
+            slot["warm"] = True
         return self.loss_slot
 
     def step(self, batch, global_batch: Optional[int] = None) -> torch.Tensor:
@@ -712,21 +693,14 @@ class FusedTrainer:
             graph_key = (id(g), det)
             capturable = self.use_cuda_graph and as_batched_cfg(batch).device.type == "cuda" and \
                 (graph_key in self._graphs or len(self._graphs) < self.max_resident_graphs)
-            if not capturable or shape_key not in self._warm_shapes:
-                # eager step; also the warm-up (workspace growth, lazy CUDA module init) before any capture
-                self._enqueue(g, dg, idx, vuln, global_batch)
-                self._warm_shapes.add(shape_key)
-            else:
-                # one captured CUDA graph per resident batch object (its device pointers are baked in)
-                entry = self._graphs.get(graph_key)
-                if entry is None:
-                    torch.cuda.synchronize(self.device)
-                    cg = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(cg):
-                        self._enqueue(g, dg, idx, vuln, global_batch)
-                    entry = (cg, g, idx, vuln)     # keep the captured tensors alive
-                    self._graphs[graph_key] = entry
-                entry[0].replay()
+            # one captured CUDA graph per resident batch object (its device pointers are baked in); a step that cannot be
+            # captured runs eagerly
+            entry = self._graphs.get(graph_key)
+            cg = self._graph_step(entry[0] if entry else None, capturable and shape_key in self._warm_shapes,
+                                  lambda: self._enqueue(g, dg, idx, vuln, global_batch))
+            if entry is None and cg is not None:
+                self._graphs[graph_key] = (cg, g, idx, vuln)     # keep the captured tensors alive
+            self._warm_shapes.add(shape_key)
         return self.loss_slot
 
     # ------------------------------------------------------------------------------------
