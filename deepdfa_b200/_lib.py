@@ -95,6 +95,12 @@ _SIGNATURES = {
     "ddfa_adam_flat_guarded": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "ddfa_p2p_guard_state_bytes": (_sz, []),
     "ddfa_allreduce_adam_p2p_guarded": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ddfa_node_sample_workspace_bytes": (_sz, [_i32]),
+    "ddfa_node_sample": (_int, [_vp, _vp, _i32, C.c_double, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ddfa_node_head_fwd": (_int, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "ddfa_node_bce": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, _vp, _vp, _vp]),
+    "ddfa_node_head_bwd_workspace_bytes": (_sz, [_i32, _i32]),
+    "ddfa_node_head_bwd": (_int, [_vp] * 5 + [_i32, _i32, _vp, _i32] + [_vp] * 6 + [_sz, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
 }
 
@@ -104,7 +110,8 @@ TUNE_DETERMINISTIC = 6
 _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_version", "ddfa_last_error", "ddfa_device_supported", "ddfa_launch_count", "ddfa_engine_available",
               "ddfa_build_csr_workspace_bytes", "ddfa_arena_batch_workspace_bytes", "ddfa_gru_step_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes_steps",
               "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes",
-              "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes"}
+              "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
+              "ddfa_node_head_bwd_workspace_bytes"}
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
 
 

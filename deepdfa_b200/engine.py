@@ -285,8 +285,10 @@ def node_indices(g: BatchedCFG, concat_all_absdf: bool, feature_key: str, device
 # Forward / backward
 # ------------------------------------------------------------------------------------------
 def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps: int, *, training: bool,
-            engine: int = ENGINE_SIMT, alloc=None, oob_counter: Optional[torch.Tensor] = None):
-    """Returns (pooled [B,2D], logits [B] or None, Saved or None)."""
+            engine: int = ENGINE_SIMT, alloc=None, oob_counter: Optional[torch.Tensor] = None, head: bool = True):
+    """Returns (pooled [B,2D], logits [B] or None, Saved or None).  ``head=False`` stops before the readout and returns
+    (x [N,D], h_T [N,D], Saved or None) instead: the label_style="node" trainer runs its own head over a row list
+    (``node_head_fwd``); Saved then holds no readout state."""
     _require_cuda(*params.flat_list(), dg.indptr, *idx)
     L = _lib.lib()
     _lib.apply_deterministic_mode()
@@ -376,6 +378,12 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
                 hs.append(h_next); ss.append(s_t); gs.append(g_t)
             h_cur = h_next
 
+    if not head:
+        saved = None
+        if training:
+            saved = Saved(T, D, x, hs, ss, gs, w_fold, b_fold, None, None, None, None, None, idx,
+                          h_img=h_imgs if use_images else None)
+        return x, h_cur, saved
     pooled = alloc.get("pooled", (B, 2 * D))
     logits = alloc.get("logits", (B,)) if nl > 0 else None
     gate_logit = alloc.get("gate_logit", (N,)) if training else None
@@ -394,8 +402,12 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
 
 
 def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack, *, dlogits: Optional[torch.Tensor] = None,
-             dpooled: Optional[torch.Tensor] = None, engine: int = ENGINE_SIMT, alloc=None, on_small_grads_ready=None):
-    """Accumulates (+=) parameter gradients into ``grads``.  Exactly one of dlogits / dpooled is given.
+             dpooled: Optional[torch.Tensor] = None, engine: int = ENGINE_SIMT, alloc=None, on_small_grads_ready=None,
+             dh_final: Optional[torch.Tensor] = None, dx_direct: Optional[torch.Tensor] = None):
+    """Accumulates (+=) parameter gradients into ``grads``.  Exactly one of dlogits / dpooled / (dh_final, dx_direct) is given.
+    ``dh_final`` / ``dx_direct`` ([N, D] each, from ``node_head_bwd``): the gradients of h_T and of the direct use of x; the
+    GGNN backward starts from them and the MLP / readout backward is skipped (their gradients are left alone).  ``dh_final``
+    is used as scratch afterwards.
     ``on_small_grads_ready``: called once every gradient EXCEPT those of ggnn.linears[0] and the GRU weight matrices (w_msg,
     b_msg, w_ih, w_hh) is final — with the tcgen05 engine that is before the batched weight-gradient launch, so a data-parallel
     trainer can start reducing them while that launch runs."""
@@ -412,7 +424,10 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     if dg.indptr_t is None:
         raise DdfaError("backward needs the transposed CSR (prepare_graph(need_transpose=True))")
 
-    if dlogits is not None:
+    if dh_final is not None or dx_direct is not None:
+        if dh_final is None or dx_direct is None or dlogits is not None or dpooled is not None:
+            raise DdfaError("backward: dh_final and dx_direct go together, without dlogits / dpooled")
+    elif dlogits is not None:
         if nl == 0:
             raise DdfaError("dlogits given but the module has no MLP head")
         dpooled_buf = alloc.get("dpooled", (B, 2 * D))
@@ -424,14 +439,17 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     elif dpooled is None:
         raise DdfaError("backward: neither dlogits nor dpooled given")
 
-    dh = alloc.get("dh_a", (N, D))
     dh_alt = alloc.get("dh_b", (N, D))
-    dx_direct = alloc.get("dx_direct", (N, D))
-    ro_bytes = L.call("ddfa_readout_bwd_workspace_bytes", B, D)
-    ro_ws = alloc.get("readout_bwd_ws", (max(ro_bytes, 16),), torch.uint8)
-    _call("ddfa_readout_bwd_ws", _p(dpooled), _p(saved.pooled), _p(saved.h[T]), _p(saved.x), _p(dg.graph_ptr), B, D,
-           _p(params.w_gate), _p(saved.gate_logit), _p(saved.seg_max), _p(saved.seg_sum), _p(dh), _p(dx_direct),
-           _p(grads.w_gate), _p(grads.b_gate), _p(ro_ws), ro_bytes, st, tag="ddfa_readout_bwd")
+    if dh_final is not None:
+        dh = dh_final
+    else:
+        dh = alloc.get("dh_a", (N, D))
+        dx_direct = alloc.get("dx_direct", (N, D))
+        ro_bytes = L.call("ddfa_readout_bwd_workspace_bytes", B, D)
+        ro_ws = alloc.get("readout_bwd_ws", (max(ro_bytes, 16),), torch.uint8)
+        _call("ddfa_readout_bwd_ws", _p(dpooled), _p(saved.pooled), _p(saved.h[T]), _p(saved.x), _p(dg.graph_ptr), B, D,
+               _p(params.w_gate), _p(saved.gate_logit), _p(saved.seg_max), _p(saved.seg_sum), _p(dh), _p(dx_direct),
+               _p(grads.w_gate), _p(grads.b_gate), _p(ro_ws), ro_bytes, st, tag="ddfa_readout_bwd")
 
     dw_fold = alloc.get("dw_fold", (3 * D, D))
     db_fold = alloc.get("db_fold", (3 * D,))
@@ -501,3 +519,67 @@ def graph_label_bce(dg: DeviceGraph, vuln: torch.Tensor, logits: Optional[torch.
     L.call("ddfa_graph_label_bce_valid", _p(logits), _p(vuln.contiguous()), _p(dg.graph_ptr), B, B if num_valid is None else int(num_valid),
            float(pos_weight), float(loss_scale), float(grad_scale), _p(labels), _p(loss), _p(dlogits), _stream_ptr())
     return labels, loss, dlogits
+
+
+# ------------------------------------------------------------------------------------------
+# label_style="node": the loss rows drawn on the device, the head and the loss over them (csrc/node_loss.cu)
+# ------------------------------------------------------------------------------------------
+def undersample_count(n_vuln: int, factor: float) -> int:
+    """How many non-vulnerable rows an undersampled node-style loss draws: ``round(n_vuln * factor)`` (base_module.py:96-137),
+    Python's round-half-to-even of the fp64 product — what ``ddfa_node_sample`` computes on the device with ``rint``."""
+    return round(n_vuln * float(factor))
+
+
+def node_sample(vuln: torch.Tensor, num_valid: torch.Tensor, factor: Optional[float], seed: int, draw: torch.Tensor,
+                rows: torch.Tensor, num_rows: torch.Tensor, status: torch.Tensor, alloc=None):
+    """``ddfa_node_sample``: writes the loss rows of the batch (ascending) into ``rows`` (int32 [N]) and their count into
+    ``num_rows`` (int32 [1]), on the device.  ``factor=None``: every valid node.  ``draw`` (int64 [1]) is advanced by the call;
+    ``status`` (int32 [1]) is set to 1 when the draw asks for more non-vulnerable nodes than there are."""
+    N = rows.numel()
+    f = -1.0 if factor is None else float(factor)
+    ws_bytes = _lib.lib().call("ddfa_node_sample_workspace_bytes", N) if factor is not None else 0
+    alloc = alloc or _FreshAlloc(rows.device)
+    ws = alloc.get("node_sample_ws", (max(ws_bytes, 16),), torch.uint8) if factor is not None else None
+    _call("ddfa_node_sample", _p(vuln), _p(num_valid), N, f, int(seed), _p(draw), _p(rows), _p(num_rows), _p(status), _p(ws),
+          ws_bytes, _stream_ptr())
+
+
+def node_head_fwd(params: ParamPack, x: torch.Tensor, h_final: torch.Tensor, rows: torch.Tensor, num_rows: torch.Tensor, alloc=None):
+    """``ddfa_node_head_fwd``: logits (fp32 [N] capacity; the first S are valid) and the hidden activations
+    ([L-1, N, 2D] capacity, or None for one layer) of the MLP head over the listed rows of ``[h_final | x]``."""
+    N, D = x.shape
+    nl = len(params.mlp_w)
+    alloc = alloc or _FreshAlloc(x.device)
+    logits = alloc.get("node_logits", (N,))
+    act = alloc.get("node_mlp_act", (nl - 1, N, 2 * D)) if nl > 1 else None
+    _call("ddfa_node_head_fwd", _p(h_final), _p(x), _p(rows), _p(num_rows), N, D, ptr_array([_p(t) for t in params.mlp_w]),
+          ptr_array([_p(t) for t in params.mlp_b]), nl, _p(act), _p(logits), _stream_ptr())
+    return logits, act
+
+
+def node_bce(logits: torch.Tensor, vuln: torch.Tensor, rows: torch.Tensor, num_rows: torch.Tensor, pos_weight: float,
+             loss_out: torch.Tensor, alloc=None):
+    """``ddfa_node_bce``: the mean BCE over the S rows into ``loss_out`` and dlogits (fp32 [N] capacity), returned."""
+    N = logits.numel()
+    alloc = alloc or _FreshAlloc(logits.device)
+    dlogits = alloc.get("node_dlogits", (N,))
+    _call("ddfa_node_bce", _p(logits), _p(vuln), _p(rows), _p(num_rows), N, float(pos_weight), _p(loss_out), _p(dlogits), _stream_ptr())
+    return dlogits
+
+
+def node_head_bwd(params: ParamPack, grads: ParamPack, dlogits: torch.Tensor, x: torch.Tensor, h_final: torch.Tensor,
+                  rows: torch.Tensor, num_rows: torch.Tensor, act: Optional[torch.Tensor], alloc=None):
+    """``ddfa_node_head_bwd``: accumulates the head's weight / bias gradients into ``grads`` and returns (dh_final, dx_direct),
+    [N, D] each, zero outside the listed rows — the starting point of ``backward(..., dh_final=, dx_direct=)``."""
+    N, D = x.shape
+    nl = len(params.mlp_w)
+    L = _lib.lib()
+    alloc = alloc or _FreshAlloc(x.device)
+    dh = alloc.get("dh_a", (N, D))
+    dx = alloc.get("dx_direct", (N, D))
+    ws_bytes = L.call("ddfa_node_head_bwd_workspace_bytes", N, D)
+    ws = alloc.get("node_head_bwd_ws", (max(ws_bytes, 16),), torch.uint8)
+    _call("ddfa_node_head_bwd", _p(dlogits), _p(h_final), _p(x), _p(rows), _p(num_rows), N, D,
+          ptr_array([_p(t) for t in params.mlp_w]), nl, _p(act), _p(dh), _p(dx), ptr_array([_p(t) for t in grads.mlp_w]),
+          ptr_array([_p(t) for t in grads.mlp_b]), _p(ws), ws_bytes, _stream_ptr())
+    return dh, dx

@@ -38,6 +38,17 @@ def flat_offsets(plist):
     return offs, total
 
 
+def flat_param_list(module):
+    """The tensors the flat buffers hold, in ``module.param_list()`` order: every parameter of the module.  In
+    label_style="node" the two gate slots of ``param_list()`` are non-persistent zero buffers, not parameters (the style has no
+    pooling), and are left out; the graph-style list is ``param_list()`` itself."""
+    plist = module.param_list()
+    if module.hparams.label_style == "node":
+        k = len(module._tables())
+        plist = plist[:k + 6] + plist[k + 8:]
+    return plist
+
+
 def owned_range(numel: int, rank: int, world: int):
     """``[lo, hi)``: the elements of the flat buffers whose Adam moments rank ``rank`` of ``world`` keeps up to date under
     ``exchange="p2p"``.  Mirrors ``allreduce_adam_p2p_kernel``: the buffers are cut into 16-byte units and every rank owns
@@ -74,11 +85,11 @@ class FusedAdam(torch.optim.Optimizer):
         keeps the moments of its :func:`owned_range` only (``exchange="p2p"``)."""
         params = list(module.parameters())
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, **_ADAM_FLAGS))
-        plist = module.param_list()
+        plist = flat_param_list(module)
         offs, total = flat_offsets(plist)
         where = {id(p): o for p, o in zip(plist, offs)}
         if len(plist) != len(params) or any(id(p) not in where for p in params):
-            raise ValueError("FusedAdam: module.parameters() and module.param_list() hold different tensors")
+            raise ValueError("FusedAdam: module.parameters() and the flat parameter list hold different tensors")
         if exp_avg.numel() != total or exp_avg_sq.numel() != total:
             raise ValueError(f"FusedAdam: moment buffers of {exp_avg.numel()} / {exp_avg_sq.numel()} elements, layout needs {total}")
         self._slots = [(where[id(p)], p.numel()) for p in params]      # per module.parameters() index: (flat offset, numel)
@@ -214,7 +225,7 @@ class FusedTrainer:
                  weight_decay: float = 1e-2, process_group=None, use_cuda_graph: bool = False, max_graph_shapes: int = 8,
                  max_resident_graphs: int = 64, distributed: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
                  bucket_min_pad_nodes: int = 64, overlap_allreduce: bool = True, exchange: str = "auto",
-                 max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False):
+                 max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False, node_sample_seed: int = 0):
         """``distributed=False`` makes this a single-rank trainer even inside an initialised process group (no all-reduce).
         ``bucket_nodes`` / ``bucket_edges`` > 0 switch on shape bucketing for HOST batches under ``use_cuda_graph``: every batch
         is padded with ONE dummy graph of isolated nodes up to the next multiple of ``bucket_nodes`` nodes (at least
@@ -227,12 +238,24 @@ class FusedTrainer:
         max_grad_norm)`` would, between the exchange and Adam, inside the (captured) step; ``float("inf")`` measures the norm
         without clipping.  ``skip_nonfinite=True`` makes a step whose norm is not finite leave parameters, moments and the Adam
         step count bit-unchanged (GradScaler's rule) and count it in ``skipped_steps``.  ``grad_norm`` holds the last step's
-        pre-clip norm; ``max_grad_norm`` can be changed later, also after capture."""
+        pre-clip norm; ``max_grad_norm`` can be changed later, also after capture.
+
+        label_style="node": the loss is the mean BCE over per-node logits, on every valid node, or with
+        ``undersample_node_on_loss_factor`` on every vulnerable node plus ``round(n_vuln * factor)`` non-vulnerable ones drawn on
+        the device inside the step (``ddfa_node_sample``: Philox keys from ``node_sample_seed`` and the draw counter
+        ``node_sample_draws``).  The head runs over that row list only.  A draw that asks for more non-vulnerable nodes than the
+        batch has takes them all and raises ``ValueError`` at the next step or at ``check_inputs()`` (``random.sample`` raises
+        on the module path).  One rank only."""
         if module.device.type != "cuda":
             raise _lib.DdfaError("FusedTrainer needs the module on a CUDA device (no CPU fallback)")
-        if module.hparams.label_style != "graph" or module.hparams.encoder_mode:
-            raise NotImplementedError("FusedTrainer fuses the shipped configuration (label_style='graph', a classifier head); train "
-                                      "label_style='node' / encoder_mode modules through module.training_step + torch.optim")
+        self._node = module.hparams.label_style == "node"
+        if module.hparams.label_style not in ("graph", "node") or module.hparams.encoder_mode or module._num_layers == 0:
+            raise NotImplementedError("FusedTrainer trains a classifier head (label_style='graph' or 'node', not encoder_mode); train "
+                                      "other modules through module.training_step + torch.optim")
+        seed = int(node_sample_seed)
+        if not 0 <= seed < 2 ** 64:
+            raise ValueError(f"node_sample_seed must be in [0, 2**64), got {node_sample_seed!r}")
+        self.node_sample_seed = seed
         self.module = module
         self.device = module.device
         self.pg = process_group
@@ -262,13 +285,17 @@ class FusedTrainer:
                                    or torch.cuda.device_count() < self.world):
                 exchange, self.exchange_note = "nccl", "auto: ranks span more than this node (or a non-NCCL group): NCCL all-reduce"
         self.exchange = exchange if self.world > 1 else "nccl"
+        if self._node and self.world > 1:
+            # the global mean divides by the S of all ranks: their row counts would have to be exchanged before the gradient scale
+            raise NotImplementedError("FusedTrainer: label_style='node' trains on one rank (distributed=False or a one-rank group)")
         self.use_cuda_graph = use_cuda_graph
         # a captured graph bakes in the batch SHAPE (and, for resident batches, the batch object): cap how many are kept so a
         # stream of ever-new shapes (un-bucketed real data) degrades to eager launches instead of growing without bound
         self.max_graph_shapes = max_graph_shapes
         self.max_resident_graphs = max_resident_graphs
         plist = module.param_list()
-        offs, total = flat_offsets(plist)
+        flat = flat_param_list(module)
+        offs, total = flat_offsets(flat)
         self.numel = total
         ntab = len(module._tables())
         self._gemm_grad_range = (offs[ntab], offs[ntab + 4])     # flat offsets of [w_msg, b_msg, w_ih, w_hh]
@@ -313,13 +340,27 @@ class FusedTrainer:
                 else:
                     self._guard_ws = torch.empty(L.call("ddfa_grad_norm_workspace_bytes", total), dtype=torch.uint8, device=self.device)
         gviews = []
-        for p, o in zip(plist, offs):
+        for p, o in zip(flat, offs):
             view = self.flat_p[o:o + p.numel()].view_as(p)
             view.copy_(p.data)
             p.data = view                      # module parameters now alias the flat buffer
             gviews.append(self.flat_g[o:o + p.numel()].view_as(p))
         K, nl = len(module._tables()), module._num_layers
-        self.params = E.ParamPack.from_flat_list([p.data for p in plist], K, nl)
+        pviews = [p.data for p in flat]
+        if self._node:
+            # the gate slots of the ParamPack: the module's zero buffers, and gradients nothing reads (the node head has no gate)
+            gate = plist[K + 6:K + 8]
+            self._gate_grad_sink = [torch.zeros_like(t) for t in gate]
+            pviews = pviews[:K + 6] + [t.data for t in gate] + pviews[K + 6:]
+            gviews = gviews[:K + 6] + self._gate_grad_sink + gviews[K + 6:]
+            with torch.cuda.device(self.device):
+                self._draw = torch.zeros(1, dtype=torch.int64, device=self.device)         # draws made (ddfa_node_sample advances it)
+                self._num_rows = torch.zeros(1, dtype=torch.int32, device=self.device)     # S of the last step
+                self._sample_status = torch.zeros(1, dtype=torch.int32, device=self.device)
+            self._status_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+            self._status_pending = None
+            self._last_rows = None
+        self.params = E.ParamPack.from_flat_list(pviews, K, nl)
         self.grads = E.ParamPack.from_flat_list(gviews, K, nl)
         self.loss_slot = self.flat_g[total:total + 1]          # this rank's share of the loss goes here (the kernels' loss_out)
         if self.exchange == "p2p":                                # ... and the global loss into a local word (peers read the slot above)
@@ -377,6 +418,60 @@ class FusedTrainer:
         """Steps skipped because their gradient norm was not finite (reads the device counter: one synchronisation)."""
         return int(self._skipped.item()) if self._guard else 0
 
+    # ---- label_style="node" ------------------------------------------------------------------------------------------------
+    def _require_node(self, what):
+        if not self._node:
+            raise ValueError(f"{what}: this FusedTrainer trains a label_style='graph' module")
+
+    @property
+    def node_sample_draws(self) -> int:
+        """Undersampling draws made so far (the Philox counter of the next draw).  Reading it synchronises.  Setting it writes
+        the device word in stream order, so a resumed run that restores it draws what the uninterrupted run would have drawn."""
+        self._require_node("node_sample_draws")
+        return int(self._draw.item())
+
+    @node_sample_draws.setter
+    def node_sample_draws(self, value: int):
+        self._require_node("node_sample_draws")
+        v = int(value)
+        if v < 0:
+            raise ValueError(f"node_sample_draws must be >= 0, got {value!r}")
+        self._draw.fill_(v)
+
+    def last_loss_rows(self) -> torch.Tensor:
+        """int32 device tensor: the nodes the last step's loss was taken over, ascending (reads S: one synchronisation)."""
+        self._require_node("last_loss_rows")
+        if self._last_rows is None:
+            return torch.zeros(0, dtype=torch.int32, device=self.device)
+        return self._last_rows[:int(self._num_rows.item())].clone()
+
+    def _node_step_done(self, rows):
+        """After a node-style step: remembers its row list and sends the sampler's status word to the host behind it."""
+        self._last_rows = rows
+        self._status_host.copy_(self._sample_status, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._status_pending = ev
+
+    def _raise_deferred_sample_errors(self, wait: bool = False):
+        if not self._node or self._status_pending is None:
+            return
+        if wait:
+            self._status_pending.synchronize()
+        elif not self._status_pending.query():
+            return
+        self._status_pending = None
+        if int(self._status_host[0]):
+            self._sample_status.zero_()
+            self._status_host.zero_()
+            raise ValueError("undersample_node_on_loss_factor asked for more non-vulnerable nodes than an earlier batch had "
+                             "(random.sample raises 'Sample larger than population'); that step drew all of them")
+
+    def check_inputs(self):
+        """Waits for the last step and raises what it deferred: ``ValueError`` when a node-style undersampling draw asked for
+        more non-vulnerable nodes than the batch had."""
+        self._raise_deferred_sample_errors(wait=True)
+
     # ------------------------------------------------------------------------------------
     def _setup_p2p(self, total: int):
         """Symmetric allocations + rendezvous (torch.distributed._symmetric_memory): every rank gets device pointers to every
@@ -431,11 +526,15 @@ class FusedTrainer:
                                  "the loss is the mean over the GLOBAL batch)")
         return int(local_graphs)
 
-    def _enqueue(self, g, dg, idx, vuln, global_batch: int, num_valid: Optional[int] = None):
+    def _enqueue(self, g, dg, idx, vuln, global_batch: int, num_valid: Optional[int] = None, valid_nodes: Optional[torch.Tensor] = None):
+        """Enqueues one step.  Node style returns the row-list buffer the step's loss rows go to; ``valid_nodes``: the int32
+        device word of its valid node count under bucketing (None: every node is valid)."""
         m = self.module
         eng = _ENGINES[m.engine]
         pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
         self.flat_g.zero_()
+        if self._node:
+            return self._enqueue_node(dg, idx, vuln, eng, pw, valid_nodes)
         _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws)
         _, _, dlogits = E.graph_label_bce(dg, vuln, logits, pw, 1.0 / global_batch, 1.0 / global_batch, True,
                                           alloc=self.ws, loss_out=self._loss_local if self.exchange == "p2p" else self.loss_slot,
@@ -455,6 +554,29 @@ class FusedTrainer:
         L, stream = _lib.lib(), torch.cuda.current_stream().cuda_stream
         for name, args in self._update:
             L.call(name, *args, stream)
+
+    def _enqueue_node(self, dg, idx, vuln, eng, pw, valid_nodes):
+        """label_style="node" (one rank): GGNN forward without the readout, the loss rows drawn on the device, the head and
+        the BCE over them, the head backward into dh_T / dx, the GGNN backward from there, the update."""
+        m, ws = self.module, self.ws
+        N = dg.num_nodes
+        if vuln.dtype != torch.int32:
+            vuln = vuln.to(torch.int32)
+        x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False)
+        if valid_nodes is None:
+            valid_nodes = ws.get("node_valid", (1,), torch.int32)
+            valid_nodes.fill_(N)
+        rows = ws.get("node_rows", (N,), torch.int32)
+        E.node_sample(vuln, valid_nodes, m.hparams.undersample_node_on_loss_factor, self.node_sample_seed, self._draw, rows,
+                      self._num_rows, self._sample_status, alloc=ws)
+        logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
+        dlogits = E.node_bce(logits, vuln, rows, self._num_rows, pw, self.loss_slot, alloc=ws)
+        dh, dx = E.node_head_bwd(self.params, self.grads, dlogits, x, h_T, rows, self._num_rows, act, alloc=ws)
+        E.backward(self.params, dg, saved, self.grads, engine=eng, alloc=ws, dh_final=dh, dx_direct=dx)
+        L, stream = _lib.lib(), torch.cuda.current_stream().cuda_stream
+        for name, args in self._update:
+            L.call(name, *args, stream)
+        return rows
 
     def _reduce_small_grads(self):
         """All-reduce of the embedding / bias / readout / MLP gradients and the loss slot on a side stream (engine.backward
@@ -516,7 +638,8 @@ class FusedTrainer:
                 st = {"src": torch.empty(Es, dtype=src.dtype, device=dev), "dst": torch.empty(Es, dtype=dst.dtype, device=dev),
                       "bnn": torch.empty(Bs, dtype=torch.int64, device=dev),
                       "ndata": {k: torch.zeros((Ns,) + tuple(v.shape[1:]), dtype=v.dtype, device=dev) for k, v in g.ndata.items()},
-                      "graph": None, "keep": None, "free": None, "ready": None}
+                      "graph": None, "keep": None, "free": None, "ready": None, "rows": None,
+                      "valid_nodes": torch.zeros(1, dtype=torch.int32, device=dev) if (bucket and self._node) else None}
                 return st
             # two input-buffer sets: while the graph of one set runs, the next batch is copied into the other (prefetch)
             slot = {"sets": [new_set(), new_set()], "next": 0, "staged": None, "warm": False, "N": Ns, "gb": gb,
@@ -542,6 +665,8 @@ class FusedTrainer:
             st["bnn"][:B].copy_(g.batch_num_nodes(), non_blocking=True)
             for k, v in g.ndata.items():
                 st["ndata"][k][:N].copy_(v, non_blocking=True)
+            if st["valid_nodes"] is not None:
+                st["valid_nodes"].fill_(N)              # node style: the sampler leaves the padding nodes (the tail) out
             if slot["valid"] is not None:
                 Nb, Eb = slot["N"], st["src"].shape[0]
                 pad_nodes = Nb - N
@@ -601,11 +726,13 @@ class FusedTrainer:
                 vuln = gs.ndata["_VULN"]
                 if vuln.dtype != torch.int32:
                     vuln = vuln.to(torch.int32)
-                self._enqueue(g_, dg, idx, vuln.contiguous(), gb, num_valid=slot["valid"])
+                st["rows"] = self._enqueue(g_, dg, idx, vuln.contiguous(), gb, num_valid=slot["valid"], valid_nodes=st["valid_nodes"])
                 st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
 
             st["graph"] = self._graph_step(st["graph"], slot["warm"], enqueue)
             slot["warm"] = True
+            if self._node:
+                self._node_step_done(st["rows"])
             ev = torch.cuda.Event()
             ev.record(main)
             st["free"] = ev
@@ -616,6 +743,7 @@ class FusedTrainer:
         f1: the batch producer).  With ``use_cuda_graph`` the batch is assembled into static per-shape buffers by
         ``ddfa_arena_batch`` inside one captured graph, so a step costs the H2D copy of the id list plus one graph launch;
         otherwise it is ``step(arena.batch(ids))``."""
+        self._raise_deferred_sample_errors()
         self.optimizer.step()
         if not self.use_cuda_graph:
             return self._step_eager(arena.batch(ids), global_batch)
@@ -656,17 +784,20 @@ class FusedTrainer:
             def enqueue():
                 g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
                 g_, dg, idx = m._prepare(g)
-                self._enqueue(g_, dg, idx, g.ndata["_VULN"], gb)
+                slot["rows"] = self._enqueue(g_, dg, idx, g.ndata["_VULN"], gb)
                 slot["keep"] = (g, dg, idx)
 
             slot["graph"] = self._graph_step(slot["graph"], slot["warm"], enqueue)
             slot["warm"] = True
+            if self._node:
+                self._node_step_done(slot["rows"])
         return self.loss_slot
 
     def step(self, batch, global_batch: Optional[int] = None) -> torch.Tensor:
         """One optimisation step on this rank's shard.  Returns the device tensor holding the
         global mean loss (valid after the step's stream work completes).  Starts with ``self.optimizer.step()``, which hands
         the current learning rate etc. to this step's Adam launch (an LR scheduler on ``self.optimizer`` sees that call)."""
+        self._raise_deferred_sample_errors()
         self.optimizer.step()
         if self.use_cuda_graph:
             gb_ = as_batched_cfg(batch)
@@ -696,11 +827,16 @@ class FusedTrainer:
             # one captured CUDA graph per resident batch object (its device pointers are baked in); a step that cannot be
             # captured runs eagerly
             entry = self._graphs.get(graph_key)
-            cg = self._graph_step(entry[0] if entry else None, capturable and shape_key in self._warm_shapes,
-                                  lambda: self._enqueue(g, dg, idx, vuln, global_batch))
+            out = {}
+
+            def enqueue():
+                out["rows"] = self._enqueue(g, dg, idx, vuln, global_batch)
+            cg = self._graph_step(entry[0] if entry else None, capturable and shape_key in self._warm_shapes, enqueue)
             if entry is None and cg is not None:
-                self._graphs[graph_key] = (cg, g, idx, vuln)     # keep the captured tensors alive
+                self._graphs[graph_key] = (cg, g, idx, vuln, out["rows"])     # keep the captured tensors alive
             self._warm_shapes.add(shape_key)
+            if self._node:
+                self._node_step_done(out["rows"] if "rows" in out else entry[4])
         return self.loss_slot
 
     # ------------------------------------------------------------------------------------

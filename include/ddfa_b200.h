@@ -357,6 +357,51 @@ int ddfa_graph_label_bce_valid(const float *logits, const int32_t *vuln, const i
                                float grad_scale, float *labels, float *loss_out, float *dlogits, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K8'  label_style="node" loss (csrc/node_loss.cu): the rows the loss is taken over, drawn on the device, and the MLP head +
+ * BCEWithLogits(pos_weight) over that row list.  Replaces BaseModule.resample (base_module.py:96-137: every vulnerable node plus
+ * random.sample of round(n_vuln * factor) non-vulnerable ones) and the node-style loss (base_module.py:84-85,178-183).  Nothing
+ * syncs with the host: num_nodes N is a CAPACITY that sizes every grid, the row count S lives in a device word, so one captured
+ * CUDA graph serves every batch of a bucket shape.
+ *
+ * ddfa_node_sample: rows int32[N] receives the row list in ascending node order, *num_rows = S.
+ *   Valid nodes are [0, *num_valid) (a device word: under shape bucketing the padding nodes are the tail).
+ *   factor < 0 (no undersampling): every valid node; vuln / draw / status / workspace are not read (may be NULL).  One launch.
+ *   factor >= 0: every valid node with vuln != 0, plus k = rint((double)n_vuln * factor) valid nodes with vuln == 0 drawn
+ *   uniformly without replacement: the k smallest (key, node) pairs, key = word 0 of Philox4x32-10 with key `seed` and counter
+ *   (draw lo, draw hi, node, 0).  *draw (int64 device word) is this call's draw index; the call advances it by one, so every
+ *   replay of a captured launch draws afresh.  k larger than the population sets *status = 1 (never cleared by the call) and
+ *   takes the whole population.  Launch sequence (fixed, 13 kernels + 1 memset): clear control words; count n_vuln and the
+ *   population; k and the draw index; 4 x (key histogram of one 8-bit digit over the candidates, one-CTA bin pick) = radix
+ *   select of the k-th smallest key, ties at it taken in node order; per-CTA counts; one-CTA scan in CTA order; write.
+ *   Integer counts only: the rows do not depend on CTA scheduling.
+ *   workspace: ddfa_node_sample_workspace_bytes(N) bytes, 4-byte aligned, scratch.
+ * ddfa_node_head_fwd: for s < S, row r = rows[s]: o = [h_final[r] | x[r]] (read from the two fp32 [N, D] planes), num_layers
+ *   linears with ReLU between (mlp_w / mlp_b as in ddfa_readout_mlp_fwd), logits[s] = the last output (fp32[N] capacity,
+ *   compact).  mlp_act fp32[(L-1)][N][2D] receives the hidden activations (post-ReLU), compact: row s of layer i at
+ *   mlp_act[(i*N + s)*2D].  SIMT fp32.
+ * ddfa_node_bce: loss_out[0] = mean over s < S of bce(logits[s], (float)vuln[rows[s]]; pos_weight) (NaN for S = 0: a mean over
+ *   nothing), dlogits[s] = its derivative (compact; may be NULL).  One CTA, a fixed summation order in both tuning modes.
+ * ddfa_node_head_bwd: dlogits[S] -> dh_final, dx (fp32 [N, D] each, overwritten whole: zero outside the listed rows); accumulates
+ *   (+=) dmlp_w / dmlp_b (host arrays of device pointers).  Weight and bias gradients are reduced over the rows in a fixed order
+ *   in both tuning modes (32 private partials over fixed row chunks, added in chunk order): bit-reproducible.
+ *   workspace: ddfa_node_head_bwd_workspace_bytes(N, D) bytes, 16-byte aligned, scratch.
+ * ------------------------------------------------------------------------------------- */
+size_t ddfa_node_sample_workspace_bytes(int32_t num_nodes);
+int ddfa_node_sample(const int32_t *vuln, const int32_t *num_valid, int32_t num_nodes, double factor, uint64_t seed,
+                     int64_t *draw, int32_t *rows, int32_t *num_rows, int32_t *status, void *workspace,
+                     size_t workspace_bytes, void *stream);
+int ddfa_node_head_fwd(const float *h_final, const float *x, const int32_t *rows, const int32_t *num_rows,
+                       int32_t num_nodes, int32_t dim, const float *const *mlp_w, const float *const *mlp_b,
+                       int32_t num_layers, float *mlp_act, float *logits, void *stream);
+int ddfa_node_bce(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows,
+                  int32_t num_nodes, float pos_weight, float *loss_out, float *dlogits, void *stream);
+size_t ddfa_node_head_bwd_workspace_bytes(int32_t num_nodes, int32_t dim);
+int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *x, const int32_t *rows,
+                       const int32_t *num_rows, int32_t num_nodes, int32_t dim, const float *const *mlp_w,
+                       int32_t num_layers, const float *mlp_act, float *dh_final, float *dx, float *const *dmlp_w,
+                       float *const *dmlp_b, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K10  torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 (DDFA/configs/
  * config_default.yaml:43-47) over one flat parameter buffer.  step_count: int32[1] device
  * counter, incremented by the kernel (graph-capture safe).
