@@ -365,14 +365,17 @@ __global__ void __launch_bounds__(kD3Threads, 1) dgrad3_kernel(const uint8_t *__
 //            dh', the packed gates and h (image pieces, or fp32 rows at step 0) arrive by TMA bulk copies in one 64 KB stage;
 //            the transposed edge gather of ds_in is folded in (register loads, data-dependent addresses).  It writes the four q
 //            images (global: the weight-gradient GEMM reads them later; rows N .. Npad-1 as zeros) and dh' * z into the rows
-//            of the dh OUTPUT, which the dh-role CTAs overwrite with acc + dh' * z in phase B — dh' * z never needs a plane of
-//            its own (so dh must alias neither dh_out nor ds_in: other clusters are still in phase A when this one writes dh);
-//   handover every writer fences its generic-proxy stores against the async proxy (the q tiles are read back by TMA), then
-//            the cluster barrier (arrive.release / wait.acquire);
+//            of the dh OUTPUT, onto which the dh-role CTAs add acc in phase B — dh' * z never needs a plane of its own (so dh
+//            must alias neither dh_out nor ds_in: other clusters are still in phase A when this one writes dh);
+//   handover every writer fences its generic-proxy stores against the async proxy (the q tiles are read back by TMA, dh' * z
+//            is added to by bulk reductions), then the cluster barrier (arrive.release / wait.acquire);
 //   phase B  dgrad3_kernel's MMA loop, unchanged: the three q tiles of the role by bulk copy (L2 hits: written microseconds
-//            earlier), m64n64k16 bf16x3, the same MMA order, so ds and dh are bit-identical to the two-kernel path.
+//            earlier), m64n64k16 bf16x3, the same MMA order.  The accumulator leaves through shared memory: ds by bulk copies,
+//            dh by bulk fp32 add-reductions onto dh' * z (one rounding to nearest, as the register add of the two-kernel path),
+//            so ds and dh are bit-identical to the two-kernel path.
 // The phase-A operands of a tile and the q tiles share the two 64 KB stages as one ring, four uses per tile (A, q0, q1, q2):
-// the next tile's phase-A copy goes into the stage that q1 releases, so it streams from HBM while phase B runs.
+// the next tile's phase-A copy goes into the stage that q1 releases, so it streams from HBM while phase B runs.  q2's stage
+// then holds the staged output until the end of the next tile's phase A, while its copies drain.
 // Persistent over tiles, one cluster per 4 SMs; every CTA of a cluster runs the same tiles (each iteration holds a cluster
 // barrier).  HF32: h as fp32 rows (step 0: h_0 = x) or the activation image.  CSRP: the CSR scalars / first neighbour ids of the
 // folded gather pipelined across tiles, one value per lane (DDFA_TUNE_GATE_BWD_TMA = 2, default; 1 = fetched inside the tile).
@@ -384,8 +387,40 @@ constexpr int kGtPre = 2;           // neighbour rows of the folded gather reque
 constexpr int kGtRowsPerWarp = kGtRows / kEpiWarps;
 
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive_n(uint32_t bar, uint32_t n) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory");
+}
+// Bulk copies shared -> global, tracked per issuing thread in bulk groups: a plain copy, and one that adds the fp32 values onto the
+// destination at L2 (UBLKRED.G.S.ADD.F32.RN: round to nearest even, and on the H100 subnormal inputs and results kept, the bits
+// of an fp32 register add in every probed case; DESIGN §3)
+__device__ __forceinline__ void bulk_s2g_hint(float *dst, uint32_t src, uint32_t bytes, uint64_t pol) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst), "r"(src), "r"(bytes), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_s2g_add_f32_hint(float *dst, uint32_t src, uint32_t bytes, uint64_t pol) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.L2::cache_hint.add.f32 [%0], [%1], %2, %3;" ::"l"(dst), "r"(src),
+               "r"(bytes), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }   // sources read
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }             // writes done
+
+// Phase B's output goes out through the stage that held q2 (always stage 1: four ring uses per tile over two stages), as [64 rows
+// x 64 fp32] per warpgroup, rows padded from 256 to 272 bytes: the 8 rows of one warp store instruction start 4 banks apart, so
+// each bank is hit twice by the 256 bytes of a v2 store (the minimum).  Row r of warpgroup wg lies at (r / 16) x 16 KB + wg x 8 KB
+// + (r % 16) x 272 — inside the bytes of q2 that wg's own MMAs read (rows 64 wg .. 64 wg + 63 of each 16 KB chunk), so a
+// warpgroup may overwrite them as soon as all of its last MMAs have completed.
+constexpr int kD3OutStage = 3 % kD3Stages;
+static_assert(4 % kD3Stages == 0, "q2 lands in the same stage every tile");
+constexpr int kStRowBytes = 64 * 4 + 16;
+static_assert(16 * kStRowBytes <= kChunkBytes / 2, "16 staged rows fit in a warpgroup's half of a chunk");
+__device__ __forceinline__ uint32_t staged_row(uint32_t stage, int wg, int r) {
+  return stage + (uint32_t)((r >> 4) * kChunkBytes + wg * (kChunkBytes / 2) + (r & 15) * kStRowBytes);
+}
 
 template <bool HF32, bool CSRP>
 __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const float *__restrict__ dh_out, const float *__restrict__ h,
@@ -477,13 +512,10 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
     // ===== consumers: phase A, warp w owns rows w + 8 j (j < 4) of the CTA's 32; phase B, warpgroup wg owns nodes 64 wg .. + 63 =====
     pdl_wait();
     const int col = lane * 4;
-    // L2 policies (created where they are used: 64-bit values live across the whole loop made the kernel spill)
-    // pol_tmp: ds / dh / dh' * z die after the next kernel has read them; pol_dhz: the last read of dh' * z
+    // L2 policy (created where it is used: 64-bit values live across the whole loop made the kernel spill)
+    // pol_tmp: ds / dh / dh' * z die after the next kernel has read them
 #define DDFA_POL_TMP l2_policy((hints & 4) ? 2 : 0)
-#define DDFA_POL_DHZ l2_policy((hints & 8) ? 1 : 0)
     const int wg = warp >> 2;
-    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int col0 = half * 64 + 2 * (lane & 3);
     const bool tr = (warp == 0 && lane == 0);
     float4 sum[7];      // the seven column sums (bias gradients) over all the warp's rows, combined once at the end
 #pragma unroll
@@ -618,11 +650,20 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
         __syncwarp();
         if (lane == 0) mbar_arrive(empty(stage));      // this warp has read its rows of the stage
       }
+      // the previous tile's output has been read out of its stage (long ago: its copies drained during this phase A): hand the
+      // stage back for this tile's first q copy, which the producer issues only after the handover below — four arrivals per
+      // warpgroup, as the MMA loop makes for the other uses
+      if (k > 0 && (warp & 3) == 0) {
+        bulk_wait_read_all();
+        __syncwarp();
+        if (lane == 0) mbar_arrive_n(empty(kD3OutStage), kEpiWarps / 2);
+      }
       // ---------------- handover: q and dh' * z of the whole tile visible to the cluster ----------------
       fence_proxy_async_global();
       cluster_arrive_release();
       cluster_wait_acquire();
       if (tr) trace_stamp(tron, k, 11);      // 11: handover done
+      if ((warp & 3) == 0 && role == 1) fence_proxy_async_global();      // dh' * z (generic stores of the cluster) is added to by the async proxy
       // ---------------- phase B: dgrad3_kernel's loop ----------------
       if (k == 0) mbar_wait_bounded(w_full, 0);
       float acc[32];
@@ -652,44 +693,44 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
         if (pending >= 0 && lane == 0) mbar_arrive(empty(pending));
         pending = stage;
       }
-      // dh = acc + (dh' * z), the elementwise term written into dh's rows in phase A: the first of the thread's two rows is
-      // fetched while the last MMAs run, the second after them (both in flight at once would make the kernel spill)
-      float2 dv[8];
-      auto fetch_dv = [&](int hh) {
-        const uint64_t pol_dhz = DDFA_POL_DHZ;
-        const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          dv[j] = make_float2(0.f, 0.f);
-          if (role == 1 && node < N) {
-            const float *p = dh + node * kD + col0 + 8 * j;
-            dv[j] = make_float2(ldg_cg_f32_hint(p, pol_dhz), ldg_cg_f32_hint(p + 1, pol_dhz));
-          }
-        }
-      };
-      fetch_dv(0);
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      if (tr) { trace_stamp(tron, k, 6); trace_stamp(tron, k, 8); }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty(pending));
-      if (tr) trace_stamp(tron, k, 9);
+      if (tr) { trace_stamp(tron, k, 6); trace_stamp(tron, k, 8); trace_stamp(tron, k, 9); }
+      // ds = acc; dh = acc + dh' * z, the elementwise term phase A wrote into dh's rows.  The fragment goes into q2's stage (see
+      // staged_row), then one bulk copy per row leaves the SM — for dh one that adds onto dh' * z in L2, so the SM never reads it
+      // back.  Rows >= N are never written: ds and dh are unpadded [N, 128] planes.
+      const uint32_t st_base = sbase + kD3OffStage + kD3OutStage * kD3StageBytes;      // == pending
+      // a warp's wait covers the rows of q2 its own MMAs read (16 per chunk); it stages into rows its siblings read
+      if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+      else asm volatile("bar.sync 3, 128;" ::: "memory");
+      uint32_t tid;      // re-read here: addresses derived from it and kept across the tile loop made the kernel spill
+      asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        if (hh == 1) fetch_dv(1);
-        const int64_t node = (int64_t)tile * kTileM + row0 + 8 * hh;
-        if (node < N) {
-          const uint64_t pol_tmp = DDFA_POL_TMP;
-          float *out = role == 0 ? ds : dh;
+        const uint32_t rowp = staged_row(st_base, wg, (tid >> 5 & 3) * 16 + (tid >> 2 & 7) + 8 * hh) + 8 * (tid & 3);
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            st_f2_hint(out + node * kD + col0 + 8 * j, make_float2(acc[4 * j + 2 * hh] + dv[j].x, acc[4 * j + 2 * hh + 1] + dv[j].y), pol_tmp);
-        }
+        for (int j = 0; j < 8; ++j)
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(rowp + 32 * j), "f"(acc[4 * j + 2 * hh]), "f"(acc[4 * j + 2 * hh + 1]) : "memory");
       }
+      fence_proxy_async_shared();
+      if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");      // the warpgroup's 64 rows are staged
+      else asm volatile("bar.sync 3, 128;" ::: "memory");
+      if ((warp & 3) == 0 && elect_one()) {      // one thread per warpgroup issues its copies (uniform operands: straight-line issue)
+        const uint64_t pol_tmp = DDFA_POL_TMP;
+        const int64_t node0 = (int64_t)tile * kTileM + wg * 64;
+        float *out = (role == 0 ? ds : dh) + node0 * kD + half * 64;
+        const int rows = (int)min((int64_t)64, (int64_t)N - node0);
+        for (int r = 0; r < rows; ++r) {
+          if (role == 0) bulk_s2g_hint(out + (int64_t)r * kD, staged_row(st_base, wg, r), 64 * 4, pol_tmp);
+          else bulk_s2g_add_f32_hint(out + (int64_t)r * kD, staged_row(st_base, wg, r), 64 * 4, pol_tmp);
+        }
+        bulk_commit();
+      }
+      __syncwarp();
       if (tr) trace_stamp(tron, k, 10);
     }
 #undef DDFA_POL_TMP
-#undef DDFA_POL_DHZ
+    bulk_wait_all();      // ds / dh complete before the CTA exits: the next kernels of the step read them
     // bias gradients: the warps' column sums through the stages, once both warpgroups are past their last MMAs
     asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
     float *red = reinterpret_cast<float *>(smem + kD3OffStage);
