@@ -93,6 +93,7 @@ _SIGNATURES = {
     "ddfa_grad_norm_workspace_bytes": (_sz, [_i64]),
     "ddfa_grad_norm": (_int, [_vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "ddfa_adam_flat_guarded": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "ddfa_adam_flat_ranges": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _vp]),
     "ddfa_p2p_guard_state_bytes": (_sz, []),
     "ddfa_allreduce_adam_p2p_guarded": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ddfa_node_sample_workspace_bytes": (_sz, [_i32]),

@@ -5,7 +5,8 @@
 // K10 replaces torch.optim.Adam(lr=1e-3, weight_decay=1e-2) — coupled L2, not AdamW
 // (DDFA/configs/config_default.yaml:43-47) — over one flat parameter buffer, with the hyperparameters by value
 // (ddfa_adam_flat) or from a device word (ddfa_adam_flat_hp); ddfa_adam_flat_guarded is the same update on the clipped
-// gradient, after ddfa_grad_norm (grad_guard.cu).  The arithmetic is adam.cuh's.
+// gradient, after ddfa_grad_norm (grad_guard.cu); ddfa_adam_flat_ranges updates only the elements inside a list of ranges (the
+// trainable parameters of a partly frozen model).  The arithmetic is adam.cuh's.
 #include <math.h>
 
 #include "common.cuh"
@@ -75,12 +76,25 @@ __global__ void __launch_bounds__(256) bce_loss_sum_kernel(const float *__restri
   if (threadIdx.x == 0) *loss_out = loss_scale * s_t[0];
 }
 
+// i inside one of the sorted, disjoint [begin, end) pairs of ranges[2 * num_ranges] (binary search for the last begin <= i)
+__device__ __forceinline__ bool in_ranges(const int64_t *__restrict__ ranges, int32_t num_ranges, int64_t i) {
+  int32_t lo = 0, hi = num_ranges;
+  while (lo < hi) {
+    const int32_t mid = (lo + hi) >> 1;
+    if (ranges[2 * mid] <= i) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo > 0 && i < ranges[2 * lo - 1];
+}
+
 // Guarded: Adam on g * gstate[kCoef] (grad_guard.cu computed it); with skipped != NULL and a non-finite norm the CTA writes nothing.
+// ranges != NULL: elements outside the ranges are neither read nor written.
 template <bool Guarded>
 __global__ void __launch_bounds__(256) adam_flat_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
                                                         float *__restrict__ v, const int32_t *__restrict__ step_count, int64_t n,
                                                         adam::Hyper h, const float *__restrict__ hyper, const float *__restrict__ gstate,
-                                                        const int32_t *__restrict__ skipped) {
+                                                        const int32_t *__restrict__ skipped, const int64_t *__restrict__ ranges,
+                                                        int32_t num_ranges) {
   if constexpr (Guarded) {
     if (skipped && gstate[guard::kNonFinite] != 0.f) return;
   }
@@ -90,7 +104,7 @@ __global__ void __launch_bounds__(256) adam_flat_kernel(float *__restrict__ p, c
   __syncthreads();
   const adam::Bias c = s_c;
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n || (ranges && !in_ranges(ranges, num_ranges, i))) return;
   float gi = g[i];
   if constexpr (Guarded) gi = gi * gstate[guard::kCoef];     // clip_grad_norm_: grad.mul_(clip_coef_clamped)
   float pi = p[i], mi = m[i], vi = v[i];
@@ -118,11 +132,12 @@ int adam_step_inc_launch(int32_t *step_count, const float *gstate, int32_t *skip
 // the flat update and its step-count increment: two launches (none for the update when numel == 0)
 template <bool Guarded>
 static int adam_flat_launch(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
-                            adam::Hyper h, const float *hyper, const float *gstate, int32_t *skipped, void *stream_) {
+                            adam::Hyper h, const float *hyper, const float *gstate, int32_t *skipped, void *stream_,
+                            const int64_t *ranges = nullptr, int32_t num_ranges = 0) {
   cudaStream_t stream = as_stream(stream_);
   if (numel > 0) {
     adam_flat_kernel<Guarded><<<(unsigned)((numel + 255) / 256), 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel,
-                                                                                  h, hyper, gstate, skipped);
+                                                                                  h, hyper, gstate, skipped, ranges, num_ranges);
     DDFA_CHECK_LAUNCH("adam_flat_kernel");
   }
   return adam_step_inc_launch(step_count, gstate, skipped, stream);
@@ -182,6 +197,21 @@ int ddfa_adam_flat_guarded(float *params, const float *grads, float *exp_avg, fl
   DDFA_REQUIRE(numel >= 0, "ddfa_adam_flat_guarded: negative numel");
   DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && hyper && gstate, "ddfa_adam_flat_guarded: NULL pointer");
   return adam_flat_launch<true>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{}, hyper, gstate, skipped, stream_);
+}
+
+int ddfa_adam_flat_ranges(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                          const int64_t *ranges, int32_t num_ranges, const float *hyper, const float *gstate, int32_t *skipped, void *stream_) {
+  using namespace ddfa;
+  DDFA_REQUIRE(numel >= 0 && num_ranges >= 0, "ddfa_adam_flat_ranges: negative numel (%lld) or num_ranges (%d)", (long long)numel, num_ranges);
+  DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && hyper && (ranges || num_ranges == 0),
+               "ddfa_adam_flat_ranges: NULL pointer");
+  DDFA_REQUIRE(gstate || !skipped, "ddfa_adam_flat_ranges: skipped given without gstate");
+  if (num_ranges == 0) return adam_step_inc_launch(step_count, gstate, skipped, as_stream(stream_));   // nothing to update
+  if (gstate)
+    return adam_flat_launch<true>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{}, hyper, gstate, skipped, stream_,
+                                  ranges, num_ranges);
+  return adam_flat_launch<false>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{}, hyper, nullptr, nullptr, stream_,
+                                 ranges, num_ranges);
 }
 
 }  // extern "C"

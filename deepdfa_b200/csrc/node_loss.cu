@@ -599,7 +599,9 @@ int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *
   DDFA_REQUIRE(N >= 0 && D > 0 && L >= 1 && L <= kMaxLayers, "ddfa_node_head_bwd: bad shape N=%d D=%d num_layers=%d", N, D, L);
   DDFA_REQUIRE(num_rows && mlp_w && dmlp_w && dmlp_b, "ddfa_node_head_bwd: NULL pointer");
   for (int i = 0; i < L; ++i) DDFA_REQUIRE(mlp_w[i] && dmlp_w[i] && dmlp_b[i], "ddfa_node_head_bwd: MLP layer %d pointer NULL", i);
-  DDFA_REQUIRE(N == 0 || (dlogits && h_final && x && rows && dh_final && dx && (L == 1 || mlp_act)), "ddfa_node_head_bwd: NULL pointer");
+  // dh_final == dx == NULL: the MLP gradients only (the encoder is frozen), no [N, D] plane is written
+  DDFA_REQUIRE((dh_final == nullptr) == (dx == nullptr), "ddfa_node_head_bwd: dh_final and dx are both NULL (MLP gradients only) or both given");
+  DDFA_REQUIRE(N == 0 || (dlogits && h_final && x && rows && (L == 1 || mlp_act)), "ddfa_node_head_bwd: NULL pointer");
   if (workspace_bytes < ddfa_node_head_bwd_workspace_bytes(N, D) || workspace == nullptr) {
     set_error("ddfa_node_head_bwd: workspace too small (%zu < %zu)", workspace_bytes, ddfa_node_head_bwd_workspace_bytes(N, D));
     return DDFA_ERR_WORKSPACE;
@@ -609,7 +611,8 @@ int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *
   const size_t plane = (size_t)N * K;
   float *buf[2] = {static_cast<float *>(workspace), static_cast<float *>(workspace) + plane};
   float *partial = buf[1] + plane;
-  if (N > 0) {       // both planes whole: zero outside the listed rows
+  const bool input_grads = dh_final != nullptr;
+  if (N > 0 && input_grads) {       // both planes whole: zero outside the listed rows
     DDFA_CUDA(cudaMemsetAsync(dh_final, 0, sizeof(float) * (size_t)N * D, stream));
     DDFA_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * (size_t)N * D, stream));
   }
@@ -618,7 +621,7 @@ int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *
   int rc = L == 1 ? launch_wgrad<true>(dlogits, nullptr, h_final, x, rows, num_rows, D, 1, dmlp_w[0], dmlp_b[0], partial, stream)
                   : launch_wgrad<false>(dlogits, in_last, nullptr, nullptr, rows, num_rows, D, 1, dmlp_w[L - 1], dmlp_b[L - 1], partial, stream);
   if (rc) return rc;
-  if (N == 0) return DDFA_OK;
+  if (N == 0 || (L == 1 && !input_grads)) return DDFA_OK;
   const unsigned g_elem = cdiv((int64_t)N * K, 256);
   if (L == 1) {
     head_last_bwd_kernel<true><<<g_elem, 256, 0, stream>>>(dlogits, mlp_w[0], nullptr, rows, num_rows, D, N, nullptr, dh_final, dx);
@@ -634,6 +637,7 @@ int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *
     rc = i == 0 ? launch_wgrad<true>(dout, nullptr, h_final, x, rows, num_rows, D, K, dmlp_w[0], dmlp_b[0], partial, stream)
                 : launch_wgrad<false>(dout, in, nullptr, nullptr, rows, num_rows, D, K, dmlp_w[i], dmlp_b[i], partial, stream);
     if (rc) return rc;
+    if (i == 0 && !input_grads) break;
     const dim3 grid(cdiv(N, BM), cdiv(K, BN));
     if (i == 0)
       head_gemm_kernel<false, false, kScatter><<<grid, 256, 0, stream>>>(dout, nullptr, nullptr, rows, num_rows, D, K, K, mlp_w[0], nullptr,

@@ -259,11 +259,13 @@ __global__ void __launch_bounds__(kReadoutWarps * 32) readout_bwd_kernel(
         const int col = (lane + 32 * i) * 4;
         if (col < D) {
           const float4 &dpv = dp.v[q][i], &wv = wg.v[q][i], &ov = o.v[q][i];
-          float4 d;
-          d.x = fmaf(alpha, dpv.x, dg * wv.x); d.y = fmaf(alpha, dpv.y, dg * wv.y);
-          d.z = fmaf(alpha, dpv.z, dg * wv.z); d.w = fmaf(alpha, dpv.w, dg * wv.w);
-          float *dst = (q == 0 ? dh : dx) + (int64_t)n * D + col;
-          *reinterpret_cast<float4 *>(dst) = d;
+          if (dh) {          // NULL: the gate-only form (frozen encoder), no [N, D] plane is written
+            float4 d;
+            d.x = fmaf(alpha, dpv.x, dg * wv.x); d.y = fmaf(alpha, dpv.y, dg * wv.y);
+            d.z = fmaf(alpha, dpv.z, dg * wv.z); d.w = fmaf(alpha, dpv.w, dg * wv.w);
+            float *dst = (q == 0 ? dh : dx) + (int64_t)n * D + col;
+            *reinterpret_cast<float4 *>(dst) = d;
+          }
           f4_fma(dw.v[q][i], dg, ov);
         }
       }
@@ -451,7 +453,10 @@ static int readout_bwd_impl(const char *who, const float *dpooled, const float *
   DDFA_REQUIRE(has_ws || !deterministic(),
                "ddfa_readout_bwd has no deterministic form (DDFA_TUNE_DETERMINISTIC = 1): use ddfa_readout_bwd_ws");
   if (B == 0) return DDFA_OK;
-  DDFA_REQUIRE(dpooled && pooled && h_final && x && graph_ptr && w_gate && gate_logit && seg_max && seg_sum && dh_final && dx && dw_gate && db_gate,
+  // the _ws form takes dh_final == dx == NULL: only dw_gate / db_gate are computed (the encoder below the readout is frozen)
+  DDFA_REQUIRE((dh_final == nullptr) == (dx == nullptr), "%s: dh_final and dx are both NULL (gate gradients only) or both given", who);
+  DDFA_REQUIRE(has_ws || dh_final, "%s: dh_final / dx NULL: the gate-only form is ddfa_readout_bwd_ws", who);
+  DDFA_REQUIRE(dpooled && pooled && h_final && x && graph_ptr && w_gate && gate_logit && seg_max && seg_sum && dw_gate && db_gate,
                "%s: NULL pointer", who);
   float *partial = nullptr;
   if (deterministic()) {

@@ -285,10 +285,14 @@ def node_indices(g: BatchedCFG, concat_all_absdf: bool, feature_key: str, device
 # Forward / backward
 # ------------------------------------------------------------------------------------------
 def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps: int, *, training: bool,
-            engine: int = ENGINE_SIMT, alloc=None, oob_counter: Optional[torch.Tensor] = None, head: bool = True):
+            engine: int = ENGINE_SIMT, alloc=None, oob_counter: Optional[torch.Tensor] = None, head: bool = True,
+            grad_ggnn: bool = True):
     """Returns (pooled [B,2D], logits [B] or None, Saved or None).  ``head=False`` stops before the readout and returns
     (x [N,D], h_T [N,D], Saved or None) instead: the label_style="node" trainer runs its own head over a row list
-    (``node_head_fwd``); Saved then holds no readout state."""
+    (``node_head_fwd``); Saved then holds no readout state.
+    ``training=True, grad_ggnn=False`` (frozen embedding tables and GGNN): the GGNN runs in its inference form — no per-step
+    h / s images or gates are kept — and Saved holds only x, h_T and the readout state, enough for
+    ``backward(..., grad_ggnn=False)``."""
     _require_cuda(*params.flat_list(), dg.indptr, *idx)
     L = _lib.lib()
     _lib.apply_deterministic_mode()
@@ -302,12 +306,13 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     st = _stream_ptr()
 
     use_images = engine == ENGINE_TCGEN05     # activations travel as MMA-ready bf16 hi/lo images (include/ddfa_b200.h)
+    ggnn_train = training and grad_ggnn       # keep the per-step state the GGNN backward reads
     x = alloc.get("x", (N, D))
     h_imgs = None
     if use_images and OPTIONS["packed_state"]:
         # the embedding kernel writes h_0 = x as fp32 rows AND as its activation image (one pass instead of embed + ddfa_act_to_image)
         img_bytes = L.call("ddfa_act_image_bytes", N)
-        n_img = T if training else 2          # training keeps the image of every h_t (the weight-gradient GEMM reads it)
+        n_img = T if ggnn_train else 2        # training keeps the image of every h_t (the weight-gradient GEMM reads it)
         h_imgs = [alloc.get_image(f"h_img{i}", img_bytes, tail_unwritten=i == 0) for i in range(max(n_img, 1))]
         _call("ddfa_embed_concat_fwd_image", ptr_array([_p(t) for t in idx]), ptr_array([_p(t) for t in params.tables]),
               K, V, H, N, _p(x), _p(h_imgs[0]), _p(oob_counter), st)
@@ -327,17 +332,17 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     if use_images and not OPTIONS["packed_state"]:
         # round-1 form (A/B only): fp32 copy of every h_t next to its image, four fp32 gate planes per step
         img_bytes = L.call("ddfa_act_image_bytes", N)
-        n_img = T if training else 2
+        n_img = T if ggnn_train else 2
         h_imgs = [alloc.get_zeroed(f"h_img{i}", (img_bytes,), torch.uint8) for i in range(max(n_img, 1))]
         L.call("ddfa_act_to_image", _p(x), N, D, _p(h_imgs[0]), st)
         for t in range(T):
-            s_t = alloc.get_zeroed(f"s_img{t}" if training else "s_img", (img_bytes,), torch.uint8)
-            h_next = alloc.get(f"h{t + 1}" if training else f"hpp{t % 2}", (N, D))
-            g_t = alloc.get(f"gates{t}", (4, N, D)) if training else None
+            s_t = alloc.get_zeroed(f"s_img{t}" if ggnn_train else "s_img", (img_bytes,), torch.uint8)
+            h_next = alloc.get(f"h{t + 1}" if ggnn_train else f"hpp{t % 2}", (N, D))
+            g_t = alloc.get(f"gates{t}", (4, N, D)) if ggnn_train else None
             _call("ddfa_gather_sum_image", _p(dg.indptr), _p(dg.indices), _p(h_cur), N, D, _p(s_t), None, st, tag="gather_fwd")
             _call("ddfa_gru_step_fwd_image", _p(s_t), _p(h_imgs[t % n_img]), _p(h_cur), _p(dg.indptr), N, D, _p(h_next),
                   _p(h_imgs[(t + 1) % n_img]) if t + 1 < T else None, _p(g_t), _p(ws), ws_bytes, st, tag="ddfa_gru_step_fwd")
-            if training:
+            if ggnn_train:
                 hs.append(h_next); ss.append(s_t); gs.append(g_t)
             h_cur = h_next
     elif use_images:
@@ -347,8 +352,8 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
         gate_bytes = L.call("ddfa_gru_gates_packed_bytes", N, D)
         for t in range(T):
             last = t == T - 1
-            s_t = alloc.get_image(f"s_img{t}" if training else "s_img", img_bytes)
-            g_t = alloc.get(f"gates_pk{t}", (gate_bytes,), torch.uint8) if training else None
+            s_t = alloc.get_image(f"s_img{t}" if ggnn_train else "s_img", img_bytes)
+            g_t = alloc.get(f"gates_pk{t}", (gate_bytes,), torch.uint8) if ggnn_train else None
             h_in_img = h_imgs[t % n_img]
             if t == 0:
                 _call("ddfa_gather_sum_image", _p(dg.indptr), _p(dg.indices), _p(x), N, D, _p(s_t), None, st, tag="gather_fwd")
@@ -357,13 +362,13 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
             h_next = alloc.get("h_final", (N, D)) if last else None
             _call("ddfa_gru_step_fwd_image_v2", _p(s_t), _p(h_in_img), _p(x) if t == 0 else None, _p(dg.indptr), N, D, _p(h_next),
                   None if last else _p(h_imgs[(t + 1) % n_img]), _p(g_t), _p(ws), ws_bytes, st, tag="ddfa_gru_step_fwd")
-            if training:
+            if ggnn_train:
                 hs.append(h_next); ss.append(s_t); gs.append(g_t)
             if last:
                 h_cur = h_next
     else:
         for t in range(T):
-            if training:
+            if ggnn_train:
                 s_t = alloc.get(f"s{t}", (N, D))
                 h_next = alloc.get(f"h{t + 1}", (N, D))
                 g_t = alloc.get(f"gates{t}", (4, N, D))
@@ -374,10 +379,12 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
             _call("ddfa_gather_sum", _p(dg.indptr), _p(dg.indices), _p(h_cur), N, D, _p(s_t), 0, st, tag="gather_fwd")
             _call("ddfa_gru_step_fwd", _p(s_t), _p(h_cur), _p(dg.indptr), _p(w_fold), _p(b_fold), _p(params.b_ih),
                   _p(params.w_hh), _p(params.b_hh), N, D, _p(h_next), _p(g_t), _p(ws), ws_bytes, engine, st)
-            if training:
+            if ggnn_train:
                 hs.append(h_next); ss.append(s_t); gs.append(g_t)
             h_cur = h_next
 
+    if training and not grad_ggnn:
+        hs, ss, gs, h_imgs = [x] + [None] * (T - 1) + [h_cur], [], [], None     # h[T] = h_T for the readout backward
     if not head:
         saved = None
         if training:
@@ -403,14 +410,18 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
 
 def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack, *, dlogits: Optional[torch.Tensor] = None,
              dpooled: Optional[torch.Tensor] = None, engine: int = ENGINE_SIMT, alloc=None, on_small_grads_ready=None,
-             dh_final: Optional[torch.Tensor] = None, dx_direct: Optional[torch.Tensor] = None):
+             dh_final: Optional[torch.Tensor] = None, dx_direct: Optional[torch.Tensor] = None, grad_ggnn: bool = True,
+             grad_tables: bool = True):
     """Accumulates (+=) parameter gradients into ``grads``.  Exactly one of dlogits / dpooled / (dh_final, dx_direct) is given.
     ``dh_final`` / ``dx_direct`` ([N, D] each, from ``node_head_bwd``): the gradients of h_T and of the direct use of x; the
     GGNN backward starts from them and the MLP / readout backward is skipped (their gradients are left alone).  ``dh_final``
     is used as scratch afterwards.
     ``on_small_grads_ready``: called once every gradient EXCEPT those of ggnn.linears[0] and the GRU weight matrices (w_msg,
     b_msg, w_ih, w_hh) is final — with the tcgen05 engine that is before the batched weight-gradient launch, so a data-parallel
-    trainer can start reducing them while that launch runs."""
+    trainer can start reducing them while that launch runs.
+    ``grad_ggnn=False`` (frozen embedding tables and GGNN; ``saved`` may come from ``forward(..., grad_ggnn=False)``): stops after
+    the readout — the gate gradients only, no GGNN gradient, no transposed gather, no embedding backward.
+    ``grad_tables=False`` (frozen embedding tables): the full GGNN backward without the embedding backward."""
     L = _lib.lib()
     det = _lib.apply_deterministic_mode()
     dev = dg.device
@@ -421,7 +432,7 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     N, B = dg.num_nodes, dg.batch_size
     nl = len(params.mlp_w)
     st = _stream_ptr()
-    if dg.indptr_t is None:
+    if dg.indptr_t is None and grad_ggnn:
         raise DdfaError("backward needs the transposed CSR (prepare_graph(need_transpose=True))")
 
     if dh_final is not None or dx_direct is not None:
@@ -439,6 +450,17 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     elif dpooled is None:
         raise DdfaError("backward: neither dlogits nor dpooled given")
 
+    if not grad_ggnn:
+        if dh_final is not None:
+            raise DdfaError("backward: grad_ggnn=False starts from dlogits / dpooled")
+        ro_bytes = L.call("ddfa_readout_bwd_workspace_bytes", B, D)
+        ro_ws = alloc.get("readout_bwd_ws", (max(ro_bytes, 16),), torch.uint8)
+        _call("ddfa_readout_bwd_ws", _p(dpooled), _p(saved.pooled), _p(saved.h[T]), _p(saved.x), _p(dg.graph_ptr), B, D,
+              _p(params.w_gate), _p(saved.gate_logit), _p(saved.seg_max), _p(saved.seg_sum), None, None,
+              _p(grads.w_gate), _p(grads.b_gate), _p(ro_ws), ro_bytes, st, tag="ddfa_readout_bwd")
+        if on_small_grads_ready is not None:
+            on_small_grads_ready()
+        return
     dh_alt = alloc.get("dh_b", (N, D))
     if dh_final is not None:
         dh = dh_final
@@ -485,10 +507,11 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     if engine == ENGINE_TCGEN05 and T > 0 and fuse_gather:     # the gather of the last ds (step 0) has no following step to ride on
         _call("ddfa_gather_sum", _p(dg.indptr_t), _p(dg.indices_t), _p(ds_prev), N, D, _p(dh), 1, st, tag="gather_bwd")
     # the deterministic form's scratch (sort keys and partial sums): allocated only in that mode, the default form does not read it
-    emb_bytes = L.call("ddfa_embed_concat_bwd_workspace_bytes", K, V, H, N) if det else 0
-    emb_ws = alloc.get("embed_bwd_ws", (emb_bytes,), torch.uint8) if emb_bytes else None
-    _call("ddfa_embed_concat_bwd_ws", ptr_array([_p(t) for t in saved.idx]), _p(dh), _p(dx_direct), K, V, H, N,
-          ptr_array([_p(t) for t in grads.tables]), _p(emb_ws), emb_bytes, st, tag="ddfa_embed_concat_bwd")
+    if grad_tables:
+        emb_bytes = L.call("ddfa_embed_concat_bwd_workspace_bytes", K, V, H, N) if det else 0
+        emb_ws = alloc.get("embed_bwd_ws", (emb_bytes,), torch.uint8) if emb_bytes else None
+        _call("ddfa_embed_concat_bwd_ws", ptr_array([_p(t) for t in saved.idx]), _p(dh), _p(dx_direct), K, V, H, N,
+              ptr_array([_p(t) for t in grads.tables]), _p(emb_ws), emb_bytes, st, tag="ddfa_embed_concat_bwd")
     if on_small_grads_ready is not None:
         on_small_grads_ready()
     if engine == ENGINE_TCGEN05 and T > 0:
@@ -568,15 +591,16 @@ def node_bce(logits: torch.Tensor, vuln: torch.Tensor, rows: torch.Tensor, num_r
 
 
 def node_head_bwd(params: ParamPack, grads: ParamPack, dlogits: torch.Tensor, x: torch.Tensor, h_final: torch.Tensor,
-                  rows: torch.Tensor, num_rows: torch.Tensor, act: Optional[torch.Tensor], alloc=None):
+                  rows: torch.Tensor, num_rows: torch.Tensor, act: Optional[torch.Tensor], alloc=None, input_grads: bool = True):
     """``ddfa_node_head_bwd``: accumulates the head's weight / bias gradients into ``grads`` and returns (dh_final, dx_direct),
-    [N, D] each, zero outside the listed rows — the starting point of ``backward(..., dh_final=, dx_direct=)``."""
+    [N, D] each, zero outside the listed rows — the starting point of ``backward(..., dh_final=, dx_direct=)``.
+    ``input_grads=False`` (frozen encoder): the weight / bias gradients only; returns (None, None)."""
     N, D = x.shape
     nl = len(params.mlp_w)
     L = _lib.lib()
     alloc = alloc or _FreshAlloc(x.device)
-    dh = alloc.get("dh_a", (N, D))
-    dx = alloc.get("dx_direct", (N, D))
+    dh = alloc.get("dh_a", (N, D)) if input_grads else None
+    dx = alloc.get("dx_direct", (N, D)) if input_grads else None
     ws_bytes = L.call("ddfa_node_head_bwd_workspace_bytes", N, D)
     ws = alloc.get("node_head_bwd_ws", (max(ws_bytes, 16),), torch.uint8)
     _call("ddfa_node_head_bwd", _p(dlogits), _p(h_final), _p(x), _p(rows), _p(num_rows), N, D,

@@ -49,6 +49,36 @@ def flat_param_list(module):
     return plist
 
 
+def trainable_ranges(plist):
+    """The ``[begin, end)`` element ranges of the flat buffers (laid out by :func:`flat_offsets`) whose tensors have
+    ``requires_grad``, each slot with its alignment padding, adjacent slots merged; the bounds are multiples of ``_ALIGN``.
+    Raises ``ValueError`` when no tensor is trainable."""
+    offs, total = flat_offsets(plist)
+    ranges = []
+    for p, lo, hi in zip(plist, offs, offs[1:] + [total]):
+        if not p.requires_grad:
+            continue
+        if ranges and ranges[-1][1] == lo:
+            ranges[-1] = (ranges[-1][0], hi)
+        else:
+            ranges.append((lo, hi))
+    if not ranges:
+        raise ValueError("FusedTrainer: no parameter of the module has requires_grad=True: there is nothing to train")
+    return ranges
+
+
+def exchange_for_frozen(exchange: str, world: int, frozen: bool):
+    """``(exchange, note)``: the gradient exchange a trainer with frozen parameters uses over ``world`` ranks.  The peer-memory
+    exchange (``"p2p"``) runs Adam over every element of its shard, so with frozen parameters ``"auto"`` picks NCCL (``note``
+    says why) and ``"p2p"`` raises ``NotImplementedError``.  Without frozen parameters or on one rank, nothing changes."""
+    if not frozen or world <= 1 or exchange == "nccl":
+        return exchange, None
+    if exchange == "p2p":
+        raise NotImplementedError("exchange='p2p' with frozen parameters: the peer-memory exchange's sharded Adam updates every "
+                                  "parameter; use exchange='nccl' (or 'auto')")
+    return "nccl", "auto: frozen parameters (the peer-memory exchange updates every parameter): NCCL all-reduce"
+
+
 def owned_range(numel: int, rank: int, world: int):
     """``[lo, hi)``: the elements of the flat buffers whose Adam moments rank ``rank`` of ``world`` keeps up to date under
     ``exchange="p2p"``.  Mirrors ``allreduce_adam_p2p_kernel``: the buffers are cut into 16-byte units and every rank owns
@@ -93,6 +123,8 @@ class FusedAdam(torch.optim.Optimizer):
         if exp_avg.numel() != total or exp_avg_sq.numel() != total:
             raise ValueError(f"FusedAdam: moment buffers of {exp_avg.numel()} / {exp_avg_sq.numel()} elements, layout needs {total}")
         self._slots = [(where[id(p)], p.numel()) for p in params]      # per module.parameters() index: (flat offset, numel)
+        # frozen parameters (requires_grad=False when the trainer was built) get no state, as torch.optim.Adam gives them none
+        self._trainable = [bool(p.requires_grad) for p in params]
         self._flat = (exp_avg, exp_avg_sq, step_count, hyper)
         self._shard = shard
         self._pushed = None
@@ -138,7 +170,8 @@ class FusedAdam(torch.optim.Optimizer):
     def state_dict(self):
         """What ``torch.optim.Adam(module.parameters()).state_dict()`` returns after the same steps: per parameter index
         ``{"step": float32 CPU tensor, "exp_avg", "exp_avg_sq"}`` (copies, shaped like the parameter, on its device) — empty
-        before the first step — and the one parameter group.  Reads the step counter from the device: one synchronisation.
+        before the first step and for parameters frozen when the trainer was built — and the one parameter group.  Reads the
+        step counter from the device: one synchronisation.
         With sharded moments (``exchange="p2p"``) this is a collective: every rank must call it, and every rank gets the
         full state (each rank's owned slice, all-reduced)."""
         g = self._group()
@@ -148,6 +181,8 @@ class FusedAdam(torch.optim.Optimizer):
         state = {}
         if step > 0:
             for i, (p, (o, n)) in enumerate(zip(g["params"], self._slots)):
+                if not self._trainable[i]:
+                    continue
                 state[i] = {"step": torch.tensor(float(step), dtype=torch.float32),
                             "exp_avg": m[o:o + n].view_as(p).clone(), "exp_avg_sq": v[o:o + n].view_as(p).clone()}
         packed = {k: val for k, val in g.items() if k != "params"}
@@ -161,7 +196,8 @@ class FusedAdam(torch.optim.Optimizer):
         moments.  Writes IN PLACE into the flat moment buffers, the step counter and the hyperparameter word, so CUDA
         graphs captured before the load replay from the loaded state.  Every rank loads the full moments, whatever world
         size wrote them.  Raises ``ValueError`` for more than one group, a parameter count or shape mismatch, AMSGrad,
-        ``maximize``, ``decoupled_weight_decay`` (AdamW) or per-parameter steps that differ."""
+        ``maximize``, ``decoupled_weight_decay`` (AdamW) or per-parameter steps that differ.  Entries of parameters frozen when
+        the trainer was built are accepted and ignored; the step count comes from the trainable parameters only."""
         groups = state_dict.get("param_groups")
         if not isinstance(groups, (list, tuple)) or len(groups) != 1:
             raise ValueError(f"FusedAdam loads exactly one parameter group, got {len(groups) if groups is not None else None}")
@@ -179,7 +215,9 @@ class FusedAdam(torch.optim.Optimizer):
         steps, entries = set(), []
         for i, (pid, p) in enumerate(zip(ids, cur)):
             st = state.get(pid)
-            if st:
+            if not self._trainable[i]:
+                entries.append(None)              # frozen: its saved state, if any, is ignored
+            elif st:
                 for key in ("exp_avg", "exp_avg_sq"):
                     if key not in st or tuple(st[key].shape) != tuple(p.shape):
                         raise ValueError(f"parameter {i}: {key} of shape {tuple(st[key].shape) if key in st else None}, "
@@ -245,7 +283,16 @@ class FusedTrainer:
         the device inside the step (``ddfa_node_sample``: Philox keys from ``node_sample_seed`` and the draw counter
         ``node_sample_draws``).  The head runs over that row list only.  A draw that asks for more non-vulnerable nodes than the
         batch has takes them all and raises ``ValueError`` at the next step or at ``check_inputs()`` (``random.sample`` raises
-        on the module path).  One rank only."""
+        on the module path).  One rank only.
+
+        Frozen parameters: a parameter with ``requires_grad=False`` when the trainer is built is not trained — Adam runs over the
+        trainable elements only (``ddfa_adam_flat_ranges``), its gradient slot is zeroed before the norm, and it gets no optimizer
+        state, as with ``torch.optim.Adam(module.parameters())``.  With the embedding tables and the six GatedGraphConv tensors
+        all frozen the GGNN runs in its inference form and the backward stops after the readout (graph style) or the head
+        (node style); with only the tables frozen the embedding backward is skipped.  The trainable set is fixed: changing
+        ``requires_grad`` later raises ``ValueError`` at the next step, and a module with nothing trainable raises at once.  With
+        more than one rank, frozen parameters need the NCCL exchange (``exchange="auto"`` picks it, ``"p2p"`` raises
+        ``NotImplementedError``)."""
         if module.device.type != "cuda":
             raise _lib.DdfaError("FusedTrainer needs the module on a CUDA device (no CPU fallback)")
         self._node = module.hparams.label_style == "node"
@@ -276,7 +323,18 @@ class FusedTrainer:
         # ranks, else "nccl" (the reason is kept in ``exchange_note``).  Measured at N = 2 / 4 / 8: profiles/r03k, r03n, r03o.
         if exchange not in ("auto", "nccl", "p2p"):
             raise ValueError(f"exchange must be 'auto', 'nccl' or 'p2p', got {exchange!r}")
-        self.exchange_note = None
+        # Frozen parameters (requires_grad=False when the trainer is built): Adam runs over the trainable ranges only, frozen
+        # gradient slots are zeroed before the norm, and the backward is pruned to what the trainable parameters need.
+        plist = module.param_list()
+        flat = flat_param_list(module)
+        self._flat_params = flat
+        self._trainable = tuple(bool(p.requires_grad) for p in flat)
+        self._ranges = trainable_ranges(flat)
+        self._frozen = not all(self._trainable)
+        ntab = len(module._tables())
+        self._grad_ggnn = any(self._trainable[:ntab + 6])    # False: tables and all six GatedGraphConv tensors frozen
+        self._grad_tables = any(self._trainable[:ntab])      # False: no embedding backward
+        exchange, self.exchange_note = exchange_for_frozen(exchange, self.world, self._frozen)
         auto = exchange == "auto"
         if auto:
             exchange = "p2p"
@@ -293,11 +351,9 @@ class FusedTrainer:
         # stream of ever-new shapes (un-bucketed real data) degrades to eager launches instead of growing without bound
         self.max_graph_shapes = max_graph_shapes
         self.max_resident_graphs = max_resident_graphs
-        plist = module.param_list()
-        flat = flat_param_list(module)
         offs, total = flat_offsets(flat)
         self.numel = total
-        ntab = len(module._tables())
+        self._frozen_ranges = [(a[1], b[0]) for a, b in zip([(0, 0)] + self._ranges, self._ranges + [(total, total)]) if a[1] < b[0]]
         self._gemm_grad_range = (offs[ntab], offs[ntab + 4])     # flat offsets of [w_msg, b_msg, w_ih, w_hh]
         with torch.cuda.device(self.device):
             if self.exchange == "p2p":
@@ -325,6 +381,8 @@ class FusedTrainer:
             self.step_count = torch.zeros(1, dtype=torch.int32, device=self.device)
             # [lr, beta1, beta2, eps, weight_decay], read by the Adam kernels when they run; written by self.optimizer.step()
             self.hyper = torch.zeros(5, dtype=torch.float32, device=self.device)
+            if self._frozen:
+                self._ranges_dev = torch.tensor(self._ranges, dtype=torch.int64, device=self.device).reshape(-1)
             shard = (self._p2p_rank, self.world, self.pg) if self.exchange == "p2p" else None
             self.optimizer = FusedAdam(module, self.exp_avg, self.exp_avg_sq, self.step_count, self.hyper, lr=lr, betas=betas, eps=eps,
                                        weight_decay=weight_decay, shard=shard)
@@ -472,6 +530,13 @@ class FusedTrainer:
         more non-vulnerable nodes than the batch had."""
         self._raise_deferred_sample_errors(wait=True)
 
+    def _check_trainable(self):
+        """The trainable set is fixed when the trainer is built: torch keeps a step count per parameter, the fused optimizer one
+        for all, so a tensor unfrozen mid-run could not follow torch's bias correction."""
+        if tuple(p.requires_grad for p in self._flat_params) != self._trainable:
+            raise ValueError("FusedTrainer: requires_grad of a parameter changed after the trainer was built; the trainable set "
+                             "is fixed at construction — build a new FusedTrainer (and optimizer state) for the new set")
+
     # ------------------------------------------------------------------------------------
     def _setup_p2p(self, total: int):
         """Symmetric allocations + rendezvous (torch.distributed._symmetric_memory): every rank gets device pointers to every
@@ -510,6 +575,11 @@ class FusedTrainer:
                                                                     self._gstate.data_ptr(), skipped, self._guard_ws.data_ptr()))]
             return [("ddfa_allreduce_adam_p2p_hp", head + (self._ticket.data_ptr(), self.hyper.data_ptr()))]
         flat = (self.flat_p.data_ptr(), self.flat_g.data_ptr(), *adam, self.numel, self.hyper.data_ptr())
+        norm = [("ddfa_grad_norm", (self.flat_g.data_ptr(), self.numel, self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
+                                    self._guard_ws.data_ptr(), self._guard_ws.numel()))] if self._guard else []
+        if self._frozen:
+            ranged = (*flat[:6], self._ranges_dev.data_ptr(), len(self._ranges), self.hyper.data_ptr())
+            return norm + [("ddfa_adam_flat_ranges", ranged + ((self._gstate.data_ptr(), skipped) if self._guard else (None, None)))]
         if self._guard:
             return [("ddfa_grad_norm", (self.flat_g.data_ptr(), self.numel, self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
                                         self._guard_ws.data_ptr(), self._guard_ws.numel())),
@@ -535,22 +605,31 @@ class FusedTrainer:
         self.flat_g.zero_()
         if self._node:
             return self._enqueue_node(dg, idx, vuln, eng, pw, valid_nodes)
-        _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws)
+        _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws,
+                                     grad_ggnn=self._grad_ggnn)
+        prune = dict(grad_ggnn=self._grad_ggnn, grad_tables=self._grad_tables)
         _, _, dlogits = E.graph_label_bce(dg, vuln, logits, pw, 1.0 / global_batch, 1.0 / global_batch, True,
                                           alloc=self.ws, loss_out=self._loss_local if self.exchange == "p2p" else self.loss_slot,
                                           num_valid=num_valid)
         if self.exchange == "p2p":       # the exchange is the update kernel itself
-            E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws)
+            E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws, **prune)
         else:
             split = self.world > 1 and self.overlap_allreduce
             E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws,
-                       on_small_grads_ready=self._reduce_small_grads if split else None)
+                       on_small_grads_ready=self._reduce_small_grads if split else None, **prune)
             if split:
                 lo, hi = self._gemm_grad_range
                 dist.all_reduce(self.flat_g[lo:hi], op=dist.ReduceOp.SUM, group=self.pg)
                 torch.cuda.current_stream().wait_stream(self._ar_stream)     # both halves are in before the norm and Adam
             elif self.world > 1:
                 dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
+        self._enqueue_update()
+
+    def _enqueue_update(self):
+        """The optimizer update that ends the step.  With frozen parameters their gradient slots are cleared first (the full
+        backward of a mixed frozen set writes some of them), so the norm is ``clip_grad_norm_`` over the trainable parameters."""
+        for lo, hi in self._frozen_ranges:
+            self.flat_g[lo:hi].zero_()
         L, stream = _lib.lib(), torch.cuda.current_stream().cuda_stream
         for name, args in self._update:
             L.call(name, *args, stream)
@@ -562,7 +641,8 @@ class FusedTrainer:
         N = dg.num_nodes
         if vuln.dtype != torch.int32:
             vuln = vuln.to(torch.int32)
-        x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False)
+        x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False,
+                                  grad_ggnn=self._grad_ggnn)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
             valid_nodes.fill_(N)
@@ -571,11 +651,12 @@ class FusedTrainer:
                       self._num_rows, self._sample_status, alloc=ws)
         logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
         dlogits = E.node_bce(logits, vuln, rows, self._num_rows, pw, self.loss_slot, alloc=ws)
-        dh, dx = E.node_head_bwd(self.params, self.grads, dlogits, x, h_T, rows, self._num_rows, act, alloc=ws)
-        E.backward(self.params, dg, saved, self.grads, engine=eng, alloc=ws, dh_final=dh, dx_direct=dx)
-        L, stream = _lib.lib(), torch.cuda.current_stream().cuda_stream
-        for name, args in self._update:
-            L.call(name, *args, stream)
+        dh, dx = E.node_head_bwd(self.params, self.grads, dlogits, x, h_T, rows, self._num_rows, act, alloc=ws,
+                                 input_grads=self._grad_ggnn)
+        if self._grad_ggnn:
+            E.backward(self.params, dg, saved, self.grads, engine=eng, alloc=ws, dh_final=dh, dx_direct=dx,
+                       grad_tables=self._grad_tables)
+        self._enqueue_update()
         return rows
 
     def _reduce_small_grads(self):
@@ -743,6 +824,7 @@ class FusedTrainer:
         f1: the batch producer).  With ``use_cuda_graph`` the batch is assembled into static per-shape buffers by
         ``ddfa_arena_batch`` inside one captured graph, so a step costs the H2D copy of the id list plus one graph launch;
         otherwise it is ``step(arena.batch(ids))``."""
+        self._check_trainable()
         self._raise_deferred_sample_errors()
         self.optimizer.step()
         if not self.use_cuda_graph:
@@ -797,6 +879,7 @@ class FusedTrainer:
         """One optimisation step on this rank's shard.  Returns the device tensor holding the
         global mean loss (valid after the step's stream work completes).  Starts with ``self.optimizer.step()``, which hands
         the current learning rate etc. to this step's Adam launch (an LR scheduler on ``self.optimizer`` sees that call)."""
+        self._check_trainable()
         self._raise_deferred_sample_errors()
         self.optimizer.step()
         if self.use_cuda_graph:

@@ -330,7 +330,10 @@ int ddfa_readout_bwd(const float *dpooled, const float *pooled, const float *h_f
                      const float *gate_logit, const float *seg_max, const float *seg_sum,
                      float *dh_final, float *dx, float *dw_gate, float *db_gate, void *stream);
 /* Same, with scratch for the deterministic form (the graphs' dw_gate / db_gate terms added in graph order):
- * ddfa_readout_bwd_workspace_bytes(B, D) bytes; unused in the default mode. */
+ * ddfa_readout_bwd_workspace_bytes(B, D) bytes; unused in the default mode.
+ * dh_final == dx == NULL (this form only): the gate gradients alone, for an encoder whose parameters are frozen — h_final and x
+ * are read once and no [N, D] plane is written; dw_gate / db_gate are bit-identical to the full call's in deterministic mode.
+ * Exactly one of the two NULL is an error. */
 size_t ddfa_readout_bwd_workspace_bytes(int32_t num_graphs, int32_t dim);
 int ddfa_readout_bwd_ws(const float *dpooled, const float *pooled, const float *h_final, const float *x,
                         const int32_t *graph_ptr, int32_t num_graphs, int32_t dim, const float *w_gate,
@@ -384,6 +387,8 @@ int ddfa_graph_label_bce_valid(const float *logits, const int32_t *vuln, const i
  * ddfa_node_head_bwd: dlogits[S] -> dh_final, dx (fp32 [N, D] each, overwritten whole: zero outside the listed rows); accumulates
  *   (+=) dmlp_w / dmlp_b (host arrays of device pointers).  Weight and bias gradients are reduced over the rows in a fixed order
  *   in both tuning modes (32 private partials over fixed row chunks, added in chunk order): bit-reproducible.
+ *   dh_final == dx == NULL: the weight and bias gradients alone (bit-identical to the full call's), for a frozen encoder; no
+ *   [N, D] plane is written.  Exactly one of the two NULL is an error.
  *   workspace: ddfa_node_head_bwd_workspace_bytes(N, D) bytes, 16-byte aligned, scratch.
  * ------------------------------------------------------------------------------------- */
 size_t ddfa_node_sample_workspace_bytes(int32_t num_nodes);
@@ -415,6 +420,14 @@ int ddfa_adam_flat(float *params, const float *grads, float *exp_avg, float *exp
  * before the replay).  Equal values give bit-identical parameters and moments to ddfa_adam_flat. */
 int ddfa_adam_flat_hp(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
                       int32_t *step_count, int64_t numel, const float *hyper, void *stream);
+/* The update over the trainable elements of a partly frozen model: ranges = device int64[2 * num_ranges], sorted, disjoint
+ * [begin, end) pairs inside [0, numel), every bound a multiple of 4.  Elements outside the ranges are neither read nor written
+ * (parameters and both moments stay bit-unchanged); inside, results are bit-identical to ddfa_adam_flat_hp (gstate == NULL) or
+ * ddfa_adam_flat_guarded (gstate != NULL, skipped as there) on the same elements.  step_count advances once per call (not on a
+ * skipped step), also when num_ranges == 0. */
+int ddfa_adam_flat_ranges(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                          int32_t *step_count, int64_t numel, const int64_t *ranges, int32_t num_ranges,
+                          const float *hyper, const float *gstate, int32_t *skipped, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K10'  The data-parallel exchange fused with the optimizer over NVLink peer memory: ONE kernel per rank does
