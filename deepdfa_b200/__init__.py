@@ -4,6 +4,7 @@ Public surface (mirrors the reference for this path only):
   FlowGNNGGNNModule   — drop-in for code_gnn.models.flow_gnn.ggnn.FlowGNNGGNNModule
   BatchedCFG, batch, unbatch, graph, add_self_loop, collate — the DGLGraph subset the path touches
   FusedTrainer        — data-parallel fused train step (NCCL gradient all-reduce + fused Adam)
+  FusedEvaluator      — captured validation / test passes, metrics accumulated on the device
   synth.make_batch    — synthetic Big-Vul-shaped CFG batches
 
 Importing the package does not load the CUDA library; the first kernel call does, and raises if
@@ -12,9 +13,10 @@ Importing the package does not load the CUDA library; the first kernel call does
 from .batched_graph import BatchedCFG, add_self_loop, as_batched_cfg, batch, collate, graph, unbatch  # noqa: F401
 from .module import FlowGNNGGNNModule, allfeats  # noqa: F401
 from .trainer import FusedTrainer  # noqa: F401
+from .evaluator import FusedEvaluator  # noqa: F401
 from .arena import ArenaBatch, GraphArena  # noqa: F401
 from ._lib import DdfaError  # noqa: F401
 from . import synth  # noqa: F401
 
-__all__ = ["FlowGNNGGNNModule", "FusedTrainer", "GraphArena", "ArenaBatch", "BatchedCFG", "batch", "unbatch", "graph", "add_self_loop",
+__all__ = ["FlowGNNGGNNModule", "FusedTrainer", "FusedEvaluator", "GraphArena", "ArenaBatch", "BatchedCFG", "batch", "unbatch", "graph", "add_self_loop",
            "collate", "as_batched_cfg", "synth", "allfeats", "DdfaError"]

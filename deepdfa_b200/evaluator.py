@@ -1,0 +1,316 @@
+"""Fused evaluation of ``FlowGNNGGNNModule``: captured validation / test passes with the metrics accumulated on the device.
+
+Replaces, for evaluation, Lightning's loop around ``BaseModule.validation_step`` / ``test_step`` (base_module.py:211-224,
+238-323) and the torchmetrics objects the epoch ends compute (base_module.py:325-346, 348-383).  Per batch: the GGNN forward in
+its inference form (``engine.forward(training=False)``: two rotating h buffers, no saved gates, no transposed CSR), the readout +
+MLP (graph style) or the node head over every valid node (node style), then ONE metric kernel (``ddfa_eval_metrics_graph`` /
+``ddfa_eval_metrics_rows``) that adds the batch's confusion counts, its mean BCE and, optionally, its probabilities and labels to
+a persistent fp64 device state.  Nothing syncs with the host until :meth:`FusedEvaluator.compute`.
+
+The batch paths are those of :class:`~deepdfa_b200.trainer.FusedTrainer` and share its plumbing: host batches through static
+per-shape buffers (two sets, ``prefetch``) with optional shape bucketing, resident device batches (one captured graph per
+object), graph ids of a :class:`~deepdfa_b200.arena.GraphArena` assembled inside the captured graph, and eager launches beyond
+``max_graph_shapes``.
+"""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+
+from . import _lib
+from . import engine as E
+from . import trainer as T
+from .batched_graph import BatchedCFG, as_batched_cfg
+from .module import FlowGNNGGNNModule, _ENGINES
+
+# the fp64 words of the metric state (include/ddfa_b200.h, DDFA_EVAL_STATE_WORDS)
+TP, FP, TN, FN, SAMPLES, BATCHES, LOSS_W, WEIGHT, STORED, OVERFLOW = range(10)
+
+
+def _ratio(num: float, den: float) -> float:
+    return num / den if den > 0 else 0.0
+
+
+def metrics_from_state(state, prefix: str = "val_") -> dict:
+    """The metrics of a metric state (any float64 tensor or sequence of ``EVAL_STATE_WORDS`` values, e.g. a sum of the states of
+    several ranks): torchmetrics < 0.10's binary defaults — micro average, 0 wherever a denominator is 0 — and Lightning's epoch
+    mean of the batch losses weighted by the batch size (NaN when no batch had a sample).  Keys: ``{prefix}loss``,
+    ``{prefix}Accuracy``, ``{prefix}Precision``, ``{prefix}Recall``, ``{prefix}F1Score``, ``{prefix}confusion`` =
+    ``[[TN, FP], [FN, TP]]`` (sklearn's ``confusion_matrix`` layout) and ``{prefix}num_samples``."""
+    s = [float(v) for v in (state.tolist() if torch.is_tensor(state) else state)]
+    tp, fp, tn, fn = s[TP], s[FP], s[TN], s[FN]
+    n = tp + fp + tn + fn
+    precision, recall = _ratio(tp, tp + fp), _ratio(tp, tp + fn)
+    return {f"{prefix}loss": s[LOSS_W] / s[WEIGHT] if s[WEIGHT] > 0 else float("nan"),
+            f"{prefix}Accuracy": _ratio(tp + tn, n),
+            f"{prefix}Precision": precision,
+            f"{prefix}Recall": recall,
+            f"{prefix}F1Score": _ratio(2.0 * tp, 2.0 * tp + fp + fn),
+            f"{prefix}confusion": [[int(tn), int(fp)], [int(fn), int(tp)]],
+            f"{prefix}num_samples": int(n)}
+
+
+class FusedEvaluator:
+    def __init__(self, model: FlowGNNGGNNModule, use_cuda_graph: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
+                 max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64):
+        """``max_predictions`` > 0 keeps the first that many probabilities and labels (``predictions()``; the reference's
+        ``test_preds`` / ``test_labels``); more samples than that make :meth:`compute` raise, the counts stay complete.
+        ``bucket_nodes`` / ``bucket_edges``: shape bucketing of host batches under ``use_cuda_graph``, as in ``FusedTrainer``
+        (one padding graph, excluded from every metric).  The evaluator reads the module's parameters where they live when a
+        batch runs and never writes them; graphs captured over other parameter storage (a ``FusedTrainer`` built later moves
+        the parameters into its flat buffer) are recaptured."""
+        if model.device.type != "cuda":
+            raise _lib.DdfaError("FusedEvaluator needs the module on a CUDA device (no CPU fallback)")
+        hp = model.hparams
+        if hp.encoder_mode or model._num_layers == 0:
+            raise ValueError("FusedEvaluator: an encoder_mode module returns embeddings, not logits: there is nothing to score")
+        if hp.label_style not in ("graph", "node"):
+            raise ValueError(f"FusedEvaluator: label_style={hp.label_style!r} is not supported ('graph' or 'node')")
+        if int(max_predictions) < 0:
+            raise ValueError(f"max_predictions must be >= 0, got {max_predictions!r}")
+        self.module = model
+        self.device = model.device
+        self._node = hp.label_style == "node"
+        self.use_cuda_graph = bool(use_cuda_graph)
+        self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes = int(bucket_nodes), int(bucket_edges), int(bucket_min_pad_nodes)
+        self.max_graph_shapes = int(max_graph_shapes)
+        self.max_resident_graphs = int(max_resident_graphs)
+        self.max_predictions = int(max_predictions)
+        L = _lib.lib()
+        dev = self.device
+        with torch.cuda.device(dev):
+            self._state = torch.zeros(_lib.EVAL_STATE_WORDS, dtype=torch.float64, device=dev)
+            self._metric_ws = torch.empty(L.call("ddfa_eval_metrics_workspace_bytes"), dtype=torch.uint8, device=dev)
+            cap = max(self.max_predictions, 1)
+            self._probs = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
+            self._labels = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
+            self._oob = torch.zeros(1, dtype=torch.int32, device=dev)        # out-of-range embedding indices (compute() raises)
+            self._num_rows = torch.zeros(1, dtype=torch.int32, device=dev) if self._node else None
+        self.ws = E.Workspace(dev)
+        self._slots = {}
+        self._graphs = {}
+        self._warm_shapes = set()
+        self._copy_stream = None
+        self._param_key = None
+
+    # ---- the metric state ------------------------------------------------------------------------------------------------
+    def reset(self) -> None:
+        """Zeroes the metric state in stream order (the prediction store starts over at position 0)."""
+        self._state.zero_()
+
+    def state(self) -> torch.Tensor:
+        """The float64 device metric state (``EVAL_STATE_WORDS`` words, layout in include/ddfa_b200.h), a view: the evaluator
+        keeps accumulating into it.  Every word is a sum, so ``dist.all_reduce(ev.state())`` adds ranks exactly (integers below
+        2**53) and :meth:`metrics_from_state` turns the sum into the global metrics."""
+        return self._state
+
+    metrics_from_state = staticmethod(metrics_from_state)
+
+    def compute(self, prefix: str = "val_") -> dict:
+        """The metrics of everything evaluated since the last :meth:`reset` (one synchronisation).  Raises ``ValueError`` when
+        no sample was evaluated or predictions overflowed ``max_predictions``, and ``IndexError`` when a batch had node feature
+        indices outside the embedding tables."""
+        s = self._state.cpu()
+        bad = int(self._oob.item())
+        if bad:
+            self._oob.zero_()
+            raise IndexError(f"{bad} node feature indices outside [0, {self.module.input_dim}) in an evaluated batch")
+        n = int(s[TP] + s[FP] + s[TN] + s[FN])
+        if n == 0:
+            raise ValueError("FusedEvaluator.compute: no sample was evaluated since the last reset()")
+        if self._probs is not None and s[OVERFLOW] > 0:
+            raise ValueError(f"FusedEvaluator.compute: {n} predictions, max_predictions={self.max_predictions}: build the "
+                             f"evaluator with max_predictions >= {n}")
+        return metrics_from_state(s, prefix)
+
+    def predictions(self):
+        """``(probs, labels)``: fp32 device tensors of the first ``min(stored, max_predictions)`` samples in evaluation order
+        (graph order, or node order within a batch).  Reads the stored count: one synchronisation."""
+        if self._probs is None:
+            raise ValueError("FusedEvaluator.predictions: built with max_predictions=0 (no prediction store)")
+        k = int(self._state[STORED].item())
+        return self._probs[:k], self._labels[:k]
+
+    # ---- per batch -------------------------------------------------------------------------------------------------------
+    def _params(self):
+        """A ParamPack over the module's current parameter storage; a change of storage drops every captured graph."""
+        m = self.module
+        plist = [p.data for p in m.param_list()]
+        key = tuple(p.data_ptr() for p in plist)
+        if key != self._param_key:
+            if self._param_key is not None:
+                for slot in self._slots.values():
+                    for st in slot.get("sets", [slot]):
+                        st["graph"] = None
+                self._graphs.clear()
+            self._param_key = key
+        return E.ParamPack.from_flat_list(plist, len(m._tables()), m._num_layers)
+
+    def _prepare(self, graph):
+        """The device graph without the transposed CSR (inference reads none), the per-node view in node style, and the
+        embedding indices."""
+        m = self.module
+        g = as_batched_cfg(graph)
+        dg = E.prepare_graph(g, self.device, need_transpose=False)
+        if self._node:
+            dg = E.per_node_view(g, dg)
+        idx = E.node_indices(g, m.concat_all_absdf, m.feature_keys["feature"], self.device)
+        return g, dg, idx
+
+    def _enqueue(self, params, dg, idx, vuln, num_graphs: int, num_valid: Optional[int] = None,
+                 valid_nodes: Optional[torch.Tensor] = None):
+        """Enqueues one batch: the inference forward and the metric kernel.  ``num_graphs``: the batch's graph count (its
+        weight in the loss mean); ``num_valid``: graphs [num_valid, B) are bucket padding; ``valid_nodes``: the int32 device
+        word of the valid node count in node style under bucketing."""
+        m, ws = self.module, self.ws
+        eng = _ENGINES[m.engine]
+        pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
+        if vuln.dtype != torch.int32:
+            vuln = vuln.to(torch.int32)
+        store = (E._p(self._probs), E._p(self._labels), self.max_predictions)
+        mws = (self._metric_ws.data_ptr(), self._metric_ws.numel(), E._stream_ptr())
+        L = _lib.lib()
+        if not self._node:
+            _, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, oob_counter=self._oob)
+            B = dg.batch_size
+            L.call("ddfa_eval_metrics_graph", E._p(logits), E._p(vuln), E._p(dg.graph_ptr), B, B if num_valid is None else int(num_valid),
+                   pw, float(num_graphs), self._state.data_ptr(), *store, *mws)
+            return None
+        N = dg.num_nodes
+        x, h_T, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, head=False, oob_counter=self._oob)
+        if valid_nodes is None:
+            valid_nodes = ws.get("node_valid", (1,), torch.int32)
+            valid_nodes.fill_(N)
+        rows = ws.get("node_rows", (N,), torch.int32)
+        E.node_sample(vuln, valid_nodes, None, 0, None, rows, self._num_rows, None, alloc=ws)
+        logits, _ = E.node_head_fwd(params, x, h_T, rows, self._num_rows, alloc=ws)
+        L.call("ddfa_eval_metrics_rows", E._p(logits), E._p(vuln), E._p(rows), self._num_rows.data_ptr(), N, pw, float(num_graphs),
+               self._state.data_ptr(), *store, *mws)
+        return rows
+
+    def _slot(self, g):
+        N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
+        bucket = T.bucket_shape(N, Eg, self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes)
+        det = _lib.deterministic_requested()
+        key = ("bucket", bucket[0], bucket[1], B, det) if bucket else ("exact", N, Eg, B, det)
+        slot = self._slots.get(key)
+        if slot is None:
+            if len(self._slots) >= self.max_graph_shapes:
+                return None
+            slot = T.new_stream_slot(g, bucket, self.device, self._node)
+            self._slots[key] = slot
+        return slot
+
+    def prefetch(self, batch) -> None:
+        """Starts the host->device copy of a (pinned) host batch on a side stream, overlapping the batch that is running; the
+        following ``update(batch)`` with the SAME batch object picks the staged copy up.  No-op without ``use_cuda_graph`` or
+        for device batches."""
+        if not self.use_cuda_graph:
+            return
+        g = as_batched_cfg(batch)
+        if g.device.type != "cpu":
+            return
+        with torch.cuda.device(self.device):
+            if self._copy_stream is None:
+                self._copy_stream = torch.cuda.Stream(device=self.device)
+            slot = self._slot(g)
+            if slot is not None:
+                slot["staged"] = (id(batch), T.stage(slot, g, self._copy_stream))
+
+    def update(self, batch) -> None:
+        """Adds one batch (host, resident device or DGL batch; ``(batch, extrafeats)`` tuples as Lightning hands them over are
+        accepted) to the metric state.  No host synchronisation."""
+        if isinstance(batch, tuple):
+            batch = batch[0]
+        g = as_batched_cfg(batch)
+        if self.use_cuda_graph and g.device.type == "cpu":
+            return self._update_streamed(batch, g)
+        return self._update_eager(batch)
+
+    def _update_streamed(self, batch, g):
+        with torch.cuda.device(self.device):
+            slot = self._slot(g)
+            if slot is None:          # more shapes than max_graph_shapes: same kernels, launched eagerly
+                return self._update_eager(batch)
+            params = self._params()
+            N, B = slot["N"], g.batch_size
+            main = torch.cuda.current_stream()
+            staged = slot["staged"]
+            slot["staged"] = None
+            if staged is not None and staged[0] == id(batch):
+                i = staged[1]
+                main.wait_event(slot["sets"][i]["ready"])
+            else:
+                i = T.stage(slot, g, main)
+            st = slot["sets"][i]
+
+            def enqueue():
+                gs = BatchedCFG(st["src"], st["dst"], st["bnn"], dict(st["ndata"]), num_nodes=N)   # no cached device CSR
+                _, dg, idx = self._prepare(gs)
+                vuln = gs.ndata["_VULN"]
+                if vuln.dtype != torch.int32:
+                    vuln = vuln.to(torch.int32)
+                st["rows"] = self._enqueue(params, dg, idx, vuln.contiguous(), B, num_valid=slot["valid"], valid_nodes=st["valid_nodes"])
+                st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
+
+            st["graph"] = T.graph_step(self.device, st["graph"], slot["warm"], enqueue)
+            slot["warm"] = True
+            ev = torch.cuda.Event()
+            ev.record(main)
+            st["free"] = ev
+
+    def update_ids(self, arena, ids) -> None:
+        """Adds the graphs ``ids`` of a device-resident :class:`~deepdfa_b200.arena.GraphArena` (assembled by
+        ``ddfa_arena_batch`` inside the captured graph: the H2D copy of the id list plus one graph launch per batch)."""
+        if not self.use_cuda_graph:
+            return self._update_eager(arena.batch(ids))
+        ids_np, B, N, Eg = T.arena_ids(arena, ids, "update_ids")
+        key = ("arena", id(arena), N, Eg, B, _lib.deterministic_requested())
+        slot = self._slots.get(key)
+        with torch.cuda.device(self.device):
+            if slot is None:
+                if len(self._slots) >= self.max_graph_shapes:
+                    return self._update_eager(arena.batch(ids))
+                slot = T.new_arena_slot(arena, B, N, Eg)
+                self._slots[key] = slot
+            params = self._params()
+            T.push_ids(slot, ids_np)
+
+            def enqueue():
+                g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
+                _, dg, idx = self._prepare(g)
+                slot["rows"] = self._enqueue(params, dg, idx, g.ndata["_VULN"], B)
+                slot["keep"] = (g, dg, idx)
+
+            slot["graph"] = T.graph_step(self.device, slot["graph"], slot["warm"], enqueue)
+            slot["warm"] = True
+
+    def _update_eager(self, batch):
+        """Device-resident batch objects (one captured graph per object when ``use_cuda_graph``), or plain eager launches."""
+        g, dg, idx = self._prepare(batch)
+        vuln = g.ndata["_VULN"]
+        if vuln.device != self.device or vuln.dtype != torch.int32:
+            key = "vuln_dev"
+            cached = g._cache.get(key)
+            if cached is None:
+                cached = vuln.to(self.device, non_blocking=True).to(torch.int32).contiguous()
+                g._cache[key] = cached
+            vuln = cached
+        B = g.batch_size
+        with torch.cuda.device(self.device):
+            params = self._params()
+            det = _lib.deterministic_requested()
+            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size, det)
+            graph_key = (id(g), det)
+            capturable = self.use_cuda_graph and as_batched_cfg(batch).device.type == "cuda" and \
+                (graph_key in self._graphs or len(self._graphs) < self.max_resident_graphs)
+            entry = self._graphs.get(graph_key)
+            out = {}
+
+            def enqueue():
+                out["rows"] = self._enqueue(params, dg, idx, vuln, B)
+            cg = T.graph_step(self.device, entry[0] if entry else None, capturable and shape_key in self._warm_shapes, enqueue)
+            if entry is None and cg is not None:
+                self._graphs[graph_key] = (cg, g, idx, vuln, out["rows"])     # keep the captured tensors alive
+            self._warm_shapes.add(shape_key)

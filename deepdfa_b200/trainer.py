@@ -89,6 +89,123 @@ def owned_range(numel: int, rank: int, world: int):
     return 4 * lo, 4 * min(n4, lo + per)
 
 
+# ---- captured-step plumbing shared by FusedTrainer and FusedEvaluator ----------------------------------------------------------
+def graph_step(device, graph, warm: bool, enqueue):
+    """One step through a cached CUDA graph: ``enqueue()`` runs eagerly while the shape is not ``warm`` (its first visit grows
+    the workspace and loads modules outside any capture); after that ``graph`` is replayed, captured first, after a device
+    synchronise, when it is None.  Returns the graph (None when the step ran eagerly)."""
+    if not warm:
+        enqueue()
+        return None
+    if graph is None:
+        torch.cuda.synchronize(device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            enqueue()
+    graph.replay()
+    return graph
+
+
+def bucket_shape(N: int, Eg: int, bucket_nodes: int, bucket_edges: int, min_pad_nodes: int):
+    """Padded (nodes, edges) of a batch under shape bucketing, or None when bucketing is off (``bucket_nodes <= 0``)."""
+    if bucket_nodes <= 0:
+        return None
+    bn, be = bucket_nodes, max(bucket_edges, 1)
+    Nb = (N + max(min_pad_nodes, 1) + bn - 1) // bn * bn
+    Eb = (Eg + be - 1) // be * be
+    return Nb, Eb
+
+
+def new_stream_slot(g, bucket, device, valid_nodes_word: bool) -> dict:
+    """The static per-shape input buffers of host batches shaped like ``g`` (or padded to ``bucket``): two buffer sets, so
+    that while the graph of one set runs the next batch is copied into the other (prefetch).  ``valid_nodes_word``: every set
+    gets an int32 device word with the batch's valid node count (node style under bucketing)."""
+    src, dst = g.edges()
+    N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
+    Ns, Es, Bs = (bucket[0], bucket[1], B + 1) if bucket else (N, Eg, B)
+
+    def new_set():
+        return {"src": torch.empty(Es, dtype=src.dtype, device=device), "dst": torch.empty(Es, dtype=dst.dtype, device=device),
+                "bnn": torch.empty(Bs, dtype=torch.int64, device=device),
+                "ndata": {k: torch.zeros((Ns,) + tuple(v.shape[1:]), dtype=v.dtype, device=device) for k, v in g.ndata.items()},
+                "graph": None, "keep": None, "free": None, "ready": None, "rows": None,
+                "valid_nodes": torch.zeros(1, dtype=torch.int32, device=device) if (bucket and valid_nodes_word) else None}
+    return {"sets": [new_set(), new_set()], "next": 0, "staged": None, "warm": False, "N": Ns,
+            "valid": B if bucket else None,
+            "iota": torch.arange(Es, dtype=src.dtype, device=device) if bucket else None}
+
+
+def stage(slot, g, stream) -> int:
+    """Copies the host batch ``g`` into the slot's next buffer set on ``stream``; returns the set index.  Under bucketing
+    the tails are (re)written too: padding nodes get feature index 0 / _VULN 0, the padding edges become self loops spread
+    round-robin over the padding nodes, and the dummy graph's node count goes into the last ``batch_num_nodes`` entry."""
+    i = slot["next"]
+    slot["next"] = 1 - i
+    st = slot["sets"][i]
+    with torch.cuda.stream(stream):
+        if st["free"] is not None:
+            stream.wait_event(st["free"])           # the graph that last read this set has finished
+        src, dst = g.edges()
+        N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
+        st["src"][:Eg].copy_(src, non_blocking=True)
+        st["dst"][:Eg].copy_(dst, non_blocking=True)
+        st["bnn"][:B].copy_(g.batch_num_nodes(), non_blocking=True)
+        for k, v in g.ndata.items():
+            st["ndata"][k][:N].copy_(v, non_blocking=True)
+        if st["valid_nodes"] is not None:
+            st["valid_nodes"].fill_(N)              # node style: the sampler leaves the padding nodes (the tail) out
+        if slot["valid"] is not None:
+            Nb, Eb = slot["N"], st["src"].shape[0]
+            pad_nodes = Nb - N
+            st["bnn"][B:].fill_(pad_nodes)
+            for k in st["ndata"]:
+                st["ndata"][k][N:].zero_()
+            if Eb > Eg:
+                torch.remainder(slot["iota"][: Eb - Eg], pad_nodes, out=st["src"][Eg:])
+                st["src"][Eg:].add_(N)
+                st["dst"][Eg:].copy_(st["src"][Eg:])
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        st["ready"] = ev
+    return i
+
+
+def arena_ids(arena, ids, who: str):
+    """``(ids as int64 numpy, B, N, E)`` of the graph ids of ``arena``; raises IndexError for an empty list or a bad id."""
+    import numpy as np
+    ids_np = np.asarray(ids.cpu() if isinstance(ids, torch.Tensor) else ids, dtype=np.int64).reshape(-1)
+    if ids_np.size == 0 or ids_np.min() < 0 or ids_np.max() >= arena.num_graphs:
+        raise IndexError(f"{who}: empty id list or graph id out of range")
+    return ids_np, int(ids_np.shape[0]), int(arena.nodes_per_graph[ids_np].sum()), int(arena.edges_per_graph[ids_np].sum())
+
+
+def new_arena_slot(arena, B: int, N: int, Eg: int) -> dict:
+    """Static per-shape outputs of the arena batch producer and a ring of pinned id stages: the host may run several steps
+    ahead of the device (that is what the captured graph is for), so a stage is rewritten only after the H2D copy that last
+    read it has completed."""
+    return {"out": arena.alloc_outputs(B, N, Eg), "stages": [torch.empty(B, dtype=torch.int32).pin_memory() for _ in range(4)],
+            "stage_done": [None] * 4, "turn": 0, "steps": 0,
+            "graph": None, "warm": False, "keep": None, "arena": arena}     # the arena stays alive with its graph
+
+
+def push_ids(slot, ids_np) -> None:
+    """Copies the id list into the slot's next pinned stage and from there, in stream order, into its device id buffer; every
+    256 calls the producer's device error counter of the last batch is checked (one synchronisation)."""
+    import numpy as np
+    k = slot["turn"]
+    slot["turn"] = (k + 1) % len(slot["stages"])
+    if slot["stage_done"][k] is not None:
+        slot["stage_done"][k].synchronize()
+    slot["stages"][k].copy_(torch.from_numpy(ids_np.astype(np.int32)))
+    slot["out"]["ids"].copy_(slot["stages"][k], non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record()
+    slot["stage_done"][k] = ev
+    slot["steps"] += 1
+    if slot["keep"] is not None and slot["steps"] % 256 == 0:
+        slot["keep"][0].check()      # the assembler's device error counter (bad id / totals mismatch): one sync every 256 steps
+
+
 _ADAM_FLAGS = dict(amsgrad=False, maximize=False, foreach=None, capturable=False, differentiable=False, fused=None,
                    decoupled_weight_decay=False)
 _UNSUPPORTED = ("amsgrad", "maximize", "decoupled_weight_decay")
@@ -263,7 +380,8 @@ class FusedTrainer:
                  weight_decay: float = 1e-2, process_group=None, use_cuda_graph: bool = False, max_graph_shapes: int = 8,
                  max_resident_graphs: int = 64, distributed: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
                  bucket_min_pad_nodes: int = 64, overlap_allreduce: bool = True, exchange: str = "auto",
-                 max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False, node_sample_seed: int = 0):
+                 max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False, node_sample_seed: int = 0,
+                 track_metrics: bool = False):
         """``distributed=False`` makes this a single-rank trainer even inside an initialised process group (no all-reduce).
         ``bucket_nodes`` / ``bucket_edges`` > 0 switch on shape bucketing for HOST batches under ``use_cuda_graph``: every batch
         is padded with ONE dummy graph of isolated nodes up to the next multiple of ``bucket_nodes`` nodes (at least
@@ -292,7 +410,12 @@ class FusedTrainer:
         (node style); with only the tables frozen the embedding backward is skipped.  The trainable set is fixed: changing
         ``requires_grad`` later raises ``ValueError`` at the next step, and a module with nothing trainable raises at once.  With
         more than one rank, frozen parameters need the NCCL exchange (``exchange="auto"`` picks it, ``"p2p"`` raises
-        ``NotImplementedError``)."""
+        ``NotImplementedError``).
+
+        ``track_metrics=True``: the step ends with one ``ddfa_eval_metrics_*`` call on its own logits — graph style over the valid
+        graphs, node style over the drawn loss rows (what base_module.py:178-190 feeds ``train_metrics``) — each step weighted by
+        its number of graphs; :meth:`metrics` / :meth:`reset_metrics` mirror ``training_epoch_end``.  This rank's samples only.
+        With the default ``False`` the step enqueues nothing for it."""
         if module.device.type != "cuda":
             raise _lib.DdfaError("FusedTrainer needs the module on a CUDA device (no CPU fallback)")
         self._node = module.hparams.label_style == "node"
@@ -427,6 +550,11 @@ class FusedTrainer:
         # with the guard a step may go non-finite and the run continues: images whose padding rows a producer leaves unwritten
         # get their last tile cleared every step, so no NaN of a skipped step can sit in rows a later, smaller batch pads with
         self.ws = E.Workspace(self.device, scrub_image_tails=self._guard)
+        self.track_metrics = bool(track_metrics)
+        if self.track_metrics:
+            with torch.cuda.device(self.device):
+                self._metric_state = torch.zeros(_lib.EVAL_STATE_WORDS, dtype=torch.float64, device=self.device)
+                self._metric_ws = torch.empty(_lib.lib().call("ddfa_eval_metrics_workspace_bytes"), dtype=torch.uint8, device=self.device)
         self._update = self._update_calls()
         self._graphs = {}
         self._stream_slots = {}
@@ -604,7 +732,12 @@ class FusedTrainer:
         pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
         self.flat_g.zero_()
         if self._node:
-            return self._enqueue_node(dg, idx, vuln, eng, pw, valid_nodes)
+            rows = self._enqueue_node(dg, idx, vuln, eng, pw, valid_nodes)
+            if self.track_metrics:
+                self._enqueue_metrics("ddfa_eval_metrics_rows", (E._p(self._last_logits), E._p(vuln), E._p(rows),
+                                                                 self._num_rows.data_ptr(), dg.num_nodes),
+                                      pw, g.batch_size if num_valid is None else num_valid)
+            return rows
         _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws,
                                      grad_ggnn=self._grad_ggnn)
         prune = dict(grad_ggnn=self._grad_ggnn, grad_tables=self._grad_tables)
@@ -624,6 +757,41 @@ class FusedTrainer:
             elif self.world > 1:
                 dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
         self._enqueue_update()
+        if self.track_metrics:
+            B = dg.batch_size
+            nv = B if num_valid is None else int(num_valid)
+            if vuln.dtype != torch.int32:
+                vuln = vuln.to(torch.int32)
+            self._enqueue_metrics("ddfa_eval_metrics_graph", (E._p(logits), E._p(vuln.contiguous()), E._p(dg.graph_ptr), B, nv), pw, nv)
+
+    def _enqueue_metrics(self, name, head, pw, num_graphs):
+        """track_metrics: the step's logits into the training metric state (no prediction store), weighted by the graph count."""
+        _lib.lib().call(name, *head, pw, float(num_graphs), self._metric_state.data_ptr(), None, None, 0,
+                        self._metric_ws.data_ptr(), self._metric_ws.numel(), torch.cuda.current_stream().cuda_stream)
+
+    def metrics(self, prefix: str = "train_") -> dict:
+        """The training metrics of the steps since the last :meth:`reset_metrics` (``track_metrics=True``; one synchronisation):
+        the keys of ``FusedEvaluator.compute``, the loss being the epoch mean of the step losses weighted by their graph counts.
+        Raises ``ValueError`` when no step was tracked."""
+        from .evaluator import metrics_from_state, SAMPLES
+        if not self.track_metrics:
+            raise ValueError("this FusedTrainer was built with track_metrics=False")
+        s = self._metric_state.cpu()
+        if s[SAMPLES] == 0:
+            raise ValueError("FusedTrainer.metrics: no sample was tracked since the last reset_metrics()")
+        return metrics_from_state(s, prefix)
+
+    def reset_metrics(self) -> None:
+        """Zeroes the training metric state in stream order (``training_epoch_end``)."""
+        if not self.track_metrics:
+            raise ValueError("this FusedTrainer was built with track_metrics=False")
+        self._metric_state.zero_()
+
+    def metric_state(self) -> torch.Tensor:
+        """The float64 device training metric state (``ddfa_eval_metrics_*`` layout), for a cross-rank ``all_reduce``."""
+        if not self.track_metrics:
+            raise ValueError("this FusedTrainer was built with track_metrics=False")
+        return self._metric_state
 
     def _enqueue_update(self):
         """The optimizer update that ends the step.  With frozen parameters their gradient slots are cleared first (the full
@@ -650,6 +818,7 @@ class FusedTrainer:
         E.node_sample(vuln, valid_nodes, m.hparams.undersample_node_on_loss_factor, self.node_sample_seed, self._draw, rows,
                       self._num_rows, self._sample_status, alloc=ws)
         logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
+        self._last_logits = logits
         dlogits = E.node_bce(logits, vuln, rows, self._num_rows, pw, self.loss_slot, alloc=ws)
         dh, dx = E.node_head_bwd(self.params, self.grads, dlogits, x, h_T, rows, self._num_rows, act, alloc=ws,
                                  input_grads=self._grad_ggnn)
@@ -674,28 +843,10 @@ class FusedTrainer:
     # ------------------------------------------------------------------------------------
     # ---- host batches through per-shape static buffers + captured graphs -------------------------------------------------
     def _graph_step(self, graph, warm: bool, enqueue):
-        """One step through a cached CUDA graph: ``enqueue()`` runs eagerly while the shape is not ``warm`` (its first visit
-        grows the workspace and loads modules outside any capture); after that ``graph`` is replayed, captured first, after a
-        device synchronise, when it is None.  Returns the graph (None when the step ran eagerly)."""
-        if not warm:
-            enqueue()
-            return None
-        if graph is None:
-            torch.cuda.synchronize(self.device)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                enqueue()
-        graph.replay()
-        return graph
+        return graph_step(self.device, graph, warm, enqueue)
 
     def _bucket_shape(self, N: int, Eg: int):
-        """Padded (nodes, edges) of a batch under shape bucketing, or None when bucketing is off."""
-        if self.bucket_nodes <= 0:
-            return None
-        bn, be = self.bucket_nodes, max(self.bucket_edges, 1)
-        Nb = (N + max(self.bucket_min_pad_nodes, 1) + bn - 1) // bn * bn
-        Eb = (Eg + be - 1) // be * be
-        return Nb, Eb
+        return bucket_shape(N, Eg, self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes)
 
     def num_bucket_shapes(self) -> int:
         return sum(1 for k in self._stream_slots if k[0] == "bucket")
@@ -711,57 +862,13 @@ class FusedTrainer:
         if slot is None:
             if len(self._stream_slots) >= self.max_graph_shapes:
                 return None
-            src, dst = g.edges()
-            dev = self.device
-            Ns, Es, Bs = (bucket[0], bucket[1], B + 1) if bucket else (N, Eg, B)
-
-            def new_set():
-                st = {"src": torch.empty(Es, dtype=src.dtype, device=dev), "dst": torch.empty(Es, dtype=dst.dtype, device=dev),
-                      "bnn": torch.empty(Bs, dtype=torch.int64, device=dev),
-                      "ndata": {k: torch.zeros((Ns,) + tuple(v.shape[1:]), dtype=v.dtype, device=dev) for k, v in g.ndata.items()},
-                      "graph": None, "keep": None, "free": None, "ready": None, "rows": None,
-                      "valid_nodes": torch.zeros(1, dtype=torch.int32, device=dev) if (bucket and self._node) else None}
-                return st
-            # two input-buffer sets: while the graph of one set runs, the next batch is copied into the other (prefetch)
-            slot = {"sets": [new_set(), new_set()], "next": 0, "staged": None, "warm": False, "N": Ns, "gb": gb,
-                    "valid": B if bucket else None,
-                    "iota": torch.arange(Es, dtype=src.dtype, device=dev) if bucket else None}
+            slot = new_stream_slot(g, bucket, self.device, self._node)
+            slot["gb"] = gb
             self._stream_slots[key] = slot
         return slot
 
     def _stage(self, slot, g, stream):
-        """Copies the host batch ``g`` into the slot's next buffer set on ``stream``; returns the set index.  Under bucketing
-        the tails are (re)written too: padding nodes get feature index 0 / _VULN 0, the padding edges become self loops spread
-        round-robin over the padding nodes, and the dummy graph's node count goes into the last ``batch_num_nodes`` entry."""
-        i = slot["next"]
-        slot["next"] = 1 - i
-        st = slot["sets"][i]
-        with torch.cuda.stream(stream):
-            if st["free"] is not None:
-                stream.wait_event(st["free"])           # the graph that last read this set has finished
-            src, dst = g.edges()
-            N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
-            st["src"][:Eg].copy_(src, non_blocking=True)
-            st["dst"][:Eg].copy_(dst, non_blocking=True)
-            st["bnn"][:B].copy_(g.batch_num_nodes(), non_blocking=True)
-            for k, v in g.ndata.items():
-                st["ndata"][k][:N].copy_(v, non_blocking=True)
-            if st["valid_nodes"] is not None:
-                st["valid_nodes"].fill_(N)              # node style: the sampler leaves the padding nodes (the tail) out
-            if slot["valid"] is not None:
-                Nb, Eb = slot["N"], st["src"].shape[0]
-                pad_nodes = Nb - N
-                st["bnn"][B:].fill_(pad_nodes)
-                for k in st["ndata"]:
-                    st["ndata"][k][N:].zero_()
-                if Eb > Eg:
-                    torch.remainder(slot["iota"][: Eb - Eg], pad_nodes, out=st["src"][Eg:])
-                    st["src"][Eg:].add_(N)
-                    st["dst"][Eg:].copy_(st["src"][Eg:])
-            ev = torch.cuda.Event()
-            ev.record(stream)
-            st["ready"] = ev
-        return i
+        return stage(slot, g, stream)
 
     def prefetch(self, batch, global_batch: Optional[int] = None) -> None:
         """Starts the host->device copy of a (pinned) host batch on a side stream so that it overlaps the step that is running;
@@ -829,14 +936,8 @@ class FusedTrainer:
         self.optimizer.step()
         if not self.use_cuda_graph:
             return self._step_eager(arena.batch(ids), global_batch)
-        import numpy as np
         m = self.module
-        ids_np = np.asarray(ids.cpu() if isinstance(ids, torch.Tensor) else ids, dtype=np.int64).reshape(-1)
-        if ids_np.size == 0 or ids_np.min() < 0 or ids_np.max() >= arena.num_graphs:
-            raise IndexError("step_ids: empty id list or graph id out of range")
-        B = int(ids_np.shape[0])
-        N = int(arena.nodes_per_graph[ids_np].sum())
-        Eg = int(arena.edges_per_graph[ids_np].sum())
+        ids_np, B, N, Eg = arena_ids(arena, ids, "step_ids")
         gb = self._global_batch(global_batch, B)
         key = ("arena", id(arena), N, Eg, B, gb, _lib.deterministic_requested())
         slot = self._stream_slots.get(key)
@@ -844,24 +945,9 @@ class FusedTrainer:
             if slot is None:
                 if len(self._stream_slots) >= self.max_graph_shapes:
                     return self._step_eager(arena.batch(ids), global_batch)
-                # a ring of pinned id stages: the host may run several steps ahead of the device (that is what the captured
-                # graph is for), so a stage is rewritten only after the H2D copy that last read it has completed
-                slot = {"out": arena.alloc_outputs(B, N, Eg), "stages": [torch.empty(B, dtype=torch.int32).pin_memory() for _ in range(4)],
-                        "stage_done": [None] * 4, "turn": 0, "steps": 0,
-                        "graph": None, "warm": False, "keep": None, "arena": arena}     # the arena stays alive with its graph
+                slot = new_arena_slot(arena, B, N, Eg)
                 self._stream_slots[key] = slot
-            k = slot["turn"]
-            slot["turn"] = (k + 1) % len(slot["stages"])
-            if slot["stage_done"][k] is not None:
-                slot["stage_done"][k].synchronize()
-            slot["stages"][k].copy_(torch.from_numpy(ids_np.astype(np.int32)))
-            slot["out"]["ids"].copy_(slot["stages"][k], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record()
-            slot["stage_done"][k] = ev
-            slot["steps"] += 1
-            if slot["keep"] is not None and slot["steps"] % 256 == 0:
-                slot["keep"][0].check()      # the assembler's device error counter (bad id / totals mismatch): one sync every 256 steps
+            push_ids(slot, ids_np)
 
             def enqueue():
                 g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])

@@ -407,6 +407,44 @@ int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *
                        float *const *dmlp_b, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K9  evaluation metrics accumulated on the device (csrc/eval_metrics.cu).  Replaces the torchmetrics bookkeeping of
+ * BaseModule.validation_step (base_module.py:211-224: val_loss, Accuracy / Precision / Recall / F1Score of sigmoid(out)), of
+ * test_step (base_module.py:238-323: the same metrics plus CatMetric test_preds / test_labels for the confusion matrix, the sklearn
+ * report and the PR curve) and what the epoch ends compute from them (base_module.py:325-346).  One call adds one batch to a
+ * persistent device METRIC STATE; nothing syncs with the host, so the launches can be captured into a CUDA graph.
+ *
+ * state: DDFA_EVAL_STATE_WORDS fp64 words, zero-initialised by the caller, 8-byte aligned:
+ *   [0] TP  [1] FP  [2] TN  [3] FN  [4] samples  [5] batches  [6] sum_b loss_b * weight_b  [7] sum_b weight_b
+ *   [8] predictions stored  [9] predictions dropped (overflow)  [10..15] reserved (left at zero)
+ *   loss_b = the mean BCEWithLogits(pos_weight) over the batch's samples; a batch without samples adds no loss and no weight.
+ *   Every count is an integer held exactly in fp64 (< 2^53), so states of several ranks add exactly (one all-reduce).
+ * Per sample: x = logit, y = label (0 / 1), p = 1.f / (1.f + expf(-x)) (torch.sigmoid's expression), predicted positive iff
+ *   p >= 0.5f — the binarisation of torchmetrics < 0.10, which val_* / test_* use.  The sklearn report of test_epoch_end uses
+ *   p > 0.5; the two rules differ only at p == 0.5 exactly.  The BCE term is graph_label_bce's stable form, in fp32, summed in fp64.
+ * Prediction store (probs_out / labels_out both NULL, or both fp32[capacity]): the batch's p and y go to positions
+ *   state[8] + i (i = graph or row index), in input order; positions >= capacity are dropped and counted in state[9], the counts
+ *   stay complete.
+ * Order: per-CTA fp64 partials over a grid that depends on the capacity (num_graphs or num_nodes) only, added in CTA order by a
+ *   second one-thread launch that also updates the state, in stream order: the state is bit-reproducible in both
+ *   DDFA_TUNE_DETERMINISTIC modes.  Two launches per call.
+ * weight: the batch's weight in the loss mean (finite, >= 0), by value.
+ * workspace: ddfa_eval_metrics_workspace_bytes() bytes, 8-byte aligned, scratch.
+ *
+ * ddfa_eval_metrics_graph: label_style="graph".  Graph b < num_valid: y = max of vuln over [graph_ptr[b], graph_ptr[b+1]) (as
+ *   ddfa_graph_label_bce), x = logits[b].  Graphs [num_valid, num_graphs) are bucket padding and are ignored.
+ * ddfa_eval_metrics_rows: label_style="node".  Row s < S = *num_rows (a device word, clamped to [0, num_nodes]):
+ *   x = logits[s] (compact, as ddfa_node_head_fwd writes them), y = vuln[rows[s]] (as ddfa_node_bce reads them).
+ * ------------------------------------------------------------------------------------- */
+#define DDFA_EVAL_STATE_WORDS 16
+size_t ddfa_eval_metrics_workspace_bytes(void);
+int ddfa_eval_metrics_graph(const float *logits, const int32_t *vuln, const int32_t *graph_ptr, int32_t num_graphs,
+                            int32_t num_valid, float pos_weight, double weight, double *state, float *probs_out,
+                            float *labels_out, int64_t capacity, void *workspace, size_t workspace_bytes, void *stream);
+int ddfa_eval_metrics_rows(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows,
+                           int32_t num_nodes, float pos_weight, double weight, double *state, float *probs_out,
+                           float *labels_out, int64_t capacity, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K10  torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 (DDFA/configs/
  * config_default.yaml:43-47) over one flat parameter buffer.  step_count: int32[1] device
  * counter, incremented by the kernel (graph-capture safe).
