@@ -458,6 +458,10 @@ static int readout_bwd_impl(const char *who, const float *dpooled, const float *
   DDFA_REQUIRE(has_ws || dh_final, "%s: dh_final / dx NULL: the gate-only form is ddfa_readout_bwd_ws", who);
   DDFA_REQUIRE(dpooled && pooled && h_final && x && graph_ptr && w_gate && gate_logit && seg_max && seg_sum && dw_gate && db_gate,
                "%s: NULL pointer", who);
+  // the kernel reads and writes every [., D] row with 16-byte vector accesses (dh_final / dx may be NULL: aligned16(NULL) holds)
+  DDFA_REQUIRE(aligned16(dpooled) && aligned16(pooled) && aligned16(h_final) && aligned16(x) && aligned16(w_gate) && aligned16(dh_final) &&
+                   aligned16(dx),
+               "%s: 16-byte alignment required", who);
   float *partial = nullptr;
   if (deterministic()) {
     if (workspace == nullptr || workspace_bytes < ddfa_readout_bwd_workspace_bytes(B, D)) {

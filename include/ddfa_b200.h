@@ -324,7 +324,8 @@ int ddfa_mlp_bwd(const float *dlogits, const float *pooled, const float *mlp_act
                  float *dpooled, float *const *dmlp_w, float *const *dmlp_b, float *scratch,
                  void *stream);
 /* Readout backward: dpooled[B,2D] -> dh_final[N,D], dx[N,D] (both overwritten);
- * accumulates dw_gate[2D], db_gate[1] (+=). */
+ * accumulates dw_gate[2D], db_gate[1] (+=).  dpooled, pooled, h_final, x, w_gate, dh_final and dx
+ * must be 16-byte aligned. */
 int ddfa_readout_bwd(const float *dpooled, const float *pooled, const float *h_final, const float *x,
                      const int32_t *graph_ptr, int32_t num_graphs, int32_t dim, const float *w_gate,
                      const float *gate_logit, const float *seg_max, const float *seg_sum,

@@ -60,6 +60,23 @@ def test_argument_validation_is_reported_without_a_gpu(libpath):
     assert rc == -1 and "FWD_PAIR" in L.last_error() and L.call("ddfa_tuning_get", _lib.TUNE_FWD_PAIR) == 0
 
 
+@pytest.mark.parametrize("name", ["ddfa_readout_bwd", "ddfa_readout_bwd_ws"])
+@pytest.mark.parametrize("arg", ["dpooled", "pooled", "h_final", "x", "w_gate", "dh_final", "dx"])
+def test_readout_bwd_rejects_unaligned_rows_without_a_gpu(libpath, name, arg):
+    """The readout backward reads and writes its [., D] rows with 16-byte vector accesses: each of those pointers 4 bytes off is
+    refused before any launch (fake pointers: a launch would fault)."""
+    L = _lib.lib()
+    F = 256
+    names = ["dpooled", "pooled", "h_final", "x", "graph_ptr", "B", "D", "w_gate", "gate_logit", "seg_max", "seg_sum", "dh_final",
+             "dx", "dw_gate", "db_gate"]
+    args = [F] * len(names)
+    args[names.index("B")], args[names.index("D")] = 4, 128
+    args[names.index(arg)] = F + 4
+    extra = (F, 1 << 20, None) if name.endswith("_ws") else (None,)
+    rc = L.raw(name)(*args, *extra)
+    assert rc == -1 and "16-byte alignment" in L.last_error()
+
+
 def test_header_is_plain_c_and_a_c_host_links_the_library(libpath, tmp_path):
     """The boundary is a C ABI: include/ddfa_b200.h must compile as C99 (no C++, no torch / CUDA headers) and a C host must link
     against libddfa_b200.so and call the entry points that need no GPU (version, error string, size queries, argument validation)."""
