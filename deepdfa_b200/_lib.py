@@ -100,11 +100,13 @@ _SIGNATURES = {
     "ddfa_node_sample": (_int, [_vp, _vp, _i32, C.c_double, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ddfa_node_head_fwd": (_int, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
     "ddfa_node_bce": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, _vp, _vp, _vp]),
+    "ddfa_node_bce_scaled": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, _f32, _vp, _vp, _vp]),
     "ddfa_node_head_bwd_workspace_bytes": (_sz, [_i32, _i32]),
     "ddfa_node_head_bwd": (_int, [_vp] * 5 + [_i32, _i32, _vp, _i32] + [_vp] * 6 + [_sz, _vp]),
     "ddfa_eval_metrics_workspace_bytes": (_sz, []),
     "ddfa_eval_metrics_graph": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, C.c_double, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
     "ddfa_eval_metrics_rows": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, C.c_double, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
+    "ddfa_grad_accumulate": (_int, [_vp, _vp, _i64, _i64, _i32, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
 }
 
@@ -118,6 +120,7 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
               "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes"}
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
+GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate
 
 
 class _Lib:

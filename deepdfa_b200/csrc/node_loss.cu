@@ -447,13 +447,15 @@ __global__ void __launch_bounds__(256) chunk_reduce_kernel(const float *__restri
   out[i] += acc;
 }
 
-// mean BCEWithLogits(pos_weight) over the S rows, one CTA in a fixed order (graph_label_bce_kernel's formula); S = 0 gives NaN
+// mean BCEWithLogits(pos_weight) over the S rows, one CTA in a fixed order (graph_label_bce_kernel's formula); S = 0 gives NaN.
+// Scaled: the gradient's row scale is (1 / S) * grad_scale (gradient accumulation); the unscaled form never reads grad_scale.
+template <bool Scaled>
 __global__ void __launch_bounds__(1024) node_bce_kernel(const float *__restrict__ logits, const int32_t *__restrict__ vuln,
                                                         const int32_t *__restrict__ rows, const int32_t *__restrict__ num_rows, float pos_weight,
-                                                        float *__restrict__ loss_out, float *__restrict__ dlogits) {
+                                                        float grad_scale, float *__restrict__ loss_out, float *__restrict__ dlogits) {
   __shared__ float s_t[1024];
   const int32_t S = *num_rows;
-  const float inv = 1.f / (float)S;
+  const float inv = Scaled ? (1.f / (float)S) * grad_scale : 1.f / (float)S;
   float acc = 0.f;
   for (int32_t s = threadIdx.x; s < S; s += 1024) {
     const float xv = logits[s], y = (float)vuln[rows[s]];
@@ -579,7 +581,18 @@ int ddfa_node_bce(const float *logits, const int32_t *vuln, const int32_t *rows,
   using namespace ddfa::node;
   DDFA_REQUIRE(N >= 0, "ddfa_node_bce: num_nodes=%d < 0", N);
   DDFA_REQUIRE(logits && vuln && rows && num_rows, "ddfa_node_bce: NULL pointer");
-  node_bce_kernel<<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, pos_weight, loss_out, dlogits);
+  node_bce_kernel<false><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, pos_weight, 1.f, loss_out, dlogits);
+  DDFA_CHECK_LAUNCH("node_bce_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_node_bce_scaled(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows, int32_t N,
+                         float pos_weight, float grad_scale, float *loss_out, float *dlogits, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  DDFA_REQUIRE(N >= 0, "ddfa_node_bce_scaled: num_nodes=%d < 0", N);
+  DDFA_REQUIRE(logits && vuln && rows && num_rows, "ddfa_node_bce_scaled: NULL pointer");
+  node_bce_kernel<true><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, pos_weight, grad_scale, loss_out, dlogits);
   DDFA_CHECK_LAUNCH("node_bce_kernel");
   return DDFA_OK;
 }

@@ -581,13 +581,27 @@ def node_head_fwd(params: ParamPack, x: torch.Tensor, h_final: torch.Tensor, row
 
 
 def node_bce(logits: torch.Tensor, vuln: torch.Tensor, rows: torch.Tensor, num_rows: torch.Tensor, pos_weight: float,
-             loss_out: torch.Tensor, alloc=None):
-    """``ddfa_node_bce``: the mean BCE over the S rows into ``loss_out`` and dlogits (fp32 [N] capacity), returned."""
+             loss_out: torch.Tensor, alloc=None, grad_scale: Optional[float] = None):
+    """``ddfa_node_bce``: the mean BCE over the S rows into ``loss_out`` and dlogits (fp32 [N] capacity), returned.
+    ``grad_scale``: ``ddfa_node_bce_scaled`` instead, dlogits scaled by it (the loss is not); None: the unscaled entry point."""
     N = logits.numel()
     alloc = alloc or _FreshAlloc(logits.device)
     dlogits = alloc.get("node_dlogits", (N,))
-    _call("ddfa_node_bce", _p(logits), _p(vuln), _p(rows), _p(num_rows), N, float(pos_weight), _p(loss_out), _p(dlogits), _stream_ptr())
+    if grad_scale is None:
+        _call("ddfa_node_bce", _p(logits), _p(vuln), _p(rows), _p(num_rows), N, float(pos_weight), _p(loss_out), _p(dlogits), _stream_ptr())
+    else:
+        _call("ddfa_node_bce_scaled", _p(logits), _p(vuln), _p(rows), _p(num_rows), N, float(pos_weight), float(grad_scale), _p(loss_out),
+              _p(dlogits), _stream_ptr())
     return dlogits
+
+
+def grad_accumulate(acc: torch.Tensor, grads: torch.Tensor, begin: int, end: int, mode: int) -> None:
+    """``ddfa_grad_accumulate`` over the elements ``[begin, end)`` of two flat fp32 buffers: ``mode`` is
+    ``_lib.GRAD_ACC_SET`` (acc = grads), ``GRAD_ACC_ADD`` (acc += grads) or ``GRAD_ACC_APPLY`` (grads += acc)."""
+    _require_cuda(acc, grads)
+    if acc.dtype != torch.float32 or grads.dtype != torch.float32 or acc.numel() < end or grads.numel() < end:
+        raise DdfaError(f"grad_accumulate: fp32 buffers of at least {end} elements needed")
+    _call("ddfa_grad_accumulate", _p(acc), _p(grads), int(begin), int(end), int(mode), _stream_ptr())
 
 
 def node_head_bwd(params: ParamPack, grads: ParamPack, dlogits: torch.Tensor, x: torch.Tensor, h_final: torch.Tensor,

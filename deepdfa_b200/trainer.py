@@ -15,6 +15,7 @@ from __future__ import annotations
 
 from typing import Optional
 
+import numbers
 import os
 
 import torch
@@ -206,6 +207,8 @@ def push_ids(slot, ids_np) -> None:
         slot["keep"][0].check()      # the assembler's device error counter (bad id / totals mismatch): one sync every 256 steps
 
 
+_FIRST, _ADD, _APPLY = "first", "add", "apply"     # what a micro-batch does with its gradient (FusedTrainer._phase)
+
 _ADAM_FLAGS = dict(amsgrad=False, maximize=False, foreach=None, capturable=False, differentiable=False, fused=None,
                    decoupled_weight_decay=False)
 _UNSUPPORTED = ("amsgrad", "maximize", "decoupled_weight_decay")
@@ -268,8 +271,10 @@ class FusedAdam(torch.optim.Optimizer):
         self._pushed = vals
 
     def step(self, closure=None):
-        """Hands ``param_groups[0]``'s lr / betas / eps / weight_decay to the kernels of the NEXT trainer step (the trainer
-        calls this at the start of every step; a value is written only when it changed).  Computes nothing itself."""
+        """Hands ``param_groups[0]``'s lr / betas / eps / weight_decay to the kernels of the NEXT trainer step that updates the
+        parameters (the trainer calls this at the start of every such step — with gradient accumulation, the last micro-batch
+        of a window and ``flush()`` — so a scheduler stepped once per optimizer step follows the windows; a value is written
+        only when it changed).  Computes nothing itself."""
         if closure is not None:
             raise ValueError("FusedAdam.step takes no closure: FusedTrainer.step runs forward and backward")
         self._push()
@@ -381,7 +386,7 @@ class FusedTrainer:
                  max_resident_graphs: int = 64, distributed: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
                  bucket_min_pad_nodes: int = 64, overlap_allreduce: bool = True, exchange: str = "auto",
                  max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False, node_sample_seed: int = 0,
-                 track_metrics: bool = False):
+                 track_metrics: bool = False, accumulate_grad_batches: int = 1):
         """``distributed=False`` makes this a single-rank trainer even inside an initialised process group (no all-reduce).
         ``bucket_nodes`` / ``bucket_edges`` > 0 switch on shape bucketing for HOST batches under ``use_cuda_graph``: every batch
         is padded with ONE dummy graph of isolated nodes up to the next multiple of ``bucket_nodes`` nodes (at least
@@ -415,7 +420,25 @@ class FusedTrainer:
         ``track_metrics=True``: the step ends with one ``ddfa_eval_metrics_*`` call on its own logits — graph style over the valid
         graphs, node style over the drawn loss rows (what base_module.py:178-190 feeds ``train_metrics``) — each step weighted by
         its number of graphs; :meth:`metrics` / :meth:`reset_metrics` mirror ``training_epoch_end``.  This rank's samples only.
-        With the default ``False`` the step enqueues nothing for it."""
+        With the default ``False`` the step enqueues nothing for it.
+
+        ``accumulate_grad_batches=k`` (Lightning's ``accumulate_grad_batches``, the ``--gradient_accumulation_steps`` of HF-style
+        loops): every :meth:`step` / :meth:`step_ids` call is one micro-batch whose gradient is that of its loss divided by ``k``;
+        the gradients of ``k`` consecutive micro-batches (a window) are summed in fp32, in micro-batch order, and the window's last
+        micro-batch runs the exchange, the guard and Adam over that sum — once per window, as DDP's ``no_sync`` does.  The other
+        micro-batches run no collective, no norm and no Adam, and do not call ``optimizer.step()``; the step count advances once
+        per window.  The returned loss is the micro-batch's own mean loss, not divided by ``k``; on a micro-batch that does not
+        end its window, with more than one rank, it is this rank's share of it (no collective runs).  :attr:`accumulated` counts
+        the micro-batches of the open window; :meth:`flush` applies a partial one (the end of an epoch).  Node-row draws,
+        ``track_metrics``, bucketing and input checks stay per micro-batch.  ``optimizer.state_dict()`` may be taken during an
+        open window: it holds no partial sum (as Lightning does not checkpoint ``.grad``), so a resumed run starts a fresh
+        window.  ``k`` is fixed for the trainer's life.  With the default ``k = 1`` the step enqueues exactly what it did without
+        the argument."""
+        k = accumulate_grad_batches
+        if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
+            raise ValueError(f"accumulate_grad_batches must be an integer >= 1, got {accumulate_grad_batches!r}")
+        self._k = int(k)
+        self._accumulated = 0
         if module.device.type != "cuda":
             raise _lib.DdfaError("FusedTrainer needs the module on a CUDA device (no CPU fallback)")
         self._node = module.hparams.label_style == "node"
@@ -501,6 +524,8 @@ class FusedTrainer:
                 self.flat_g = torch.zeros(total + _ALIGN, dtype=torch.float32, device=self.device)  # [+ loss slot]
             self.exp_avg = torch.zeros(total, dtype=torch.float32, device=self.device)
             self.exp_avg_sq = torch.zeros(total, dtype=torch.float32, device=self.device)
+            # the window's gradient sum (ddfa_grad_accumulate), laid out as flat_g without its loss slot; only with k > 1
+            self._acc = torch.zeros(total, dtype=torch.float32, device=self.device) if self._k > 1 else None
             self.step_count = torch.zeros(1, dtype=torch.int32, device=self.device)
             # [lr, beta1, beta2, eps, weight_decay], read by the Adam kernels when they run; written by self.optimizer.step()
             self.hyper = torch.zeros(5, dtype=torch.float32, device=self.device)
@@ -604,7 +629,80 @@ class FusedTrainer:
         """Steps skipped because their gradient norm was not finite (reads the device counter: one synchronisation)."""
         return int(self._skipped.item()) if self._guard else 0
 
-    # ---- label_style="node" ------------------------------------------------------------------------------------------------
+    # ---- gradient accumulation ---------------------------------------------------------------------------------------------
+    @property
+    def accumulated(self) -> int:
+        """Micro-batches in the open accumulation window: 0 right after an update (always 0 with ``accumulate_grad_batches=1``)."""
+        return self._accumulated
+
+    def _phase(self) -> str:
+        """What the next micro-batch does with its gradient: ``"first"`` (starts the window's sum), ``"add"`` (adds to it) or
+        ``"apply"`` (adds the sum to its own gradient, then exchange, guard and Adam — every step with ``k = 1``)."""
+        if self._accumulated == self._k - 1:
+            return _APPLY
+        return _FIRST if self._accumulated == 0 else _ADD
+
+    def _phase_key(self, phase: str) -> tuple:
+        """Part of every captured-graph key: a graph bakes in its phase's launches.  Empty with ``k = 1`` (the keys stay as they were)."""
+        return () if self._k == 1 else (phase,)
+
+    def _begin(self) -> str:
+        """Start of a micro-batch: the checks of every step, and the optimizer's ``step()`` when this one updates the parameters."""
+        self._check_trainable()
+        self._raise_deferred_sample_errors()
+        phase = self._phase()
+        if phase == _APPLY:
+            self.optimizer.step()
+        return phase
+
+    def _end(self, phase: str) -> torch.Tensor:
+        """Counts the enqueued micro-batch into the window and returns its loss word.  Under peer memory, where the exchange kernel
+        writes the global loss into a local word, a micro-batch that runs no exchange returns this rank's own loss slot."""
+        self._accumulated = 0 if phase == _APPLY else self._accumulated + 1
+        if phase != _APPLY and self.exchange == "p2p":
+            return self._loss_local
+        return self.loss_slot
+
+    def flush(self) -> None:
+        """Applies the open window now, short as it is: the exchange, the guard and Adam over the gradients accumulated so far
+        (each still scaled by ``1 / accumulate_grad_batches``), with no forward pass — what Lightning does on the last batch of an
+        epoch.  Calls ``optimizer.step()`` first, as a full window does.  Does nothing when the window is empty.  Collective when
+        the exchange is: every rank must call it.  The loss slot is not touched, so on one rank the last micro-batch's returned
+        loss keeps its value."""
+        if self._accumulated == 0:
+            return
+        self._check_trainable()
+        self.optimizer.step()
+        with torch.cuda.device(self.device):
+            self.flat_g[:self.numel].zero_()
+            self._finish(_APPLY)
+        self._accumulated = 0
+
+    def _add_window(self, lo: int, hi: int) -> None:
+        """The applying micro-batch: adds the window's sum to flat_g[lo:hi) (nothing with k = 1)."""
+        if self._acc is not None:
+            E.grad_accumulate(self._acc, self.flat_g, lo, hi, _lib.GRAD_ACC_APPLY)
+
+    def _finish(self, phase: str, split: bool = False) -> None:
+        """After a micro-batch's backward: its gradient goes into the window's sum, or — on the applying micro-batch — the sum
+        is added to it and the exchange, the guard and Adam follow.  ``split``: the small-gradient ranges were already summed and
+        handed to the side-stream all-reduce (``_reduce_small_grads``); the GEMM range remains."""
+        if phase != _APPLY:
+            mode = _lib.GRAD_ACC_SET if phase == _FIRST else _lib.GRAD_ACC_ADD
+            E.grad_accumulate(self._acc, self.flat_g, 0, self.numel, mode)
+            return
+        if split:
+            lo, hi = self._gemm_grad_range
+            self._add_window(lo, hi)
+            dist.all_reduce(self.flat_g[lo:hi], op=dist.ReduceOp.SUM, group=self.pg)
+            torch.cuda.current_stream().wait_stream(self._ar_stream)     # both halves are in before the norm and Adam
+        else:
+            self._add_window(0, self.numel)
+            if self.exchange != "p2p" and self.world > 1:     # under p2p the exchange is the update kernel itself
+                dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
+        self._enqueue_update()
+
+    # ---- label_style="node"------------------------------------------------------------------------------------------------
     def _require_node(self, what):
         if not self._node:
             raise ValueError(f"{what}: this FusedTrainer trains a label_style='graph' module")
@@ -724,15 +822,17 @@ class FusedTrainer:
                                  "the loss is the mean over the GLOBAL batch)")
         return int(local_graphs)
 
-    def _enqueue(self, g, dg, idx, vuln, global_batch: int, num_valid: Optional[int] = None, valid_nodes: Optional[torch.Tensor] = None):
-        """Enqueues one step.  Node style returns the row-list buffer the step's loss rows go to; ``valid_nodes``: the int32
-        device word of its valid node count under bucketing (None: every node is valid)."""
+    def _enqueue(self, g, dg, idx, vuln, global_batch: int, num_valid: Optional[int] = None, valid_nodes: Optional[torch.Tensor] = None,
+                 phase: str = _APPLY):
+        """Enqueues one step (one micro-batch, ``phase`` as :meth:`_phase` says).  Node style returns the row-list buffer the
+        step's loss rows go to; ``valid_nodes``: the int32 device word of its valid node count under bucketing (None: every node
+        is valid)."""
         m = self.module
         eng = _ENGINES[m.engine]
         pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
         self.flat_g.zero_()
         if self._node:
-            rows = self._enqueue_node(dg, idx, vuln, eng, pw, valid_nodes)
+            rows = self._enqueue_node(dg, idx, vuln, eng, pw, valid_nodes, phase)
             if self.track_metrics:
                 self._enqueue_metrics("ddfa_eval_metrics_rows", (E._p(self._last_logits), E._p(vuln), E._p(rows),
                                                                  self._num_rows.data_ptr(), dg.num_nodes),
@@ -741,22 +841,15 @@ class FusedTrainer:
         _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws,
                                      grad_ggnn=self._grad_ggnn)
         prune = dict(grad_ggnn=self._grad_ggnn, grad_tables=self._grad_tables)
-        _, _, dlogits = E.graph_label_bce(dg, vuln, logits, pw, 1.0 / global_batch, 1.0 / global_batch, True,
+        # the gradient of loss / k (k = 1: 1 / global_batch as ever); the loss itself stays the micro-batch's mean
+        _, _, dlogits = E.graph_label_bce(dg, vuln, logits, pw, 1.0 / global_batch, 1.0 / (global_batch * self._k), True,
                                           alloc=self.ws, loss_out=self._loss_local if self.exchange == "p2p" else self.loss_slot,
                                           num_valid=num_valid)
-        if self.exchange == "p2p":       # the exchange is the update kernel itself
-            E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws, **prune)
-        else:
-            split = self.world > 1 and self.overlap_allreduce
-            E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws,
-                       on_small_grads_ready=self._reduce_small_grads if split else None, **prune)
-            if split:
-                lo, hi = self._gemm_grad_range
-                dist.all_reduce(self.flat_g[lo:hi], op=dist.ReduceOp.SUM, group=self.pg)
-                torch.cuda.current_stream().wait_stream(self._ar_stream)     # both halves are in before the norm and Adam
-            elif self.world > 1:
-                dist.all_reduce(self.flat_g, op=dist.ReduceOp.SUM, group=self.pg)
-        self._enqueue_update()
+        # NCCL over several ranks: the small-gradient ranges are all-reduced on a side stream during the weight-gradient launch
+        split = phase == _APPLY and self.exchange != "p2p" and self.world > 1 and self.overlap_allreduce
+        E.backward(self.params, dg, saved, self.grads, dlogits=dlogits, engine=eng, alloc=self.ws,
+                   on_small_grads_ready=self._reduce_small_grads if split else None, **prune)
+        self._finish(phase, split)
         if self.track_metrics:
             B = dg.batch_size
             nv = B if num_valid is None else int(num_valid)
@@ -802,9 +895,10 @@ class FusedTrainer:
         for name, args in self._update:
             L.call(name, *args, stream)
 
-    def _enqueue_node(self, dg, idx, vuln, eng, pw, valid_nodes):
+    def _enqueue_node(self, dg, idx, vuln, eng, pw, valid_nodes, phase):
         """label_style="node" (one rank): GGNN forward without the readout, the loss rows drawn on the device, the head and
-        the BCE over them, the head backward into dh_T / dx, the GGNN backward from there, the update."""
+        the BCE over them, the head backward into dh_T / dx, the GGNN backward from there, the update (or, inside an
+        accumulation window, the gradient into the window's sum)."""
         m, ws = self.module, self.ws
         N = dg.num_nodes
         if vuln.dtype != torch.int32:
@@ -819,19 +913,22 @@ class FusedTrainer:
                       self._num_rows, self._sample_status, alloc=ws)
         logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
         self._last_logits = logits
-        dlogits = E.node_bce(logits, vuln, rows, self._num_rows, pw, self.loss_slot, alloc=ws)
+        dlogits = E.node_bce(logits, vuln, rows, self._num_rows, pw, self.loss_slot, alloc=ws,
+                             grad_scale=None if self._k == 1 else 1.0 / self._k)
         dh, dx = E.node_head_bwd(self.params, self.grads, dlogits, x, h_T, rows, self._num_rows, act, alloc=ws,
                                  input_grads=self._grad_ggnn)
         if self._grad_ggnn:
             E.backward(self.params, dg, saved, self.grads, engine=eng, alloc=ws, dh_final=dh, dx_direct=dx,
                        grad_tables=self._grad_tables)
-        self._enqueue_update()
+        self._finish(phase)
         return rows
 
     def _reduce_small_grads(self):
         """All-reduce of the embedding / bias / readout / MLP gradients and the loss slot on a side stream (engine.backward
-        calls this before the weight-gradient launch)."""
+        calls this before the weight-gradient launch).  The window's sum goes into those ranges first."""
         lo, hi = self._gemm_grad_range
+        self._add_window(0, lo)
+        self._add_window(hi, self.numel)
         main = torch.cuda.current_stream()
         if self._ar_stream is None:
             self._ar_stream = torch.cuda.Stream(device=self.device)
@@ -849,15 +946,16 @@ class FusedTrainer:
         return bucket_shape(N, Eg, self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes)
 
     def num_bucket_shapes(self) -> int:
-        return sum(1 for k in self._stream_slots if k[0] == "bucket")
+        return len({k[:6] for k in self._stream_slots if k[0] == "bucket"})     # the phases of one shape count once
 
-    def _stream_slot(self, g, global_batch: Optional[int]):
+    def _stream_slot(self, g, global_batch: Optional[int], phase: str):
         N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
         gb = self._global_batch(global_batch, B)
         bucket = self._bucket_shape(N, Eg)
         # keyed by the deterministic mode too: a captured graph keeps the kernels of the mode it was captured in
         det = _lib.deterministic_requested()
         key = ("bucket", bucket[0], bucket[1], B, gb, det) if bucket else ("exact", N, Eg, B, gb, det)
+        key += self._phase_key(phase)
         slot = self._stream_slots.get(key)
         if slot is None:
             if len(self._stream_slots) >= self.max_graph_shapes:
@@ -872,8 +970,8 @@ class FusedTrainer:
 
     def prefetch(self, batch, global_batch: Optional[int] = None) -> None:
         """Starts the host->device copy of a (pinned) host batch on a side stream so that it overlaps the step that is running;
-        the following ``step(batch)`` with the SAME batch object picks the staged copy up.  No-op without ``use_cuda_graph`` or
-        for device batches."""
+        the following ``step(batch)`` with the SAME batch object picks the staged copy up (with gradient accumulation: the very
+        next micro-batch).  No-op without ``use_cuda_graph`` or for device batches."""
         if not self.use_cuda_graph:
             return
         g = as_batched_cfg(batch)
@@ -882,21 +980,21 @@ class FusedTrainer:
         with torch.cuda.device(self.device):
             if self._copy_stream is None:
                 self._copy_stream = torch.cuda.Stream(device=self.device)
-            slot = self._stream_slot(g, global_batch)
+            slot = self._stream_slot(g, global_batch, self._phase())
             if slot is not None:
                 slot["staged"] = (id(batch), self._stage(slot, g, self._copy_stream))
 
-    def _step_streamed(self, batch, g, global_batch: Optional[int]) -> torch.Tensor:
+    def _step_streamed(self, batch, g, global_batch: Optional[int], phase: str) -> None:
         """Host batch + use_cuda_graph: the batch's arrays are copied into device buffers that are STATIC per shape
         (num_nodes, num_edges, batch_size — or per BUCKET shape with ``bucket_nodes`` / ``bucket_edges``) and one captured
         CUDA graph per buffer set covers the whole step including the device CSR build — a new batch of a known shape costs
         its H2D copies (overlappable: ``prefetch``) plus one graph launch.  The first visit of a shape runs eagerly
-        (workspace growth), the next two capture."""
+        (workspace growth), the next two capture.  Every phase of a shape has a slot of its own."""
         m = self.module
         with torch.cuda.device(self.device):
-            slot = self._stream_slot(g, global_batch)
+            slot = self._stream_slot(g, global_batch, phase)
             if slot is None:          # more shapes than max_graph_shapes: same kernels, launched eagerly
-                return self._step_eager(batch, global_batch)
+                return self._step_eager(batch, global_batch, phase)
             N, gb = slot["N"], slot["gb"]
             main = torch.cuda.current_stream()
             staged = slot["staged"]
@@ -914,7 +1012,8 @@ class FusedTrainer:
                 vuln = gs.ndata["_VULN"]
                 if vuln.dtype != torch.int32:
                     vuln = vuln.to(torch.int32)
-                st["rows"] = self._enqueue(g_, dg, idx, vuln.contiguous(), gb, num_valid=slot["valid"], valid_nodes=st["valid_nodes"])
+                st["rows"] = self._enqueue(g_, dg, idx, vuln.contiguous(), gb, num_valid=slot["valid"], valid_nodes=st["valid_nodes"],
+                                           phase=phase)
                 st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
 
             st["graph"] = self._graph_step(st["graph"], slot["warm"], enqueue)
@@ -924,27 +1023,26 @@ class FusedTrainer:
             ev = torch.cuda.Event()
             ev.record(main)
             st["free"] = ev
-        return self.loss_slot
 
     def step_ids(self, arena, ids, global_batch: Optional[int] = None) -> torch.Tensor:
         """One optimisation step on the graphs ``ids`` of a device-resident :class:`deepdfa_b200.arena.GraphArena` (SURVEY.md §8
         f1: the batch producer).  With ``use_cuda_graph`` the batch is assembled into static per-shape buffers by
         ``ddfa_arena_batch`` inside one captured graph, so a step costs the H2D copy of the id list plus one graph launch;
-        otherwise it is ``step(arena.batch(ids))``."""
-        self._check_trainable()
-        self._raise_deferred_sample_errors()
-        self.optimizer.step()
+        otherwise it is ``step(arena.batch(ids))``.  One micro-batch, as :meth:`step`."""
+        phase = self._begin()
         if not self.use_cuda_graph:
-            return self._step_eager(arena.batch(ids), global_batch)
+            self._step_eager(arena.batch(ids), global_batch, phase)
+            return self._end(phase)
         m = self.module
         ids_np, B, N, Eg = arena_ids(arena, ids, "step_ids")
         gb = self._global_batch(global_batch, B)
-        key = ("arena", id(arena), N, Eg, B, gb, _lib.deterministic_requested())
+        key = ("arena", id(arena), N, Eg, B, gb, _lib.deterministic_requested()) + self._phase_key(phase)
         slot = self._stream_slots.get(key)
         with torch.cuda.device(self.device):
             if slot is None:
                 if len(self._stream_slots) >= self.max_graph_shapes:
-                    return self._step_eager(arena.batch(ids), global_batch)
+                    self._step_eager(arena.batch(ids), global_batch, phase)
+                    return self._end(phase)
                 slot = new_arena_slot(arena, B, N, Eg)
                 self._stream_slots[key] = slot
             push_ids(slot, ids_np)
@@ -952,29 +1050,30 @@ class FusedTrainer:
             def enqueue():
                 g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
                 g_, dg, idx = m._prepare(g)
-                slot["rows"] = self._enqueue(g_, dg, idx, g.ndata["_VULN"], gb)
+                slot["rows"] = self._enqueue(g_, dg, idx, g.ndata["_VULN"], gb, phase=phase)
                 slot["keep"] = (g, dg, idx)
 
             slot["graph"] = self._graph_step(slot["graph"], slot["warm"], enqueue)
             slot["warm"] = True
             if self._node:
                 self._node_step_done(slot["rows"])
-        return self.loss_slot
+        return self._end(phase)
 
     def step(self, batch, global_batch: Optional[int] = None) -> torch.Tensor:
         """One optimisation step on this rank's shard.  Returns the device tensor holding the
         global mean loss (valid after the step's stream work completes).  Starts with ``self.optimizer.step()``, which hands
-        the current learning rate etc. to this step's Adam launch (an LR scheduler on ``self.optimizer`` sees that call)."""
-        self._check_trainable()
-        self._raise_deferred_sample_errors()
-        self.optimizer.step()
-        if self.use_cuda_graph:
-            gb_ = as_batched_cfg(batch)
-            if gb_.device.type == "cpu":
-                return self._step_streamed(batch, gb_, global_batch)
-        return self._step_eager(batch, global_batch)
+        the current learning rate etc. to this step's Adam launch (an LR scheduler on ``self.optimizer`` sees that call).
+        With ``accumulate_grad_batches=k > 1`` the call is one micro-batch: only the last of a window updates the parameters
+        and calls ``optimizer.step()`` (see the constructor)."""
+        phase = self._begin()
+        gb_ = as_batched_cfg(batch) if self.use_cuda_graph else None
+        if gb_ is not None and gb_.device.type == "cpu":
+            self._step_streamed(batch, gb_, global_batch, phase)
+        else:
+            self._step_eager(batch, global_batch, phase)
+        return self._end(phase)
 
-    def _step_eager(self, batch, global_batch: Optional[int] = None) -> torch.Tensor:
+    def _step_eager(self, batch, global_batch: Optional[int] = None, phase: str = _APPLY) -> None:
         """Device-resident batch objects (one captured graph per object when ``use_cuda_graph``), or plain eager launches."""
         m = self.module
         g, dg, idx = m._prepare(batch)
@@ -989,8 +1088,8 @@ class FusedTrainer:
         global_batch = self._global_batch(global_batch, dg.batch_size)
         with torch.cuda.device(self.device):
             det = _lib.deterministic_requested()
-            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size, det)
-            graph_key = (id(g), det)
+            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size, det) + self._phase_key(phase)
+            graph_key = (id(g), det) + self._phase_key(phase)
             capturable = self.use_cuda_graph and as_batched_cfg(batch).device.type == "cuda" and \
                 (graph_key in self._graphs or len(self._graphs) < self.max_resident_graphs)
             # one captured CUDA graph per resident batch object (its device pointers are baked in); a step that cannot be
@@ -999,14 +1098,13 @@ class FusedTrainer:
             out = {}
 
             def enqueue():
-                out["rows"] = self._enqueue(g, dg, idx, vuln, global_batch)
+                out["rows"] = self._enqueue(g, dg, idx, vuln, global_batch, phase=phase)
             cg = self._graph_step(entry[0] if entry else None, capturable and shape_key in self._warm_shapes, enqueue)
             if entry is None and cg is not None:
                 self._graphs[graph_key] = (cg, g, idx, vuln, out["rows"])     # keep the captured tensors alive
             self._warm_shapes.add(shape_key)
             if self._node:
                 self._node_step_done(out["rows"] if "rows" in out else entry[4])
-        return self.loss_slot
 
     # ------------------------------------------------------------------------------------
     @staticmethod

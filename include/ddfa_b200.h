@@ -401,6 +401,10 @@ int ddfa_node_head_fwd(const float *h_final, const float *x, const int32_t *rows
                        int32_t num_layers, float *mlp_act, float *logits, void *stream);
 int ddfa_node_bce(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows,
                   int32_t num_nodes, float pos_weight, float *loss_out, float *dlogits, void *stream);
+/* ddfa_node_bce with dlogits[s] scaled by grad_scale: the row scale is (1.f / S) * grad_scale (gradient accumulation over k
+ * micro-batches passes 1 / k).  loss_out is the unscaled mean; grad_scale = 1 gives results bit-identical to ddfa_node_bce. */
+int ddfa_node_bce_scaled(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows,
+                         int32_t num_nodes, float pos_weight, float grad_scale, float *loss_out, float *dlogits, void *stream);
 size_t ddfa_node_head_bwd_workspace_bytes(int32_t num_nodes, int32_t dim);
 int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *x, const int32_t *rows,
                        const int32_t *num_rows, int32_t num_nodes, int32_t dim, const float *const *mlp_w,
@@ -534,6 +538,20 @@ int ddfa_allreduce_adam_p2p_guarded(void *const *peer_params, const void *const 
                                     int64_t numel, int64_t loss_offset, float *loss_out, const float *hyper,
                                     const float *max_norm, float *gstate, int32_t *skipped, void *guard_state,
                                     void *stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Gradient accumulation over micro-batches (Lightning's accumulate_grad_batches): elementwise over the elements
+ * [begin, end) of two flat fp32 buffers, the accumulator `acc` and a micro-batch's gradients `grads`:
+ *   DDFA_GRAD_ACC_SET   acc = grads    (the first micro-batch of a window)
+ *   DDFA_GRAD_ACC_ADD   acc += grads   (the micro-batches after it)
+ *   DDFA_GRAD_ACC_APPLY grads += acc   (the window's last micro-batch: the exchange and the update then read grads as always)
+ * Both bounds multiples of 4, 0 <= begin <= end; acc and grads 16-byte aligned; nothing outside the range is read or written.
+ * One launch (none for an empty range).  One fp32 add per element: bit-reproducible in both DDFA_TUNE_DETERMINISTIC modes.
+ * ------------------------------------------------------------------------------------- */
+#define DDFA_GRAD_ACC_SET 0
+#define DDFA_GRAD_ACC_ADD 1
+#define DDFA_GRAD_ACC_APPLY 2
+int ddfa_grad_accumulate(float *acc, float *grads, int64_t begin, int64_t end, int32_t mode, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Generic row-major fp32 GEMM on the SIMT engine (building block, exported for tests):
