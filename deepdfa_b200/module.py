@@ -35,6 +35,8 @@ logger = logging.getLogger(__name__)
 allfeats = ["api", "datatype", "literal", "operator"]  # reference ggnn.py:17-19
 
 _ENGINES = {"simt": ENGINE_SIMT, "tcgen05": ENGINE_TCGEN05}
+MAX_HIDDEN_WIDTH = 512      # readout.cu (kMaxChunks = 4: D <= 512) and the embedding backward (K * H <= 512)
+TCGEN05_WIDTH = 128         # the tensor-core GRU kernels are written for D == 128
 
 
 def default_engine(hidden_width: int) -> str:
@@ -124,7 +126,9 @@ class FlowGNNGGNNModule(nn.Module):
     """Drop-in for ``code_gnn.models.flow_gnn.ggnn.FlowGNNGGNNModule`` (reference ggnn.py:21-109).
 
     Extra keyword (not in the reference): ``engine`` = "simt" | "tcgen05" selects the GEMM engine of the
-    GRU step (default: ``$DDFA_B200_ENGINE`` if set, else ``DEFAULT_ENGINE``).
+    GRU step (default: ``$DDFA_B200_ENGINE`` if set, else ``default_engine(W)``).  The hidden width W (``hidden_dim``, times 4
+    with ``concat_all_absdf``) must be a multiple of 4 and at most 512; "tcgen05" runs W = 128 only.  Both are checked here
+    (``ValueError``).
     """
 
     def __init__(self, feat, input_dim, hidden_dim, n_steps, num_output_layers, label_style="graph",
@@ -193,10 +197,21 @@ class FlowGNNGGNNModule(nn.Module):
             self.output_layer = nn.Sequential(*layers)
             self._num_layers = num_output_layers
 
+        # the kernels cap the width: the readout holds a [h | x] row of 2 * W floats in four 128-float chunks per half, and the
+        # embedding backward one K * H row per CTA; checked here rather than as a DdfaError from inside the first forward
+        config = f"hidden_dim={self.hparams.hidden_dim}, concat_all_absdf={concat_all_absdf}"
+        if hidden_dim > MAX_HIDDEN_WIDTH:
+            raise ValueError(f"hidden width {hidden_dim} ({config}) exceeds {MAX_HIDDEN_WIDTH}, the widest the readout and embedding "
+                             "kernels run")
+        source = "engine argument"
         if engine is None:
+            source = "DDFA_B200_ENGINE" if os.environ.get("DDFA_B200_ENGINE") else "default"
             engine = os.environ.get("DDFA_B200_ENGINE") or default_engine(hidden_dim)
         if engine not in _ENGINES:
             raise ValueError(f"engine must be one of {sorted(_ENGINES)}, got {engine!r}")
+        if engine == "tcgen05" and hidden_dim != TCGEN05_WIDTH:
+            raise ValueError(f"engine='tcgen05' (from the {source}) runs hidden width {TCGEN05_WIDTH} only, got {hidden_dim} ({config}); "
+                             "use engine='simt'")
         self.engine = engine
         # Input validation (the reference raises on an out-of-range embedding index; DGL rejects edge ids >= num_nodes):
         #   "deferred" (default)     device-side counters, read without a host sync -> IndexError at the NEXT call / check_inputs()
