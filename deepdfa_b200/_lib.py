@@ -96,6 +96,10 @@ _SIGNATURES = {
     "ddfa_adam_flat_ranges": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _vp]),
     "ddfa_p2p_guard_state_bytes": (_sz, []),
     "ddfa_allreduce_adam_p2p_guarded": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ddfa_adam_flat_groups": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "ddfa_allreduce_adam_p2p_groups": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _i32, _vp]),
+    "ddfa_allreduce_adam_p2p_groups_guarded": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _i32, _vp, _i32,
+                                                      _vp, _vp, _vp, _vp, _vp]),
     "ddfa_node_sample_workspace_bytes": (_sz, [_i32]),
     "ddfa_node_sample": (_int, [_vp, _vp, _i32, C.c_double, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ddfa_node_head_fwd": (_int, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
@@ -121,6 +125,8 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
 GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate
+ADAM_GROUP_WORDS = 8          # DDFA_ADAM_GROUP_WORDS: fp32 words per row of the parameter-group table
+ADAM_MAX_GROUPS = 64          # DDFA_ADAM_MAX_GROUPS: rows the grouped Adam entry points accept
 
 
 class _Lib:

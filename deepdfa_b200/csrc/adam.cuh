@@ -1,7 +1,8 @@
 // The optimizer arithmetic, written once for every Adam entry point: the flat update (loss_adam.cu), the peer-memory exchange
 // (allreduce_adam.cu) and the gradient guard (grad_guard.cu).
 //
-// Adam is torch.optim.Adam with coupled L2 (not AdamW, DDFA/configs/config_default.yaml:43-47).  Every entry point computes
+// Adam is torch.optim.Adam with coupled L2 (DDFA/configs/config_default.yaml:43-47); the grouped entry points also run the
+// decoupled form of torch.optim.AdamW per parameter group (update_decoupled, below).  Every entry point computes
 // bit-identical results from the same inputs, so the expression order below must not change: a reordered or re-rounded term
 // changes parameters in the last bits.
 //
@@ -56,6 +57,54 @@ __device__ __forceinline__ void update(const float4 &g, float4 &p, float4 &m, fl
   update(g.y, p.y, m.y, v.y, h, c);
   update(g.z, p.z, m.z, v.z, h, c);
   update(g.w, p.w, m.w, v.w, h, c);
+}
+
+// Decoupled weight decay: torch.optim.AdamW / Adam(decoupled_weight_decay=True), torch/optim/adam.py _single_tensor_adam:
+//   param.mul_(1 - lr * weight_decay)            decay = fp32(1 - lr * wd), computed by the host in fp64 and rounded once
+// then the moments and the step exactly as in update() with no wd * p term in the gradient.  decay == 1 (wd == 0) leaves p as is.
+__device__ __forceinline__ void update_decoupled(float g, float &p, float &m, float &v, const Hyper &h, float decay, const Bias &c) {
+  p = p * decay;
+  m = fmaf(h.beta1, m, (1.f - h.beta1) * g);
+  v = fmaf(h.beta2, v, (1.f - h.beta2) * g * g);
+  const float denom = sqrtf(v) / c.bc2s + h.eps;
+  p = p - c.step_size * (m / denom);
+}
+
+// ---- parameter groups: a device table of G rows of kGroupWords floats, read when the kernel runs
+constexpr int kMaxGroups = 64;
+constexpr int kGroupWords = 8;
+enum GroupWord { kLr = 0, kBeta1, kBeta2, kEps, kWd, kDecoupled, kDecay, kPad };
+
+struct Group {
+  Hyper h;
+  float decay;       // decoupled groups: fp32(1 - lr * wd); coupled groups: unused
+  bool decoupled;
+};
+__device__ __forceinline__ Group load_group(const float *row) {
+  return Group{Hyper{row[kLr], row[kBeta1], row[kBeta2], row[kEps], row[kWd]}, row[kDecay], row[kDecoupled] != 0.f};
+}
+// one element of a group: the coupled form is update() itself, so a coupled group is bit-identical to the single-group kernels
+__device__ __forceinline__ void update(float g, float &p, float &m, float &v, const Group &gr, const Bias &c) {
+  if (gr.decoupled)
+    update_decoupled(g, p, m, v, gr.h, gr.decay, c);
+  else
+    update(g, p, m, v, gr.h, c);
+}
+__device__ __forceinline__ void update(const float4 &g, float4 &p, float4 &m, float4 &v, const Group &gr, const Bias &c) {
+  update(g.x, p.x, m.x, v.x, gr, c);
+  update(g.y, p.y, m.y, v.y, gr, c);
+  update(g.z, p.z, m.z, v.z, gr, c);
+  update(g.w, p.w, m.w, v.w, gr, c);
+}
+
+// Threads [0, num_groups) of the CTA load the table into shared memory and compute each group's bias correction (fp64, from the
+// one shared step count); the caller synchronises before reading.
+__device__ __forceinline__ void load_groups(const float *__restrict__ table, int32_t num_groups, int32_t step, Group *s_g, Bias *s_c) {
+  if ((int)threadIdx.x < num_groups) {
+    const Group gr = load_group(table + (size_t)threadIdx.x * kGroupWords);
+    s_g[threadIdx.x] = gr;
+    s_c[threadIdx.x] = bias_correction(gr.h.lr, gr.h.beta1, gr.h.beta2, step);
+  }
 }
 
 }  // namespace adam

@@ -19,8 +19,11 @@
 // Flags are epochs (identical on all ranks, read from device memory: the launch is CUDA-graph capturable); every wait is bounded
 // and traps instead of hanging the device.
 //
-// ddfa_allreduce_adam_p2p[_hp] and ddfa_allreduce_adam_p2p_guarded run one kernel, allreduce_adam_p2p_kernel<Guarded>.  The
-// guarded form (gradient clipping and skipping of non-finite steps, adam.cuh) differs in four places:
+// ddfa_allreduce_adam_p2p[_hp] and ddfa_allreduce_adam_p2p_guarded run one kernel, allreduce_adam_p2p_kernel<Guarded, Grouped>;
+// the _groups forms (Grouped) update only the parts of the slice inside a list of [begin, end, group] ranges, each with its
+// parameter group's row of a device table (coupled Adam or decoupled AdamW, adam.cuh) and bias correction.  The norm of the
+// guarded form covers the whole slice either way.
+// The guarded form (gradient clipping and skipping of non-finite steps, adam.cuh) differs in four places:
 //   norm     a rank reduces only its own 1/R slice, but the norm needs all of them, so a norm phase sits between phase 1 and the
 //            update: every CTA sums the squares of its part of the reduced slice in fp64 (a fixed tree) into a per-CTA partial;
 //            the last CTA by ticket adds the partials in CTA order and writes the slice sum into EVERY peer's flag area (slot
@@ -104,10 +107,11 @@ __device__ __forceinline__ float4 reduced_grad(const Peers &pp, int world, int64
   return g;
 }
 
-// Adam on this rank's units [lo, hi) (guarded: on g * coef); the new parameters go to every rank
-template <bool Guarded>
+// Adam on this rank's units [lo, hi) (guarded: on g * coef); the new parameters go to every rank.  H: adam::Hyper (one coupled
+// group) or adam::Group (a row of the group table).
+template <bool Guarded, typename H>
 __device__ __forceinline__ void update_slice(const Peers &pp, int rank, int world, float *__restrict__ m, float *__restrict__ v, int64_t lo,
-                                             int64_t hi, const adam::Hyper &h, const adam::Bias &c, float coef) {
+                                             int64_t hi, const H &h, const adam::Bias &c, float coef) {
   for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (int64_t)gridDim.x * blockDim.x) {
     float4 g = reduced_grad(pp, world, i);
     if constexpr (Guarded) g = make_float4(g.x * coef, g.y * coef, g.z * coef, g.w * coef);
@@ -117,6 +121,20 @@ __device__ __forceinline__ void update_slice(const Peers &pp, int rank, int worl
     *reinterpret_cast<float4 *>(m + 4 * i) = mi;
     *reinterpret_cast<float4 *>(v + 4 * i) = vi;
     for (int p = 0; p < world; ++p) *reinterpret_cast<float4 *>(pp.params[p] + 4 * i) = w;
+  }
+}
+
+// Parameter groups: this rank's units [lo, hi) intersected with every [begin, end, group] range (bounds multiples of 4), each
+// with its group's row and bias correction (shared memory); units outside every range are neither read nor written.
+template <bool Guarded>
+__device__ __forceinline__ void update_slice_groups(const Peers &pp, int rank, int world, float *__restrict__ m, float *__restrict__ v,
+                                                    int64_t lo, int64_t hi, const int64_t *__restrict__ ranges, int32_t num_ranges,
+                                                    int32_t num_groups, const adam::Group *s_g, const adam::Bias *s_c, float coef) {
+  for (int32_t r = 0; r < num_ranges; ++r) {
+    const int64_t grp = ranges[3 * r + 2];
+    if (grp < 0 || grp >= num_groups) continue;
+    const int64_t a = max(lo, ranges[3 * r] >> 2), b = min(hi, ranges[3 * r + 1] >> 2);
+    if (a < b) update_slice<Guarded>(pp, rank, world, m, v, a, b, s_g[grp], s_c[grp], coef);
   }
 }
 
@@ -210,21 +228,29 @@ __device__ __forceinline__ void norm_phase(const Peers &pp, int rank, int world,
   __syncthreads();
 }
 
-// Unguarded: ticket is the caller's word, gs .. skipped are NULL.  Guarded: ticket is NULL.
-template <bool Guarded>
+// Unguarded: ticket is the caller's word, gs .. skipped are NULL.  Guarded: ticket is NULL.  Grouped: h / hyper are unused and
+// ranges / table (num_groups rows) select each element's group; otherwise ranges and table are NULL.
+template <bool Guarded, bool Grouped>
 __global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp, int rank, int world, float *__restrict__ m,
                                                                  float *__restrict__ v, int32_t *__restrict__ step_count, int64_t numel,
                                                                  int64_t loss_off, float *__restrict__ loss_out, uint32_t *__restrict__ ticket,
                                                                  adam::Hyper h, const float *__restrict__ hyper, GuardState *__restrict__ gs,
                                                                  const float *__restrict__ max_norm, float *__restrict__ gstate,
-                                                                 int32_t *__restrict__ skipped) {
-  h = adam::load(h, hyper);
+                                                                 int32_t *__restrict__ skipped, const int64_t *__restrict__ ranges,
+                                                                 int32_t num_ranges, const float *__restrict__ table, int32_t num_groups) {
   __shared__ adam::Bias s_c;
+  __shared__ adam::Group s_grp[Grouped ? adam::kMaxGroups : 1];
+  __shared__ adam::Bias s_grp_c[Grouped ? adam::kMaxGroups : 1];
   __shared__ float s_coef;
   __shared__ int s_last, s_skip;
   const int32_t t0 = *step_count;
   const uint32_t epoch = (Guarded ? *reinterpret_cast<volatile uint32_t *>(&gs->launches) : (uint32_t)t0) + 1u;
-  if (threadIdx.x == 0) s_c = adam::bias_correction(h.lr, h.beta1, h.beta2, t0);
+  if constexpr (Grouped) {
+    adam::load_groups(table, num_groups, t0, s_grp, s_grp_c);      // phase1 ends with __syncthreads
+  } else {
+    h = adam::load(h, hyper);
+    if (threadIdx.x == 0) s_c = adam::bias_correction(h.lr, h.beta1, h.beta2, t0);
+  }
   phase1(pp, rank, world, epoch);
   const adam::Bias c = s_c;
   // this rank's slice, in 16-byte units (numel is a multiple of 4: the trainer aligns every parameter to 64 elements)
@@ -233,7 +259,14 @@ __global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp,
   const int64_t lo = (int64_t)rank * per, hi = min(n4, lo + per);
   if constexpr (Guarded) {
     norm_phase(pp, rank, world, epoch, lo, hi, gs, max_norm, gstate, skipped, s_last, &s_coef, &s_skip);
-    if (!s_skip) update_slice<true>(pp, rank, world, m, v, lo, hi, h, c, s_coef);
+    if (!s_skip) {
+      if constexpr (Grouped)
+        update_slice_groups<true>(pp, rank, world, m, v, lo, hi, ranges, num_ranges, num_groups, s_grp, s_grp_c, s_coef);
+      else
+        update_slice<true>(pp, rank, world, m, v, lo, hi, h, c, s_coef);
+    }
+  } else if constexpr (Grouped) {
+    update_slice_groups<false>(pp, rank, world, m, v, lo, hi, ranges, num_ranges, num_groups, s_grp, s_grp_c, 1.f);
   } else {
     update_slice<false>(pp, rank, world, m, v, lo, hi, h, c, 1.f);
   }
@@ -253,17 +286,23 @@ __global__ void __launch_bounds__(256) allreduce_adam_p2p_kernel(const Peers pp,
 
 // Argument checks (`name` is the entry point), Peers, the grid, the launch.  Unguarded, the step-count increment follows as a
 // launch of its own; guarded, the kernel advances the counters itself.
-template <bool Guarded>
+template <bool Guarded, bool Grouped = false>
 static int launch(const char *name, void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
                   int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel, int64_t loss_offset, float *loss_out,
                   uint32_t *ticket, adam::Hyper h, const float *hyper, void *guard_state, const float *max_norm, float *gstate,
-                  int32_t *skipped, void *stream_) {
+                  int32_t *skipped, void *stream_, const int64_t *ranges = nullptr, int32_t num_ranges = 0, const float *table = nullptr,
+                  int32_t num_groups = 0) {
   DDFA_REQUIRE(world >= 1 && world <= kMaxRanks && rank >= 0 && rank < world, "%s: rank %d / world %d (max %d ranks)", name, rank, world,
                kMaxRanks);
   DDFA_REQUIRE(numel >= 0 && numel % 4 == 0, "%s: numel (%lld) must be a multiple of 4", name, (long long)numel);
   DDFA_REQUIRE(peer_params && peer_grads && peer_flags && exp_avg && exp_avg_sq && step_count &&
-                   (Guarded ? hyper && gstate && guard_state : ticket != nullptr),
+                   (Guarded ? (Grouped || hyper) && gstate && guard_state : ticket != nullptr),
                "%s: NULL pointer", name);
+  if constexpr (Grouped) {
+    DDFA_REQUIRE(num_ranges >= 0 && num_groups >= 1 && num_groups <= adam::kMaxGroups,
+                 "%s: num_ranges (%d) must be >= 0 and num_groups (%d) in [1, %d]", name, num_ranges, num_groups, adam::kMaxGroups);
+    DDFA_REQUIRE(table && (ranges || num_ranges == 0), "%s: NULL pointer", name);
+  }
   DDFA_REQUIRE(!Guarded || aligned16(guard_state), "%s: guard_state must be 16-byte aligned", name);
   Peers pp = {};
   for (int p = 0; p < world; ++p) {
@@ -280,9 +319,9 @@ static int launch(const char *name, void *const *peer_params, const void *const 
   int blocks = (int)((per + 255) / 256);
   if (blocks < 1) blocks = 1;
   if (blocks > kMaxCtas) blocks = kMaxCtas;     // co-resident, and one partial slot each
-  allreduce_adam_p2p_kernel<Guarded><<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset, loss_out,
-                                                                 ticket, h, hyper, static_cast<GuardState *>(guard_state), max_norm, gstate,
-                                                                 skipped);
+  allreduce_adam_p2p_kernel<Guarded, Grouped><<<blocks, 256, 0, stream>>>(pp, rank, world, exp_avg, exp_avg_sq, step_count, numel, loss_offset,
+                                                                          loss_out, ticket, h, hyper, static_cast<GuardState *>(guard_state),
+                                                                          max_norm, gstate, skipped, ranges, num_ranges, table, num_groups);
   DDFA_CHECK_LAUNCH("allreduce_adam_p2p_kernel");
   return Guarded ? DDFA_OK : adam_step_inc_launch(step_count, nullptr, nullptr, stream);
 }
@@ -320,4 +359,27 @@ extern "C" int ddfa_allreduce_adam_p2p_guarded(void *const *peer_params, const v
   return p2p::launch<true>("ddfa_allreduce_adam_p2p_guarded", peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq,
                            step_count, numel, loss_offset, loss_out, nullptr, adam::Hyper{}, hyper, guard_state, max_norm, gstate, skipped,
                            stream_);
+}
+
+// Parameter groups (torch.optim.AdamW / Adam with several param_groups): the protocol of ddfa_allreduce_adam_p2p_hp and
+// ddfa_allreduce_adam_p2p_guarded, with Adam on the intersection of this rank's slice with the [begin, end, group] ranges.
+extern "C" int ddfa_allreduce_adam_p2p_groups(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags, int32_t rank,
+                                              int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                                              int64_t loss_offset, float *loss_out, uint32_t *ticket, const int64_t *ranges, int32_t num_ranges,
+                                              const float *groups, int32_t num_groups, void *stream_) {
+  using namespace ddfa;
+  return p2p::launch<false, true>("ddfa_allreduce_adam_p2p_groups", peer_params, peer_grads, peer_flags, rank, world, exp_avg, exp_avg_sq,
+                                  step_count, numel, loss_offset, loss_out, ticket, adam::Hyper{}, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                  stream_, ranges, num_ranges, groups, num_groups);
+}
+
+extern "C" int ddfa_allreduce_adam_p2p_groups_guarded(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags,
+                                                      int32_t rank, int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count,
+                                                      int64_t numel, int64_t loss_offset, float *loss_out, const int64_t *ranges,
+                                                      int32_t num_ranges, const float *groups, int32_t num_groups, const float *max_norm,
+                                                      float *gstate, int32_t *skipped, void *guard_state, void *stream_) {
+  using namespace ddfa;
+  return p2p::launch<true, true>("ddfa_allreduce_adam_p2p_groups_guarded", peer_params, peer_grads, peer_flags, rank, world, exp_avg,
+                                 exp_avg_sq, step_count, numel, loss_offset, loss_out, nullptr, adam::Hyper{}, nullptr, guard_state, max_norm,
+                                 gstate, skipped, stream_, ranges, num_ranges, groups, num_groups);
 }

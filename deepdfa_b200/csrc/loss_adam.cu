@@ -6,7 +6,8 @@
 // (DDFA/configs/config_default.yaml:43-47) — over one flat parameter buffer, with the hyperparameters by value
 // (ddfa_adam_flat) or from a device word (ddfa_adam_flat_hp); ddfa_adam_flat_guarded is the same update on the clipped
 // gradient, after ddfa_grad_norm (grad_guard.cu); ddfa_adam_flat_ranges updates only the elements inside a list of ranges (the
-// trainable parameters of a partly frozen model).  The arithmetic is adam.cuh's.
+// trainable parameters of a partly frozen model); ddfa_adam_flat_groups gives every range a parameter group of its own
+// hyperparameters, coupled (Adam) or decoupled (AdamW) weight decay.  The arithmetic is adam.cuh's.
 #include <math.h>
 
 #include "common.cuh"
@@ -114,6 +115,50 @@ __global__ void __launch_bounds__(256) adam_flat_kernel(float *__restrict__ p, c
   p[i] = pi;
 }
 
+static_assert(adam::kMaxGroups == DDFA_ADAM_MAX_GROUPS && adam::kGroupWords == DDFA_ADAM_GROUP_WORDS, "group table layout");
+
+// The range of ranges[3 * num_ranges] (sorted, disjoint [begin, end, group] triples) holding i, or -1 (binary search as in_ranges)
+__device__ __forceinline__ int32_t find_range(const int64_t *__restrict__ ranges, int32_t num_ranges, int64_t i) {
+  int32_t lo = 0, hi = num_ranges;
+  while (lo < hi) {
+    const int32_t mid = (lo + hi) >> 1;
+    if (ranges[3 * mid] <= i) lo = mid + 1;
+    else hi = mid;
+  }
+  return (lo > 0 && i < ranges[3 * lo - 2]) ? lo - 1 : -1;
+}
+
+// Parameter groups: element i inside range r is updated with the hyperparameters of group ranges[3r + 2] (a row of the table,
+// adam::kGroupWords floats) and that group's bias correction; elements outside every range, or of a range whose group index is
+// not in [0, num_groups), are neither read nor written.  Guarded as adam_flat_kernel.
+template <bool Guarded>
+__global__ void __launch_bounds__(256) adam_flat_groups_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
+                                                               float *__restrict__ v, const int32_t *__restrict__ step_count, int64_t n,
+                                                               const int64_t *__restrict__ ranges, int32_t num_ranges,
+                                                               const float *__restrict__ table, int32_t num_groups,
+                                                               const float *__restrict__ gstate, const int32_t *__restrict__ skipped) {
+  if constexpr (Guarded) {
+    if (skipped && gstate[guard::kNonFinite] != 0.f) return;
+  }
+  __shared__ adam::Group s_g[adam::kMaxGroups];
+  __shared__ adam::Bias s_c[adam::kMaxGroups];
+  adam::load_groups(table, num_groups, *step_count, s_g, s_c);
+  __syncthreads();
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t r = find_range(ranges, num_ranges, i);
+  if (r < 0) return;
+  const int64_t grp = ranges[3 * r + 2];
+  if (grp < 0 || grp >= num_groups) return;
+  float gi = g[i];
+  if constexpr (Guarded) gi = gi * gstate[guard::kCoef];     // clip_grad_norm_: grad.mul_(clip_coef_clamped)
+  float pi = p[i], mi = m[i], vi = v[i];
+  adam::update(gi, pi, mi, vi, s_g[grp], s_c[grp]);
+  m[i] = mi;
+  v[i] = vi;
+  p[i] = pi;
+}
+
 // gstate == NULL: the step.  Otherwise, with skipped != NULL and a non-finite norm, the skip counter instead: a skipped step
 // leaves the Adam step count alone (torch counts the optimizer.step() calls that happened).
 __global__ void adam_step_inc_kernel(int32_t *step_count, const float *gstate, int32_t *skipped) {
@@ -212,6 +257,30 @@ int ddfa_adam_flat_ranges(float *params, const float *grads, float *exp_avg, flo
                                   ranges, num_ranges);
   return adam_flat_launch<false>(params, grads, exp_avg, exp_avg_sq, step_count, numel, adam::Hyper{}, hyper, nullptr, nullptr, stream_,
                                  ranges, num_ranges);
+}
+
+int ddfa_adam_flat_groups(float *params, const float *grads, float *exp_avg, float *exp_avg_sq, int32_t *step_count, int64_t numel,
+                          const int64_t *ranges, int32_t num_ranges, const float *groups, int32_t num_groups, const float *gstate,
+                          int32_t *skipped, void *stream_) {
+  using namespace ddfa;
+  DDFA_REQUIRE(numel >= 0 && num_ranges >= 0, "ddfa_adam_flat_groups: negative numel (%lld) or num_ranges (%d)", (long long)numel, num_ranges);
+  DDFA_REQUIRE(num_groups >= 1 && num_groups <= adam::kMaxGroups, "ddfa_adam_flat_groups: num_groups (%d) must be in [1, %d]", num_groups,
+               adam::kMaxGroups);
+  DDFA_REQUIRE(params && grads && exp_avg && exp_avg_sq && step_count && groups && (ranges || num_ranges == 0),
+               "ddfa_adam_flat_groups: NULL pointer");
+  DDFA_REQUIRE(gstate || !skipped, "ddfa_adam_flat_groups: skipped given without gstate");
+  cudaStream_t stream = as_stream(stream_);
+  if (numel > 0 && num_ranges > 0) {
+    const unsigned blocks = (unsigned)((numel + 255) / 256);
+    if (gstate)
+      adam_flat_groups_kernel<true><<<blocks, 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel, ranges, num_ranges,
+                                                                groups, num_groups, gstate, skipped);
+    else
+      adam_flat_groups_kernel<false><<<blocks, 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, step_count, numel, ranges, num_ranges,
+                                                                 groups, num_groups, nullptr, nullptr);
+    DDFA_CHECK_LAUNCH("adam_flat_groups_kernel");
+  }
+  return adam_step_inc_launch(step_count, gstate, skipped, stream);
 }
 
 }  // extern "C"

@@ -9,7 +9,8 @@ data-path collective (SURVEY.md §8e); the gradient all-reduce is the only excha
 Replaces, for the hot path only, Lightning's ``Trainer.fit`` loop around
 ``BaseModule.training_step`` (base_module.py:171-199) + ``torch.optim.Adam`` (config_default.yaml:43-47).
 ``FusedTrainer.optimizer`` (:class:`FusedAdam`) is the ``torch.optim.Optimizer`` face of the fused Adam: checkpoints in
-``torch.optim.Adam``'s format and LR schedulers that reach captured steps.
+``torch.optim.Adam``'s (or, with parameter groups / decoupled weight decay, ``torch.optim.AdamW``'s) format and LR schedulers
+that reach captured steps.
 """
 from __future__ import annotations
 
@@ -212,37 +213,124 @@ _FIRST, _ADD, _APPLY = "first", "add", "apply"     # what a micro-batch does wit
 _ADAM_FLAGS = dict(amsgrad=False, maximize=False, foreach=None, capturable=False, differentiable=False, fused=None,
                    decoupled_weight_decay=False)
 _UNSUPPORTED = ("amsgrad", "maximize", "decoupled_weight_decay")
+# the keys a param_groups entry of FusedTrainer may carry: torch's Adam / AdamW group keys (amsgrad and maximize only when False;
+# foreach, capturable, differentiable and fused choose torch's implementation and mean nothing to the fused kernels)
+_GROUP_KEYS = ("lr", "betas", "eps", "weight_decay", "decoupled_weight_decay")
+_IGNORED_KEYS = ("amsgrad", "maximize", "foreach", "capturable", "differentiable", "fused")
+
+
+def resolve_param_groups(module, param_groups):
+    """Checks torch-style ``param_groups`` (a list of ``{"params": [...], <lr, betas, eps, weight_decay,
+    decoupled_weight_decay>}``) against ``module`` and returns them as new dicts with ``params`` as lists.  Raises
+    ``ValueError`` for: no group, more than ``ADAM_MAX_GROUPS`` groups, a group without ``params``, an unknown key, AMSGrad or
+    ``maximize``, a tensor that is not a parameter of the module, a parameter in two groups (or twice in one), and a trainable
+    parameter in no group (named).  Frozen parameters may appear in a group or be left out."""
+    if isinstance(param_groups, dict) or not isinstance(param_groups, (list, tuple)) or not param_groups:
+        raise ValueError("param_groups must be a non-empty list of dicts, as torch.optim.AdamW takes them")
+    if len(param_groups) > _lib.ADAM_MAX_GROUPS:
+        raise ValueError(f"param_groups: {len(param_groups)} groups, the fused Adam kernels take at most {_lib.ADAM_MAX_GROUPS}")
+    names = {id(p): n for n, p in module.named_parameters()}
+    seen, out = {}, []
+    for gi, g in enumerate(param_groups):
+        if not isinstance(g, dict) or "params" not in g:
+            raise ValueError(f"param_groups[{gi}] must be a dict with a 'params' entry")
+        unknown = sorted(set(g) - {"params", *_GROUP_KEYS, *_IGNORED_KEYS})
+        if unknown:
+            raise ValueError(f"param_groups[{gi}]: unknown key(s) {unknown}; a group may set {list(_GROUP_KEYS)}")
+        bad = [k for k in ("amsgrad", "maximize") if g.get(k)]
+        if bad:
+            raise ValueError(f"param_groups[{gi}]: {bad} are not supported by the fused Adam kernels")
+        params = [g["params"]] if isinstance(g["params"], torch.Tensor) else list(g["params"])
+        for p in params:
+            if id(p) not in names:
+                raise ValueError(f"param_groups[{gi}] holds a tensor of shape {tuple(p.shape)} that is not a parameter of the module")
+            if id(p) in seen:
+                raise ValueError(f"parameter {names[id(p)]!r} appears in param_groups[{seen[id(p)]}] and param_groups[{gi}]")
+            seen[id(p)] = gi
+        out.append(dict(g, params=params))
+    missing = [n for n, p in module.named_parameters() if p.requires_grad and id(p) not in seen]
+    if missing:
+        raise ValueError(f"trainable parameter(s) {missing} are in no group of param_groups (freeze them with "
+                         "requires_grad_(False) or add them to a group)")
+    return out
+
+
+def group_ranges(plist, group_of):
+    """``[(begin, end, group)]``: the trainable slots of the flat buffers (laid out by :func:`flat_offsets`) with the index of
+    their parameter group, each slot with its alignment padding, adjacent slots of one group merged.  ``group_of`` maps
+    ``id(tensor)`` to a group index; frozen tensors and tensors in no group are left out."""
+    offs, total = flat_offsets(plist)
+    ranges = []
+    for p, lo, hi in zip(plist, offs, offs[1:] + [total]):
+        if not p.requires_grad or id(p) not in group_of:
+            continue
+        g = group_of[id(p)]
+        if ranges and ranges[-1][1] == lo and ranges[-1][2] == g:
+            ranges[-1] = (ranges[-1][0], hi, g)
+        else:
+            ranges.append((lo, hi, g))
+    return ranges
+
+
+def group_row(group) -> tuple:
+    """A row of the device group table (``DDFA_ADAM_GROUP_WORDS`` words) for a torch param group: ``[lr, beta1, beta2, eps,
+    weight_decay, decoupled, decay, 0]``, ``decay = 1 - lr * weight_decay`` in double (the kernel's fp32 word rounds it once,
+    as torch's Python scalar in ``param.mul_(1 - lr * weight_decay)`` is rounded)."""
+    lr, wd = float(group["lr"]), float(group["weight_decay"])
+    dec = bool(group.get("decoupled_weight_decay", False))
+    return (lr, float(group["betas"][0]), float(group["betas"][1]), float(group["eps"]), wd, 1.0 if dec else 0.0,
+            1.0 - lr * wd if dec else 1.0, 0.0)
 
 
 class FusedAdam(torch.optim.Optimizer):
     """The optimizer object of a :class:`FusedTrainer` (``trainer.optimizer``): a ``torch.optim.Optimizer`` whose state is
     the trainer's flat Adam buffers.  It owns no arithmetic — the update runs inside the trainer's step, in
-    ``ddfa_adam_flat_hp`` / ``ddfa_allreduce_adam_p2p_hp`` — and exists so that the usual tools work on a fused run:
+    ``ddfa_adam_flat_hp`` / ``ddfa_allreduce_adam_p2p_hp`` or their ``_groups`` forms — and exists so that the usual tools
+    work on a fused run:
 
-    * ``state_dict()`` / ``load_state_dict()`` in ``torch.optim.Adam``'s format, parameters indexed in
-      ``module.parameters()`` order (what ``torch.optim.Adam(module.parameters())`` and a Lightning checkpoint's
-      ``optimizer_states[0]`` use; the flat buffers hold them in ``module.param_list()`` order);
-    * LR schedulers: ``step()`` copies ``param_groups[0]``'s hyperparameters into a 5-float device word that the Adam
-      kernels read when they run, so a captured CUDA graph picks up a new learning rate on its next replay.
+    * ``state_dict()`` / ``load_state_dict()`` in ``torch.optim.Adam``'s / ``torch.optim.AdamW``'s format, parameters indexed
+      in group order (one group: ``module.parameters()`` order, what ``torch.optim.Adam(module.parameters())`` and a
+      Lightning checkpoint's ``optimizer_states[0]`` use; the flat buffers hold them in ``module.param_list()`` order);
+    * LR schedulers: ``step()`` copies every group's hyperparameters into device words that the Adam kernels read when they
+      run, so a captured CUDA graph picks up a new learning rate on its next replay.
 
-    One parameter group; coupled L2 weight decay (``torch.optim.Adam``, not AdamW); no AMSGrad, no ``maximize``.
-    The buffers may live on any device, so the conversion also runs on CPU tensors."""
+    Two forms, chosen by ``hyper``:
+
+    * ``hyper`` fp32[5] ``[lr, beta1, beta2, eps, weight_decay]``: one parameter group over ``module.parameters()``, coupled
+      L2 weight decay (``torch.optim.Adam``) — the trainer's default.
+    * ``hyper`` fp32[G, DDFA_ADAM_GROUP_WORDS], the group table (rows from :func:`group_row`): the G groups of
+      ``param_groups`` (torch's list, checked by :func:`resolve_param_groups`; None: one group over ``module.parameters()``),
+      each coupled (Adam) or decoupled (AdamW) as its ``decoupled_weight_decay`` says, missing keys from the arguments.  The
+      groups are fixed: ``add_param_group`` raises.
+
+    No AMSGrad, no ``maximize``.  The buffers may live on any device, so the conversion also runs on CPU tensors."""
 
     def __init__(self, module, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, step_count: torch.Tensor, hyper: torch.Tensor,
-                 lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0, shard=None):
+                 lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.0, shard=None,
+                 param_groups=None, decoupled_weight_decay: bool = False):
         """``exp_avg`` / ``exp_avg_sq``: flat fp32 moment buffers laid out by :func:`flat_offsets`; ``step_count``: int32[1];
-        ``hyper``: fp32[5] ``[lr, beta1, beta2, eps, weight_decay]``.  ``shard = (rank, world, process_group)`` when each rank
-        keeps the moments of its :func:`owned_range` only (``exchange="p2p"``)."""
-        params = list(module.parameters())
-        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, **_ADAM_FLAGS))
+        ``hyper``: the hyperparameter words (see the class).  ``shard = (rank, world, process_group)`` when each rank keeps the
+        moments of its :func:`owned_range` only (``exchange="p2p"``)."""
+        self._table = hyper.dim() == 2
+        if not self._table and (param_groups is not None or decoupled_weight_decay):
+            raise ValueError("FusedAdam: param_groups and decoupled_weight_decay need the group table (hyper of shape [G, 8])")
+        groups = (resolve_param_groups(module, param_groups) if param_groups is not None
+                  else [{"params": list(module.parameters())}])
+        if self._table and tuple(hyper.shape) != (len(groups), _lib.ADAM_GROUP_WORDS):
+            raise ValueError(f"FusedAdam: group table of shape {tuple(hyper.shape)} for {len(groups)} groups")
+        flags = dict(_ADAM_FLAGS, decoupled_weight_decay=bool(decoupled_weight_decay))
+        self._sealed = False
+        super().__init__(groups, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, **flags))
+        self._sealed = self._table
         plist = flat_param_list(module)
         offs, total = flat_offsets(plist)
         where = {id(p): o for p, o in zip(plist, offs)}
-        if len(plist) != len(params) or any(id(p) not in where for p in params):
+        params = [p for g in self.param_groups for p in g["params"]]
+        if (param_groups is None and len(plist) != len(params)) or any(id(p) not in where for p in params):
             raise ValueError("FusedAdam: module.parameters() and the flat parameter list hold different tensors")
         if exp_avg.numel() != total or exp_avg_sq.numel() != total:
             raise ValueError(f"FusedAdam: moment buffers of {exp_avg.numel()} / {exp_avg_sq.numel()} elements, layout needs {total}")
-        self._slots = [(where[id(p)], p.numel()) for p in params]      # per module.parameters() index: (flat offset, numel)
+        self._slots = [(where[id(p)], p.numel()) for p in params]      # per state_dict index: (flat offset, numel)
         # frozen parameters (requires_grad=False when the trainer was built) get no state, as torch.optim.Adam gives them none
         self._trainable = [bool(p.requires_grad) for p in params]
         self._flat = (exp_avg, exp_avg_sq, step_count, hyper)
@@ -250,31 +338,51 @@ class FusedAdam(torch.optim.Optimizer):
         self._pushed = None
         self._push()
 
-    def _group(self):
-        if len(self.param_groups) != 1:
-            raise ValueError("FusedAdam supports exactly one parameter group")
-        g = self.param_groups[0]
-        bad = [k for k in _UNSUPPORTED if g.get(k)]
-        if bad:
-            raise ValueError(f"FusedAdam: {bad} are not supported (the fused kernels implement torch.optim.Adam with coupled L2)")
-        return g
+    def add_param_group(self, param_group):
+        """The group table's layout is fixed when the trainer is built: adding a group to it raises ``ValueError``."""
+        if self._sealed:
+            raise ValueError("FusedAdam: add_param_group after construction is not supported (the flat buffers and the group "
+                             "table are laid out when the trainer is built); pass every group to FusedTrainer(param_groups=...)")
+        super().add_param_group(param_group)
+
+    def _groups(self):
+        if not self._table and len(self.param_groups) != 1:
+            raise ValueError("FusedAdam supports exactly one parameter group (build the trainer with param_groups= for several)")
+        if len(self.param_groups) != len(self._flat[3]) and self._table:
+            raise ValueError("FusedAdam: the parameter groups no longer match the group table")
+        for g in self.param_groups:
+            bad = [k for k in (_UNSUPPORTED if not self._table else ("amsgrad", "maximize")) if g.get(k)]
+            if bad:
+                raise ValueError(f"FusedAdam: {bad} are not supported (the fused kernels implement torch.optim.Adam with coupled L2"
+                                 + ("" if self._table else "; build the trainer with decoupled_weight_decay=True or param_groups= "
+                                    "for AdamW") + ")")
+        return self.param_groups
 
     def _push(self):
-        """Writes the hyperparameters that changed since the last push into the device word, by value, in stream order
+        """Writes the hyperparameters that changed since the last push into the device words, by value, in stream order
         (no staging buffer the host could overwrite while the device lags behind)."""
-        g = self._group()
-        vals = (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))
+        groups = self._groups()
         hyper = self._flat[3]
+        if self._table:
+            rows = [group_row(g) for g in groups]
+            for i, row in enumerate(rows):
+                for j, x in enumerate(row):
+                    if self._pushed is None or self._pushed[i][j] != x:
+                        hyper[i, j].fill_(x)
+            self._pushed = rows
+            return
+        g = groups[0]
+        vals = (float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]), float(g["weight_decay"]))
         for i, x in enumerate(vals):
             if self._pushed is None or self._pushed[i] != x:
                 hyper[i].fill_(x)
         self._pushed = vals
 
     def step(self, closure=None):
-        """Hands ``param_groups[0]``'s lr / betas / eps / weight_decay to the kernels of the NEXT trainer step that updates the
-        parameters (the trainer calls this at the start of every such step — with gradient accumulation, the last micro-batch
-        of a window and ``flush()`` — so a scheduler stepped once per optimizer step follows the windows; a value is written
-        only when it changed).  Computes nothing itself."""
+        """Hands every group's lr / betas / eps / weight_decay (and, with the group table, decoupled_weight_decay) to the
+        kernels of the NEXT trainer step that updates the parameters (the trainer calls this at the start of every such step —
+        with gradient accumulation, the last micro-batch of a window and ``flush()`` — so a scheduler stepped once per optimizer
+        step follows the windows; a value is written only when it changed).  Computes nothing itself."""
         if closure is not None:
             raise ValueError("FusedAdam.step takes no closure: FusedTrainer.step runs forward and backward")
         self._push()
@@ -290,50 +398,64 @@ class FusedAdam(torch.optim.Optimizer):
         return out
 
     def state_dict(self):
-        """What ``torch.optim.Adam(module.parameters()).state_dict()`` returns after the same steps: per parameter index
-        ``{"step": float32 CPU tensor, "exp_avg", "exp_avg_sq"}`` (copies, shaped like the parameter, on its device) — empty
-        before the first step and for parameters frozen when the trainer was built — and the one parameter group.  Reads the
-        step counter from the device: one synchronisation.
+        """What ``torch.optim.Adam(groups).state_dict()`` (``torch.optim.AdamW`` for decoupled groups) returns after the same
+        steps: per parameter index — assigned in group order — ``{"step": float32 CPU tensor, "exp_avg", "exp_avg_sq"}``
+        (copies, shaped like the parameter, on its device), empty before the first step and for parameters frozen when the
+        trainer was built, and every group with its keys.  Reads the step counter from the device: one synchronisation.
         With sharded moments (``exchange="p2p"``) this is a collective: every rank must call it, and every rank gets the
         full state (each rank's owned slice, all-reduced)."""
-        g = self._group()
+        groups = self._groups()
         exp_avg, exp_avg_sq, step_count, _ = self._flat
         step = int(step_count.item())
         m, v = self._gathered(exp_avg), self._gathered(exp_avg_sq)
+        params = [p for g in groups for p in g["params"]]
         state = {}
         if step > 0:
-            for i, (p, (o, n)) in enumerate(zip(g["params"], self._slots)):
+            for i, (p, (o, n)) in enumerate(zip(params, self._slots)):
                 if not self._trainable[i]:
                     continue
                 state[i] = {"step": torch.tensor(float(step), dtype=torch.float32),
                             "exp_avg": m[o:o + n].view_as(p).clone(), "exp_avg_sq": v[o:o + n].view_as(p).clone()}
-        packed = {k: val for k, val in g.items() if k != "params"}
-        packed["params"] = list(range(len(g["params"])))
-        return {"state": state, "param_groups": [packed]}
+        packed, start = [], 0
+        for g in groups:
+            pg = {k: val for k, val in g.items() if k != "params"}
+            pg["params"] = list(range(start, start + len(g["params"])))
+            start += len(g["params"])
+            packed.append(pg)
+        return {"state": state, "param_groups": packed}
 
     def load_state_dict(self, state_dict):
         """Loads ``torch.optim.Adam``'s format (from :meth:`state_dict`, ``torch.optim.Adam.state_dict()`` or a Lightning
         checkpoint's ``optimizer_states[0]``), older forms included: ``step`` as int or tensor, group keys such as
         ``foreach`` / ``capturable`` / ``fused`` / ``differentiable`` missing; an empty ``state`` means step 0 and zero
-        moments.  Writes IN PLACE into the flat moment buffers, the step counter and the hyperparameter word, so CUDA
-        graphs captured before the load replay from the loaded state.  Every rank loads the full moments, whatever world
-        size wrote them.  Raises ``ValueError`` for more than one group, a parameter count or shape mismatch, AMSGrad,
-        ``maximize``, ``decoupled_weight_decay`` (AdamW) or per-parameter steps that differ.  Entries of parameters frozen when
-        the trainer was built are accepted and ignored; the step count comes from the trainable parameters only."""
+        moments.  With the group table, ``torch.optim.AdamW``'s too: each group's ``decoupled_weight_decay`` is loaded with its
+        other keys.  Writes IN PLACE into the flat moment buffers, the step counter and the hyperparameter words, so CUDA
+        graphs captured before the load replay from the loaded state.  Every rank loads the full moments, whatever world size
+        wrote them.  Raises ``ValueError`` (as torch does) for a different number of groups or of parameters in a group, and
+        for a shape mismatch, AMSGrad, ``maximize``, ``decoupled_weight_decay`` without the group table, or per-parameter
+        steps that differ.  Entries of parameters frozen when the trainer was built are accepted and ignored; the step count
+        comes from the trainable parameters only."""
         groups = state_dict.get("param_groups")
-        if not isinstance(groups, (list, tuple)) or len(groups) != 1:
-            raise ValueError(f"FusedAdam loads exactly one parameter group, got {len(groups) if groups is not None else None}")
-        saved = groups[0]
-        bad = [k for k in _UNSUPPORTED if saved.get(k)]
-        if bad:
-            raise ValueError(f"FusedAdam cannot load an optimizer with {bad} set")
-        cur = self._group()["params"]
-        ids = list(saved.get("params", []))
-        if len(ids) != len(cur):
-            raise ValueError(f"checkpoint has {len(ids)} parameters, the module {len(cur)}")
+        cur_groups = self._groups()
+        if not isinstance(groups, (list, tuple)) or len(groups) != len(cur_groups):
+            raise ValueError(f"FusedAdam has {len(cur_groups)} parameter group(s), the checkpoint "
+                             f"{len(groups) if isinstance(groups, (list, tuple)) else None}")
+        unsupported = _UNSUPPORTED if not self._table else ("amsgrad", "maximize")
+        ids = []
+        for gi, (saved, cur) in enumerate(zip(groups, cur_groups)):
+            bad = [k for k in unsupported if saved.get(k)]
+            if bad:
+                raise ValueError(f"FusedAdam cannot load an optimizer with {bad} set"
+                                 + ("" if self._table else " (build the trainer with decoupled_weight_decay=True or param_groups= "
+                                    "to load AdamW)"))
+            gids = list(saved.get("params", []))
+            if len(gids) != len(cur["params"]):
+                raise ValueError(f"parameter group {gi}: the checkpoint has {len(gids)} parameters, the optimizer {len(cur['params'])}")
+            ids += gids
+        cur = [p for g in cur_groups for p in g["params"]]
         state = state_dict.get("state", {})
         if set(state) - set(ids):
-            raise ValueError(f"state entries {sorted(set(state) - set(ids))} belong to no parameter of the group")
+            raise ValueError(f"state entries {sorted(set(state) - set(ids))} belong to no parameter of the groups")
         steps, entries = set(), []
         for i, (pid, p) in enumerate(zip(ids, cur)):
             st = state.get(pid)
@@ -365,8 +487,8 @@ class FusedAdam(torch.optim.Optimizer):
                     exp_avg[o:o + n].copy_(st["exp_avg"].reshape(-1))
                     exp_avg_sq[o:o + n].copy_(st["exp_avg_sq"].reshape(-1))
             step_count.fill_(step)
-        group = self.param_groups[0]
-        group.update({k: val for k, val in saved.items() if k != "params"})
+        for saved, group in zip(groups, cur_groups):
+            group.update({k: val for k, val in saved.items() if k != "params"})
         self._push()
 
 
@@ -386,7 +508,8 @@ class FusedTrainer:
                  max_resident_graphs: int = 64, distributed: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
                  bucket_min_pad_nodes: int = 64, overlap_allreduce: bool = True, exchange: str = "auto",
                  max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False, node_sample_seed: int = 0,
-                 track_metrics: bool = False, accumulate_grad_batches: int = 1):
+                 track_metrics: bool = False, accumulate_grad_batches: int = 1, param_groups=None,
+                 decoupled_weight_decay: bool = False):
         """``distributed=False`` makes this a single-rank trainer even inside an initialised process group (no all-reduce).
         ``bucket_nodes`` / ``bucket_edges`` > 0 switch on shape bucketing for HOST batches under ``use_cuda_graph``: every batch
         is padded with ONE dummy graph of isolated nodes up to the next multiple of ``bucket_nodes`` nodes (at least
@@ -433,7 +556,17 @@ class FusedTrainer:
         ``track_metrics``, bucketing and input checks stay per micro-batch.  ``optimizer.state_dict()`` may be taken during an
         open window: it holds no partial sum (as Lightning does not checkpoint ``.grad``), so a resumed run starts a fresh
         window.  ``k`` is fixed for the trainer's life.  With the default ``k = 1`` the step enqueues exactly what it did without
-        the argument."""
+        the argument.
+
+        Parameter groups and AdamW: ``param_groups`` is torch's list ``[{"params": [...], <lr, betas, eps, weight_decay,
+        decoupled_weight_decay>}, ...]`` (at most 64 groups), keys a group leaves out taking this constructor's arguments;
+        ``decoupled_weight_decay=True`` is ``torch.optim.AdamW`` / ``Adam(decoupled_weight_decay=True)`` — ``p *= 1 - lr *
+        weight_decay`` before the Adam step instead of L2 in the gradient — for every group that does not say otherwise.
+        Every trainable parameter must be in exactly one group (``ValueError`` names the one that is not); frozen parameters
+        may be in a group, and are skipped as torch skips them.  ``optimizer.state_dict()`` is then ``torch.optim.AdamW(groups)``'s
+        (``Adam``'s for coupled groups), indices in group order, and a ``LambdaLR`` with one lambda per group reaches captured
+        steps.  The update runs ``ddfa_adam_flat_groups`` / ``ddfa_allreduce_adam_p2p_groups[_guarded]`` on every step path.
+        With neither argument the step enqueues exactly what it did without them."""
         k = accumulate_grad_batches
         if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
             raise ValueError(f"accumulate_grad_batches must be an integer >= 1, got {accumulate_grad_batches!r}")
@@ -473,6 +606,9 @@ class FusedTrainer:
         # gradient slots are zeroed before the norm, and the backward is pruned to what the trainable parameters need.
         plist = module.param_list()
         flat = flat_param_list(module)
+        # parameter groups / AdamW: the group table and [begin, end, group] ranges of the grouped Adam entry points
+        self._grouped = param_groups is not None or bool(decoupled_weight_decay)
+        groups = resolve_param_groups(module, param_groups) if param_groups is not None else None
         self._flat_params = flat
         self._trainable = tuple(bool(p.requires_grad) for p in flat)
         self._ranges = trainable_ranges(flat)
@@ -527,13 +663,23 @@ class FusedTrainer:
             # the window's gradient sum (ddfa_grad_accumulate), laid out as flat_g without its loss slot; only with k > 1
             self._acc = torch.zeros(total, dtype=torch.float32, device=self.device) if self._k > 1 else None
             self.step_count = torch.zeros(1, dtype=torch.int32, device=self.device)
-            # [lr, beta1, beta2, eps, weight_decay], read by the Adam kernels when they run; written by self.optimizer.step()
-            self.hyper = torch.zeros(5, dtype=torch.float32, device=self.device)
-            if self._frozen:
-                self._ranges_dev = torch.tensor(self._ranges, dtype=torch.int64, device=self.device).reshape(-1)
+            # [lr, beta1, beta2, eps, weight_decay] — with parameter groups one such row per group, plus [decoupled, decay, pad]
+            # (group_row) — read by the Adam kernels when they run; written by self.optimizer.step()
+            if self._grouped:
+                ngroups = len(groups) if groups is not None else 1
+                self.hyper = torch.zeros(ngroups, _lib.ADAM_GROUP_WORDS, dtype=torch.float32, device=self.device)
+                group_of = ({id(p): gi for gi, g in enumerate(groups) for p in g["params"]} if groups is not None
+                            else {id(p): 0 for p in flat})
+                self._group_ranges = group_ranges(flat, group_of)
+                self._ranges_dev = torch.tensor(self._group_ranges, dtype=torch.int64, device=self.device).reshape(-1)
+            else:
+                self.hyper = torch.zeros(5, dtype=torch.float32, device=self.device)
+                if self._frozen:
+                    self._ranges_dev = torch.tensor(self._ranges, dtype=torch.int64, device=self.device).reshape(-1)
             shard = (self._p2p_rank, self.world, self.pg) if self.exchange == "p2p" else None
             self.optimizer = FusedAdam(module, self.exp_avg, self.exp_avg_sq, self.step_count, self.hyper, lr=lr, betas=betas, eps=eps,
-                                       weight_decay=weight_decay, shard=shard)
+                                       weight_decay=weight_decay, shard=shard, param_groups=groups,
+                                       decoupled_weight_decay=decoupled_weight_decay)
             if self._guard:
                 # the bound (a device word of its own, read when the step runs: not a param_groups key, so state_dict() stays
                 # torch.optim.Adam's), [norm, coef, nonfinite] of the last step, the skip counter and the norm's scratch
@@ -793,9 +939,16 @@ class FusedTrainer:
         without peer memory, the norm of the exchanged gradients comes first."""
         skipped = self._skipped.data_ptr() if self.skip_nonfinite else None      # skip_nonfinite implies the guard
         adam = (self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), self.step_count.data_ptr())
+        # parameter groups: the ranges with their group index and the group table
+        table = (self._ranges_dev.data_ptr(), len(self._group_ranges), self.hyper.data_ptr(), self.hyper.shape[0]) if self._grouped else None
         if self.exchange == "p2p":
             self._peer_arrays = tuple(_lib.ptr_array(p) for p in self._peer_ptrs)      # host arrays the calls point into
             head = (*self._peer_arrays, self._p2p_rank, self.world, *adam, self.numel, self.numel, self.loss_slot.data_ptr())
+            if self._grouped and self._guard:
+                return [("ddfa_allreduce_adam_p2p_groups_guarded", head + table + (self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
+                                                                                   skipped, self._guard_ws.data_ptr()))]
+            if self._grouped:
+                return [("ddfa_allreduce_adam_p2p_groups", head + (self._ticket.data_ptr(),) + table)]
             if self._guard:
                 return [("ddfa_allreduce_adam_p2p_guarded", head + (self.hyper.data_ptr(), self._max_norm_dev.data_ptr(),
                                                                     self._gstate.data_ptr(), skipped, self._guard_ws.data_ptr()))]
@@ -803,6 +956,8 @@ class FusedTrainer:
         flat = (self.flat_p.data_ptr(), self.flat_g.data_ptr(), *adam, self.numel, self.hyper.data_ptr())
         norm = [("ddfa_grad_norm", (self.flat_g.data_ptr(), self.numel, self._max_norm_dev.data_ptr(), self._gstate.data_ptr(),
                                     self._guard_ws.data_ptr(), self._guard_ws.numel()))] if self._guard else []
+        if self._grouped:
+            return norm + [("ddfa_adam_flat_groups", flat[:6] + table + ((self._gstate.data_ptr(), skipped) if self._guard else (None, None)))]
         if self._frozen:
             ranged = (*flat[:6], self._ranges_dev.data_ptr(), len(self._ranges), self.hyper.data_ptr())
             return norm + [("ddfa_adam_flat_ranges", ranged + ((self._gstate.data_ptr(), skipped) if self._guard else (None, None)))]

@@ -471,6 +471,23 @@ int ddfa_adam_flat_hp(float *params, const float *grads, float *exp_avg, float *
 int ddfa_adam_flat_ranges(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
                           int32_t *step_count, int64_t numel, const int64_t *ranges, int32_t num_ranges,
                           const float *hyper, const float *gstate, int32_t *skipped, void *stream);
+/* Parameter groups: torch.optim.Adam / torch.optim.AdamW (Adam(decoupled_weight_decay=True)) with several param_groups.
+ *   groups = device fp32[num_groups * DDFA_ADAM_GROUP_WORDS], one row per group:
+ *            [lr, beta1, beta2, eps, weight_decay, decoupled (1.0f / 0.0f), decay, pad], 1 <= num_groups <= DDFA_ADAM_MAX_GROUPS,
+ *            read when the kernel RUNS (as hyper in ddfa_adam_flat_hp).  decay = (float)(1.0 - (double)lr * weight_decay),
+ *            computed in double and rounded once, as torch's Python scalar is; coupled groups ignore it.
+ *   ranges = device int64[3 * num_ranges], sorted, disjoint [begin, end, group] triples inside [0, numel), every bound a
+ *            multiple of 4, group in [0, num_groups).  Elements outside every range are neither read nor written.
+ * A coupled group (decoupled = 0) computes torch.optim.Adam: results bit-identical to ddfa_adam_flat_ranges with that row's
+ * first five words as hyper.  A decoupled group computes torch.optim.AdamW's order (torch/optim/adam.py, _single_tensor_adam):
+ * p *= decay first, then the same moment and step expressions with no weight_decay * p term in the gradient.  Bias
+ * corrections are per group (fp64, from the one step_count).  gstate / skipped: NULL, or the guard as in ddfa_adam_flat_guarded.
+ * step_count advances once per call (not on a skipped step), also when num_ranges == 0. */
+#define DDFA_ADAM_GROUP_WORDS 8
+#define DDFA_ADAM_MAX_GROUPS 64
+int ddfa_adam_flat_groups(float *params, const float *grads, float *exp_avg, float *exp_avg_sq,
+                          int32_t *step_count, int64_t numel, const int64_t *ranges, int32_t num_ranges,
+                          const float *groups, int32_t num_groups, const float *gstate, int32_t *skipped, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K10'  The data-parallel exchange fused with the optimizer over NVLink peer memory: ONE kernel per rank does
@@ -538,6 +555,22 @@ int ddfa_allreduce_adam_p2p_guarded(void *const *peer_params, const void *const 
                                     int64_t numel, int64_t loss_offset, float *loss_out, const float *hyper,
                                     const float *max_norm, float *gstate, int32_t *skipped, void *guard_state,
                                     void *stream);
+/* Parameter groups over peer memory: ddfa_allreduce_adam_p2p_hp (ticket) and ddfa_allreduce_adam_p2p_guarded (guard_state) with
+ * the ranges / groups of ddfa_adam_flat_groups in place of hyper (both LOCAL device buffers, the same values on every rank).
+ * Each rank updates the intersection of its owned slice with the ranges; elements outside every range are neither read nor
+ * written, on any rank.  Every updated element is bit-identical to ddfa_adam_flat_groups on the gradient summed in rank
+ * order.  The guarded norm covers every element of every slice (the trainer zeroes gradients outside the ranges). */
+int ddfa_allreduce_adam_p2p_groups(void *const *peer_params, const void *const *peer_grads, void *const *peer_flags,
+                                   int32_t rank, int32_t world, float *exp_avg, float *exp_avg_sq, int32_t *step_count,
+                                   int64_t numel, int64_t loss_offset, float *loss_out, uint32_t *ticket,
+                                   const int64_t *ranges, int32_t num_ranges, const float *groups, int32_t num_groups,
+                                   void *stream);
+int ddfa_allreduce_adam_p2p_groups_guarded(void *const *peer_params, const void *const *peer_grads,
+                                           void *const *peer_flags, int32_t rank, int32_t world, float *exp_avg,
+                                           float *exp_avg_sq, int32_t *step_count, int64_t numel, int64_t loss_offset,
+                                           float *loss_out, const int64_t *ranges, int32_t num_ranges,
+                                           const float *groups, int32_t num_groups, const float *max_norm, float *gstate,
+                                           int32_t *skipped, void *guard_state, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Gradient accumulation over micro-batches (Lightning's accumulate_grad_batches): elementwise over the elements
