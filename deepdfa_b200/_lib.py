@@ -105,6 +105,14 @@ _SIGNATURES = {
     "ddfa_node_head_fwd": (_int, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
     "ddfa_node_bce": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, _vp, _vp, _vp]),
     "ddfa_node_bce_scaled": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, _f32, _vp, _vp, _vp]),
+    "ddfa_node_dp_exchange_words": (_sz, [_i32]),
+    "ddfa_node_dp_count": (_int, [_vp, _vp, _i32, C.c_double, _i32, _i32, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "ddfa_node_dp_plan": (_int, [_i32, C.c_double, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "ddfa_node_dp_radix_hist": (_int, [_vp, _vp, _i32, C.c_uint64, _i32, _vp, _sz, _vp, _vp]),
+    "ddfa_node_dp_radix_pick": (_int, [_i32, _i32, _vp, _sz, _vp, _vp]),
+    "ddfa_node_dp_ties": (_int, [_vp, _vp, _i32, C.c_uint64, _i32, _i32, _vp, _sz, _vp, _vp]),
+    "ddfa_node_dp_rows": (_int, [_vp, _vp, _i32, C.c_uint64, _i32, _i32, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "ddfa_node_bce_global": (_int, [_vp, _vp, _vp, _vp, _vp, _i32, _f32, _f32, _vp, _vp, _vp]),
     "ddfa_node_head_bwd_workspace_bytes": (_sz, [_i32, _i32]),
     "ddfa_node_head_bwd": (_int, [_vp] * 5 + [_i32, _i32, _vp, _i32] + [_vp] * 6 + [_sz, _vp]),
     "ddfa_eval_metrics_workspace_bytes": (_sz, []),
@@ -121,7 +129,7 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
               "ddfa_build_csr_workspace_bytes", "ddfa_arena_batch_workspace_bytes", "ddfa_gru_step_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes_steps",
               "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes",
               "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
-              "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes"}
+              "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes"}
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
 GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate

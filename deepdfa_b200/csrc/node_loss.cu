@@ -12,6 +12,11 @@
 // compacted in ascending node order by a block-count / scan / write sequence.  Integer counts only: the result does not depend on
 // the order in which CTAs run.
 //
+// Several ranks (ddfa_node_dp_*): the same kernels, run in phases over one rank's shard of a global batch, with the caller's SUM
+// exchanges between them: per-rank counts, the digit histograms (written to the exchange buffer instead of the workspace) and the
+// tie counts.  Keys are those of node kOff + n of the global batch (kOff = 0 on one rank) and the block scan takes the ties of
+// the ranks before this one first, so the union of the ranks' rows is ddfa_node_sample's row list of the concatenated batch.
+//
 // Head: SIMT fp32 (FFMA), so every hidden width works.  Hidden layers are 64 x 64-tiled GEMMs over the row list (layer 0 gathers
 // [h_T[r] | x[r]] straight from the two planes); the last layer is a warp per row.  Weight and bias gradients are reduced over the
 // rows in a fixed order in both tuning modes: kHeadChunks private partials over fixed row chunks, added in chunk order.
@@ -31,7 +36,8 @@ constexpr int kHeadChunks = 32;                      // row chunks of the weight
 constexpr int kMaxLayers = 16;
 
 // control words
-enum { kNVuln = 0, kPop = 1, kK = 2, kPrefix = 3, kKRem = 4, kDrawLo = 5, kDrawHi = 6 };
+// kOff: the node offset of this rank's shard in the global batch (0 on one rank): node n's key is that of node kOff + n
+enum { kNVuln = 0, kPop = 1, kK = 2, kPrefix = 3, kKRem = 4, kDrawLo = 5, kDrawHi = 6, kOff = 7 };
 
 inline int32_t num_blocks(int32_t N) { return (N + kPerBlock - 1) / kPerBlock; }
 
@@ -104,7 +110,7 @@ __global__ void __launch_bounds__(kThreads) sample_count_kernel(const int32_t *_
 
 // k = rint(n_vuln * factor) in fp64 (Python's round() of the same product), clamped to the population with the status word set;
 // takes this call's draw index and advances the caller's counter
-__global__ void sample_k_kernel(int32_t *__restrict__ ctl, double factor, int64_t *__restrict__ draw, int32_t *__restrict__ status) {
+__device__ __forceinline__ void draw_size(int32_t *__restrict__ ctl, double factor, int64_t *__restrict__ draw, int32_t *__restrict__ status) {
   const double want = rint((double)ctl[kNVuln] * factor);
   const int32_t pop = ctl[kPop];
   int32_t k;
@@ -123,31 +129,57 @@ __global__ void sample_k_kernel(int32_t *__restrict__ ctl, double factor, int64_
   *draw = d + 1;
 }
 
+__global__ void sample_k_kernel(int32_t *__restrict__ ctl, double factor, int64_t *__restrict__ draw, int32_t *__restrict__ status) {
+  draw_size(ctl, factor, draw, status);
+}
+
+// several ranks: counts[2q..2q+2) = [n_vuln, n_pop] of rank q (summed over the ranks by the caller's exchange).  The global counts
+// and this rank's node offset go into ctl, then k / status / draw as on one rank; num_rows_global = S of the global batch
+__global__ void dp_plan_kernel(const int32_t *__restrict__ counts, int32_t rank, int32_t world, double factor, int64_t *__restrict__ draw,
+                               int32_t *__restrict__ status, int32_t *__restrict__ ctl, int32_t *__restrict__ num_rows_global,
+                               int32_t *__restrict__ node_offset) {
+  int32_t nvul = 0, pop = 0, off = 0;
+  for (int32_t q = 0; q < world; ++q) {
+    nvul += counts[2 * q];
+    pop += counts[2 * q + 1];
+    if (q < rank) off += counts[2 * q] + counts[2 * q + 1];
+  }
+  *node_offset = off;
+  if (!(factor >= 0.0)) {      // no undersampling: every valid node of every rank
+    *num_rows_global = nvul + pop;
+    return;
+  }
+  ctl[kNVuln] = nvul;
+  ctl[kPop] = pop;
+  ctl[kOff] = off;
+  draw_size(ctl, factor, draw, status);
+  *num_rows_global = nvul + ctl[kK];
+}
+
 // histogram of digit `pass` over the candidates whose higher digits equal the prefix picked so far
 __global__ void __launch_bounds__(kThreads) radix_hist_kernel(const int32_t *__restrict__ vuln, const int32_t *__restrict__ num_valid, int32_t N,
-                                                              uint64_t seed, int pass, int32_t *__restrict__ ctl) {
+                                                              uint64_t seed, int pass, int32_t *__restrict__ ctl, uint32_t *__restrict__ hist) {
   __shared__ uint32_t s_hist[kBins];
   if (ctl[kK] == 0) return;
   s_hist[threadIdx.x] = 0u;
   __syncthreads();
   const int32_t nv = valid_count(num_valid, N);
-  const uint32_t dlo = (uint32_t)ctl[kDrawLo], dhi = (uint32_t)ctl[kDrawHi], prefix = (uint32_t)ctl[kPrefix];
+  const uint32_t dlo = (uint32_t)ctl[kDrawLo], dhi = (uint32_t)ctl[kDrawHi], prefix = (uint32_t)ctl[kPrefix], off = (uint32_t)ctl[kOff];
   const int shift = 24 - 8 * pass;
   for (int64_t n = blockIdx.x * (int64_t)kThreads + threadIdx.x; n < nv; n += (int64_t)gridDim.x * kThreads) {
     if (vuln[n] != 0) continue;
-    const uint32_t key = philox_key(dlo, dhi, (uint32_t)n, seed);
+    const uint32_t key = philox_key(dlo, dhi, off + (uint32_t)n, seed);
     if (pass > 0 && (key >> (shift + 8)) != (prefix >> (shift + 8))) continue;
     atomicAdd(&s_hist[(key >> shift) & 255u], 1u);
   }
   __syncthreads();
   const uint32_t c = s_hist[threadIdx.x];
-  if (c) atomicAdd(reinterpret_cast<uint32_t *>(ctl + kCtl) + threadIdx.x, c);
+  if (c) atomicAdd(hist + threadIdx.x, c);
 }
 
 // the bin that holds the k_rem-th smallest candidate: its digit goes into the prefix, k_rem becomes the rank inside it; clears
 // the histogram for the next pass
-__global__ void __launch_bounds__(kBins) radix_pick_kernel(int pass, int32_t *__restrict__ ctl) {
-  uint32_t *hist = reinterpret_cast<uint32_t *>(ctl + kCtl);
+__global__ void __launch_bounds__(kBins) radix_pick_kernel(int pass, int32_t *__restrict__ ctl, uint32_t *__restrict__ hist) {
   if (ctl[kK] == 0) return;
   __shared__ uint32_t s_hist[kBins];
   s_hist[threadIdx.x] = hist[threadIdx.x];
@@ -168,12 +200,12 @@ __global__ void __launch_bounds__(kBins) radix_pick_kernel(int pass, int32_t *__
 }
 
 // node n's class: 2 = in the list for sure (vulnerable, or key below the threshold), 1 = tie at the threshold key, 0 = out
-__device__ __forceinline__ int node_class(const int32_t *__restrict__ vuln, int32_t n, int32_t nv, uint32_t dlo, uint32_t dhi, uint64_t seed,
-                                          uint32_t thresh, bool any) {
+__device__ __forceinline__ int node_class(const int32_t *__restrict__ vuln, int32_t n, int32_t nv, uint32_t dlo, uint32_t dhi, uint32_t off,
+                                          uint64_t seed, uint32_t thresh, bool any) {
   if (n >= nv) return 0;
   if (vuln[n] != 0) return 2;
   if (!any) return 0;
-  const uint32_t key = philox_key(dlo, dhi, (uint32_t)n, seed);
+  const uint32_t key = philox_key(dlo, dhi, off + (uint32_t)n, seed);
   return key < thresh ? 2 : (key == thresh ? 1 : 0);
 }
 
@@ -182,13 +214,13 @@ __global__ void __launch_bounds__(kThreads) sample_block_count_kernel(const int3
                                                                       int32_t N, uint64_t seed, const int32_t *__restrict__ ctl,
                                                                       int32_t *__restrict__ blk) {
   const int32_t nv = valid_count(num_valid, N);
-  const uint32_t dlo = (uint32_t)ctl[kDrawLo], dhi = (uint32_t)ctl[kDrawHi], thresh = (uint32_t)ctl[kPrefix];
+  const uint32_t dlo = (uint32_t)ctl[kDrawLo], dhi = (uint32_t)ctl[kDrawHi], thresh = (uint32_t)ctl[kPrefix], off = (uint32_t)ctl[kOff];
   const bool any = ctl[kK] > 0;
   int32_t sure = 0, tie = 0;
   const int32_t n0 = blockIdx.x * kPerBlock + threadIdx.x * kPerThread;
 #pragma unroll
   for (int j = 0; j < kPerThread; ++j) {
-    const int c = node_class(vuln, n0 + j, nv, dlo, dhi, seed, thresh, any);
+    const int c = node_class(vuln, n0 + j, nv, dlo, dhi, off, seed, thresh, any);
     sure += c == 2;
     tie += c == 1;
   }
@@ -201,11 +233,15 @@ __global__ void __launch_bounds__(kThreads) sample_block_count_kernel(const int3
   }
 }
 
-// one CTA, in CTA order: blk[2nb..3nb) = ties before each CTA, blk[3nb..4nb) = rows before each CTA; S
+// one CTA, in CTA order: blk[2nb..3nb) = ties before each CTA, blk[3nb..4nb) = rows before each CTA; S.  Several ranks:
+// rank_ties[q] = the ties of rank q, and the ties of ranks q < rank come before this rank's (NULL: one rank)
 __global__ void __launch_bounds__(kThreads) sample_block_scan_kernel(int32_t nb, const int32_t *__restrict__ ctl, int32_t *__restrict__ blk,
-                                                                     int32_t *__restrict__ num_rows) {
+                                                                     int32_t *__restrict__ num_rows, const int32_t *__restrict__ rank_ties,
+                                                                     int32_t rank) {
   const int32_t take = ctl[kK] > 0 ? ctl[kKRem] : 0;
   int32_t tie_carry = 0, row_carry = 0;
+  if (rank_ties)
+    for (int32_t q = 0; q < rank; ++q) tie_carry += rank_ties[q];
   for (int32_t b0 = 0; b0 < nb; b0 += kThreads) {
     const int32_t b = b0 + threadIdx.x;
     const int32_t sure = b < nb ? blk[b] : 0, tie = b < nb ? blk[nb + b] : 0;
@@ -224,12 +260,21 @@ __global__ void __launch_bounds__(kThreads) sample_block_scan_kernel(int32_t nb,
   if (threadIdx.x == 0) *num_rows = row_carry;
 }
 
+// this rank's ties at the threshold key: the sum of blk[nb..2nb)
+__global__ void __launch_bounds__(kThreads) tie_total_kernel(int32_t nb, const int32_t *__restrict__ blk, int32_t *__restrict__ out) {
+  int32_t acc = 0;
+  for (int32_t b = threadIdx.x; b < nb; b += kThreads) acc += blk[nb + b];
+  int32_t total;
+  block_scan(acc, &total);
+  if (threadIdx.x == 0) *out = total;
+}
+
 __global__ void __launch_bounds__(kThreads) sample_write_kernel(const int32_t *__restrict__ vuln, const int32_t *__restrict__ num_valid, int32_t N,
                                                                 uint64_t seed, const int32_t *__restrict__ ctl, const int32_t *__restrict__ blk,
                                                                 int32_t *__restrict__ rows) {
   const int32_t nb = gridDim.x;
   const int32_t nv = valid_count(num_valid, N);
-  const uint32_t dlo = (uint32_t)ctl[kDrawLo], dhi = (uint32_t)ctl[kDrawHi], thresh = (uint32_t)ctl[kPrefix];
+  const uint32_t dlo = (uint32_t)ctl[kDrawLo], dhi = (uint32_t)ctl[kDrawHi], thresh = (uint32_t)ctl[kPrefix], off = (uint32_t)ctl[kOff];
   const bool any = ctl[kK] > 0;
   const int32_t take = any ? ctl[kKRem] : 0;
   const int32_t n0 = blockIdx.x * kPerBlock + threadIdx.x * kPerThread;
@@ -237,7 +282,7 @@ __global__ void __launch_bounds__(kThreads) sample_write_kernel(const int32_t *_
   int32_t tie = 0;
 #pragma unroll
   for (int j = 0; j < kPerThread; ++j) {
-    cls[j] = node_class(vuln, n0 + j, nv, dlo, dhi, seed, thresh, any);
+    cls[j] = node_class(vuln, n0 + j, nv, dlo, dhi, off, seed, thresh, any);
     tie += cls[j] == 1;
   }
   int32_t total;
@@ -449,13 +494,16 @@ __global__ void __launch_bounds__(256) chunk_reduce_kernel(const float *__restri
 
 // mean BCEWithLogits(pos_weight) over the S rows, one CTA in a fixed order (graph_label_bce_kernel's formula); S = 0 gives NaN.
 // Scaled: the gradient's row scale is (1 / S) * grad_scale (gradient accumulation); the unscaled form never reads grad_scale.
+// norm (several ranks): the sum over the S rows divided by *norm, the global row count, instead of S (NULL: by S)
 template <bool Scaled>
 __global__ void __launch_bounds__(1024) node_bce_kernel(const float *__restrict__ logits, const int32_t *__restrict__ vuln,
-                                                        const int32_t *__restrict__ rows, const int32_t *__restrict__ num_rows, float pos_weight,
-                                                        float grad_scale, float *__restrict__ loss_out, float *__restrict__ dlogits) {
+                                                        const int32_t *__restrict__ rows, const int32_t *__restrict__ num_rows,
+                                                        const int32_t *__restrict__ norm, float pos_weight, float grad_scale,
+                                                        float *__restrict__ loss_out, float *__restrict__ dlogits) {
   __shared__ float s_t[1024];
   const int32_t S = *num_rows;
-  const float inv = Scaled ? (1.f / (float)S) * grad_scale : 1.f / (float)S;
+  const float div = (float)(norm ? *norm : S);
+  const float inv = Scaled ? (1.f / div) * grad_scale : 1.f / div;
   float acc = 0.f;
   for (int32_t s = threadIdx.x; s < S; s += 1024) {
     const float xv = logits[s], y = (float)vuln[rows[s]];
@@ -469,7 +517,7 @@ __global__ void __launch_bounds__(1024) node_bce_kernel(const float *__restrict_
     if (threadIdx.x < o) s_t[threadIdx.x] += s_t[threadIdx.x + o];
     __syncthreads();
   }
-  if (threadIdx.x == 0 && loss_out) *loss_out = s_t[0] / (float)S;
+  if (threadIdx.x == 0 && loss_out) *loss_out = s_t[0] / div;
 }
 
 inline unsigned cdiv(int64_t a, int64_t b) { return (unsigned)((a + b - 1) / b); }
@@ -520,6 +568,7 @@ int ddfa_node_sample(const int32_t *vuln, const int32_t *num_valid, int32_t N, d
     return DDFA_ERR_WORKSPACE;
   }
   int32_t *ctl = static_cast<int32_t *>(workspace);
+  uint32_t *hist = reinterpret_cast<uint32_t *>(ctl + kCtl);
   int32_t *blk = ctl + kCtl + kBins;
   const int32_t nb = num_blocks(N) > 0 ? num_blocks(N) : 1;
   const unsigned grid = (unsigned)min(nb, 4 * kNumSMs);
@@ -529,17 +578,140 @@ int ddfa_node_sample(const int32_t *vuln, const int32_t *num_valid, int32_t N, d
   sample_k_kernel<<<1, 1, 0, stream>>>(ctl, factor, draw, status);
   DDFA_CHECK_LAUNCH("sample_k_kernel");
   for (int pass = 0; pass < 4; ++pass) {
-    radix_hist_kernel<<<grid, kThreads, 0, stream>>>(vuln, num_valid, N, seed, pass, ctl);
+    radix_hist_kernel<<<grid, kThreads, 0, stream>>>(vuln, num_valid, N, seed, pass, ctl, hist);
     DDFA_CHECK_LAUNCH("radix_hist_kernel");
-    radix_pick_kernel<<<1, kBins, 0, stream>>>(pass, ctl);
+    radix_pick_kernel<<<1, kBins, 0, stream>>>(pass, ctl, hist);
     DDFA_CHECK_LAUNCH("radix_pick_kernel");
   }
   sample_block_count_kernel<<<nb, kThreads, 0, stream>>>(vuln, num_valid, N, seed, ctl, blk);
   DDFA_CHECK_LAUNCH("sample_block_count_kernel");
-  sample_block_scan_kernel<<<1, kThreads, 0, stream>>>(nb, ctl, blk, num_rows);
+  sample_block_scan_kernel<<<1, kThreads, 0, stream>>>(nb, ctl, blk, num_rows, nullptr, 0);
   DDFA_CHECK_LAUNCH("sample_block_scan_kernel");
   sample_write_kernel<<<nb, kThreads, 0, stream>>>(vuln, num_valid, N, seed, ctl, blk, rows);
   DDFA_CHECK_LAUNCH("sample_write_kernel");
+  return DDFA_OK;
+}
+
+// ---- several ranks: the draw of the global batch in phases, with the exchanges between them left to the caller ----------------
+size_t ddfa_node_dp_exchange_words(int32_t world) {
+  using namespace ddfa::node;
+  if (world < 1) return 0;
+  return (size_t)kBins + 3 * (size_t)world;
+}
+
+namespace {
+int dp_check(const char *who, int32_t N, int32_t rank, int32_t world, const void *workspace, size_t workspace_bytes, const void *exchange) {
+  using namespace ddfa;
+  DDFA_REQUIRE(N >= 0 && world >= 1 && rank >= 0 && rank < world, "%s: num_nodes=%d rank=%d world=%d", who, N, rank, world);
+  DDFA_REQUIRE(workspace && exchange, "%s: NULL workspace or exchange buffer", who);
+  if (workspace_bytes < ddfa_node_sample_workspace_bytes(N)) {
+    set_error("%s: workspace too small (%zu < %zu)", who, workspace_bytes, ddfa_node_sample_workspace_bytes(N));
+    return DDFA_ERR_WORKSPACE;
+  }
+  return DDFA_OK;
+}
+}  // namespace
+
+int ddfa_node_dp_count(const int32_t *vuln, const int32_t *num_valid, int32_t N, double factor, int32_t rank, int32_t world,
+                       int32_t *rows, int32_t *num_rows, void *workspace, size_t workspace_bytes, int32_t *exchange, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  if (int rc = dp_check("ddfa_node_dp_count", N, rank, world, workspace, workspace_bytes, exchange)) return rc;
+  DDFA_REQUIRE(num_valid && num_rows && (vuln || N == 0) && (rows || N == 0), "ddfa_node_dp_count: NULL pointer");
+  cudaStream_t stream = as_stream(stream_);
+  int32_t *ctl = static_cast<int32_t *>(workspace);
+  const int32_t nb = num_blocks(N) > 0 ? num_blocks(N) : 1;
+  DDFA_CUDA(cudaMemsetAsync(ctl, 0, sizeof(int32_t) * (kCtl + kBins), stream));
+  DDFA_CUDA(cudaMemsetAsync(exchange, 0, sizeof(int32_t) * ddfa_node_dp_exchange_words(world), stream));
+  sample_count_kernel<<<(unsigned)min(nb, 4 * kNumSMs), kThreads, 0, stream>>>(vuln, num_valid, N, exchange + kBins + 2 * rank);
+  DDFA_CHECK_LAUNCH("sample_count_kernel");
+  if (!(factor >= 0.0)) {       // no undersampling: the rows are every local valid node now
+    sample_all_kernel<<<cdiv(N > 0 ? N : 1, kThreads), kThreads, 0, stream>>>(num_valid, N, rows, num_rows);
+    DDFA_CHECK_LAUNCH("sample_all_kernel");
+  }
+  return DDFA_OK;
+}
+
+int ddfa_node_dp_plan(int32_t N, double factor, int32_t rank, int32_t world, int64_t *draw, int32_t *status, int32_t *num_rows_global,
+                      int32_t *node_offset, void *workspace, size_t workspace_bytes, const int32_t *exchange, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  if (int rc = dp_check("ddfa_node_dp_plan", N, rank, world, workspace, workspace_bytes, exchange)) return rc;
+  DDFA_REQUIRE(num_rows_global && node_offset && (!(factor >= 0.0) || (draw && status)), "ddfa_node_dp_plan: NULL pointer");
+  dp_plan_kernel<<<1, 1, 0, as_stream(stream_)>>>(exchange + kBins, rank, world, factor, draw, status, static_cast<int32_t *>(workspace),
+                                                  num_rows_global, node_offset);
+  DDFA_CHECK_LAUNCH("dp_plan_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_node_dp_radix_hist(const int32_t *vuln, const int32_t *num_valid, int32_t N, uint64_t seed, int32_t pass, void *workspace,
+                            size_t workspace_bytes, int32_t *exchange, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  if (int rc = dp_check("ddfa_node_dp_radix_hist", N, 0, 1, workspace, workspace_bytes, exchange)) return rc;
+  DDFA_REQUIRE(pass >= 0 && pass < 4, "ddfa_node_dp_radix_hist: pass=%d not in [0, 4)", pass);
+  DDFA_REQUIRE(num_valid && (vuln || N == 0), "ddfa_node_dp_radix_hist: NULL pointer");
+  const int32_t nb = num_blocks(N) > 0 ? num_blocks(N) : 1;
+  radix_hist_kernel<<<(unsigned)min(nb, 4 * kNumSMs), kThreads, 0, as_stream(stream_)>>>(vuln, num_valid, N, seed, pass,
+                                                                                          static_cast<int32_t *>(workspace),
+                                                                                          reinterpret_cast<uint32_t *>(exchange));
+  DDFA_CHECK_LAUNCH("radix_hist_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_node_dp_radix_pick(int32_t N, int32_t pass, void *workspace, size_t workspace_bytes, int32_t *exchange, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  if (int rc = dp_check("ddfa_node_dp_radix_pick", N, 0, 1, workspace, workspace_bytes, exchange)) return rc;
+  DDFA_REQUIRE(pass >= 0 && pass < 4, "ddfa_node_dp_radix_pick: pass=%d not in [0, 4)", pass);
+  radix_pick_kernel<<<1, kBins, 0, as_stream(stream_)>>>(pass, static_cast<int32_t *>(workspace), reinterpret_cast<uint32_t *>(exchange));
+  DDFA_CHECK_LAUNCH("radix_pick_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_node_dp_ties(const int32_t *vuln, const int32_t *num_valid, int32_t N, uint64_t seed, int32_t rank, int32_t world, void *workspace,
+                      size_t workspace_bytes, int32_t *exchange, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  if (int rc = dp_check("ddfa_node_dp_ties", N, rank, world, workspace, workspace_bytes, exchange)) return rc;
+  DDFA_REQUIRE(num_valid && (vuln || N == 0), "ddfa_node_dp_ties: NULL pointer");
+  cudaStream_t stream = as_stream(stream_);
+  int32_t *ctl = static_cast<int32_t *>(workspace);
+  int32_t *blk = ctl + kCtl + kBins;
+  const int32_t nb = num_blocks(N) > 0 ? num_blocks(N) : 1;
+  sample_block_count_kernel<<<nb, kThreads, 0, stream>>>(vuln, num_valid, N, seed, ctl, blk);
+  DDFA_CHECK_LAUNCH("sample_block_count_kernel");
+  tie_total_kernel<<<1, kThreads, 0, stream>>>(nb, blk, exchange + kBins + 2 * world + rank);
+  DDFA_CHECK_LAUNCH("tie_total_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_node_dp_rows(const int32_t *vuln, const int32_t *num_valid, int32_t N, uint64_t seed, int32_t rank, int32_t world, int32_t *rows,
+                      int32_t *num_rows, void *workspace, size_t workspace_bytes, const int32_t *exchange, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  if (int rc = dp_check("ddfa_node_dp_rows", N, rank, world, workspace, workspace_bytes, exchange)) return rc;
+  DDFA_REQUIRE(num_valid && num_rows && (vuln || N == 0) && (rows || N == 0), "ddfa_node_dp_rows: NULL pointer");
+  cudaStream_t stream = as_stream(stream_);
+  int32_t *ctl = static_cast<int32_t *>(workspace);
+  int32_t *blk = ctl + kCtl + kBins;
+  const int32_t nb = num_blocks(N) > 0 ? num_blocks(N) : 1;
+  sample_block_scan_kernel<<<1, kThreads, 0, stream>>>(nb, ctl, blk, num_rows, exchange + kBins + 2 * world, rank);
+  DDFA_CHECK_LAUNCH("sample_block_scan_kernel");
+  sample_write_kernel<<<nb, kThreads, 0, stream>>>(vuln, num_valid, N, seed, ctl, blk, rows);
+  DDFA_CHECK_LAUNCH("sample_write_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_node_bce_global(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows, const int32_t *num_rows_global,
+                         int32_t N, float pos_weight, float grad_scale, float *loss_out, float *dlogits, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::node;
+  DDFA_REQUIRE(N >= 0, "ddfa_node_bce_global: num_nodes=%d < 0", N);
+  DDFA_REQUIRE(logits && vuln && rows && num_rows && num_rows_global, "ddfa_node_bce_global: NULL pointer");
+  node_bce_kernel<true><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, num_rows_global, pos_weight, grad_scale, loss_out,
+                                                            dlogits);
+  DDFA_CHECK_LAUNCH("node_bce_kernel");
   return DDFA_OK;
 }
 
@@ -581,7 +753,7 @@ int ddfa_node_bce(const float *logits, const int32_t *vuln, const int32_t *rows,
   using namespace ddfa::node;
   DDFA_REQUIRE(N >= 0, "ddfa_node_bce: num_nodes=%d < 0", N);
   DDFA_REQUIRE(logits && vuln && rows && num_rows, "ddfa_node_bce: NULL pointer");
-  node_bce_kernel<false><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, pos_weight, 1.f, loss_out, dlogits);
+  node_bce_kernel<false><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, nullptr, pos_weight, 1.f, loss_out, dlogits);
   DDFA_CHECK_LAUNCH("node_bce_kernel");
   return DDFA_OK;
 }
@@ -592,7 +764,8 @@ int ddfa_node_bce_scaled(const float *logits, const int32_t *vuln, const int32_t
   using namespace ddfa::node;
   DDFA_REQUIRE(N >= 0, "ddfa_node_bce_scaled: num_nodes=%d < 0", N);
   DDFA_REQUIRE(logits && vuln && rows && num_rows, "ddfa_node_bce_scaled: NULL pointer");
-  node_bce_kernel<true><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, pos_weight, grad_scale, loss_out, dlogits);
+  node_bce_kernel<true><<<1, 1024, 0, as_stream(stream_)>>>(logits, vuln, rows, num_rows, nullptr, pos_weight, grad_scale, loss_out,
+                                                                 dlogits);
   DDFA_CHECK_LAUNCH("node_bce_kernel");
   return DDFA_OK;
 }

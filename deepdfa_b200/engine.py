@@ -567,6 +567,91 @@ def node_sample(vuln: torch.Tensor, num_valid: torch.Tensor, factor: Optional[fl
           ws_bytes, _stream_ptr())
 
 
+class NodeDrawDP:
+    """The phases of the node-row draw over the global batch of ``world`` ranks (``ddfa_node_dp_*``, include/ddfa_b200.h), for
+    the rank ``rank`` whose shard has ``rows.numel()`` nodes (capacity).  Between the phases the caller SUM-all-reduces one
+    region of ``exchange`` over the ranks: :meth:`counts` after :meth:`count`, :meth:`hist` after each :meth:`radix_hist`,
+    :meth:`ties` after :meth:`tie_count`.  :meth:`run` sequences them with a given all-reduce; a test can call the phases of
+    several emulated ranks in lockstep.  ``node_offset`` / ``num_rows_global`` (int32 [1]) receive this shard's first node in
+    the global batch and the global row count S."""
+
+    def __init__(self, vuln, num_valid, factor, seed: int, draw, rows, num_rows, status, num_rows_global, node_offset, rank: int,
+                 world: int, alloc=None):
+        self.vuln, self.num_valid, self.seed, self.draw, self.rows, self.num_rows, self.status = vuln, num_valid, int(seed), draw, rows, num_rows, status
+        self.factor = -1.0 if factor is None else float(factor)
+        self.num_rows_global, self.node_offset, self.rank, self.world = num_rows_global, node_offset, int(rank), int(world)
+        self.N = rows.numel()
+        L = _lib.lib()
+        alloc = alloc or _FreshAlloc(rows.device)
+        self.ws_bytes = L.call("ddfa_node_sample_workspace_bytes", self.N)
+        self.ws = alloc.get("node_sample_ws", (max(self.ws_bytes, 16),), torch.uint8)
+        self.exchange = alloc.get("node_dp_exchange", (L.call("ddfa_node_dp_exchange_words", self.world),), torch.int32)
+
+    @property
+    def undersampled(self) -> bool:
+        return self.factor >= 0.0
+
+    def counts(self) -> torch.Tensor:
+        return self.exchange[256:256 + 2 * self.world]
+
+    def hist(self) -> torch.Tensor:
+        return self.exchange[:256]
+
+    def ties(self) -> torch.Tensor:
+        return self.exchange[256 + 2 * self.world:]
+
+    def count(self):
+        _call("ddfa_node_dp_count", _p(self.vuln), _p(self.num_valid), self.N, self.factor, self.rank, self.world, _p(self.rows),
+              _p(self.num_rows), _p(self.ws), self.ws_bytes, _p(self.exchange), _stream_ptr())
+
+    def plan(self):
+        _call("ddfa_node_dp_plan", self.N, self.factor, self.rank, self.world, _p(self.draw), _p(self.status), _p(self.num_rows_global),
+              _p(self.node_offset), _p(self.ws), self.ws_bytes, _p(self.exchange), _stream_ptr())
+
+    def radix_hist(self, p: int):
+        _call("ddfa_node_dp_radix_hist", _p(self.vuln), _p(self.num_valid), self.N, self.seed, p, _p(self.ws), self.ws_bytes,
+              _p(self.exchange), _stream_ptr())
+
+    def radix_pick(self, p: int):
+        _call("ddfa_node_dp_radix_pick", self.N, p, _p(self.ws), self.ws_bytes, _p(self.exchange), _stream_ptr())
+
+    def tie_count(self):
+        _call("ddfa_node_dp_ties", _p(self.vuln), _p(self.num_valid), self.N, self.seed, self.rank, self.world, _p(self.ws),
+              self.ws_bytes, _p(self.exchange), _stream_ptr())
+
+    def finish(self):
+        _call("ddfa_node_dp_rows", _p(self.vuln), _p(self.num_valid), self.N, self.seed, self.rank, self.world, _p(self.rows),
+              _p(self.num_rows), _p(self.ws), self.ws_bytes, _p(self.exchange), _stream_ptr())
+
+    def run(self, all_reduce):
+        """The whole draw on the current stream; ``all_reduce(t)`` sums the int32 tensor ``t`` over the ranks in place (one call
+        without undersampling, six with it)."""
+        self.count()
+        all_reduce(self.counts())
+        self.plan()
+        if not self.undersampled:
+            return
+        for p in range(4):
+            self.radix_hist(p)
+            all_reduce(self.hist())
+            self.radix_pick(p)
+        self.tie_count()
+        all_reduce(self.ties())
+        self.finish()
+
+
+def node_bce_global(logits: torch.Tensor, vuln: torch.Tensor, rows: torch.Tensor, num_rows: torch.Tensor, num_rows_global: torch.Tensor,
+                    pos_weight: float, loss_out: torch.Tensor, grad_scale: float = 1.0, alloc=None):
+    """``ddfa_node_bce_global``: this rank's share of the global mean BCE (the sum over its S rows / S_global) into ``loss_out``
+    and dlogits scaled by ``grad_scale / S_global`` (fp32 [N] capacity), returned."""
+    N = logits.numel()
+    alloc = alloc or _FreshAlloc(logits.device)
+    dlogits = alloc.get("node_dlogits", (N,))
+    _call("ddfa_node_bce_global", _p(logits), _p(vuln), _p(rows), _p(num_rows), _p(num_rows_global), N, float(pos_weight),
+          float(grad_scale), _p(loss_out), _p(dlogits), _stream_ptr())
+    return dlogits
+
+
 def node_head_fwd(params: ParamPack, x: torch.Tensor, h_final: torch.Tensor, rows: torch.Tensor, num_rows: torch.Tensor, alloc=None):
     """``ddfa_node_head_fwd``: logits (fp32 [N] capacity; the first S are valid) and the hidden activations
     ([L-1, N, 2D] capacity, or None for one layer) of the MLP head over the listed rows of ``[h_final | x]``."""

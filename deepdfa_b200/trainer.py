@@ -144,9 +144,12 @@ def stage(slot, g, stream) -> int:
     i = slot["next"]
     slot["next"] = 1 - i
     st = slot["sets"][i]
+    caller = torch.cuda.current_stream()
     with torch.cuda.stream(stream):
         if st["free"] is not None:
             stream.wait_event(st["free"])           # the graph that last read this set has finished
+        else:
+            stream.wait_stream(caller)              # first use: the set's zero fill, enqueued on the caller's stream, is done
         src, dst = g.edges()
         N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
         st["src"][:Eg].copy_(src, non_blocking=True)
@@ -529,7 +532,11 @@ class FusedTrainer:
         the device inside the step (``ddfa_node_sample``: Philox keys from ``node_sample_seed`` and the draw counter
         ``node_sample_draws``).  The head runs over that row list only.  A draw that asks for more non-vulnerable nodes than the
         batch has takes them all and raises ``ValueError`` at the next step or at ``check_inputs()`` (``random.sample`` raises
-        on the module path).  One rank only.
+        on the module path).  Several ranks (an NCCL group): R ranks over the shards of a global batch do what one rank does over
+        the shards concatenated in rank order — the same rows, drawn over the global batch (``engine.NodeDrawDP``: 1 or 6 small
+        NCCL collectives on a side stream under the GGNN forward), each rank keeping its own, and the mean over the rows of all
+        ranks.  ``global_batch`` is ignored; ``node_sample_seed`` must be the same on every rank (``ValueError``);
+        :meth:`last_node_offset` and :meth:`last_num_rows_global` map the rows to the global batch.  Other backends: one rank.
 
         Frozen parameters: a parameter with ``requires_grad=False`` when the trainer is built is not trained — Adam runs over the
         trainable elements only (``ddfa_adam_flat_ranges``), its gradient slot is zeroed before the norm, and it gets no optimizer
@@ -625,9 +632,10 @@ class FusedTrainer:
                                    or torch.cuda.device_count() < self.world):
                 exchange, self.exchange_note = "nccl", "auto: ranks span more than this node (or a non-NCCL group): NCCL all-reduce"
         self.exchange = exchange if self.world > 1 else "nccl"
-        if self._node and self.world > 1:
-            # the global mean divides by the S of all ranks: their row counts would have to be exchanged before the gradient scale
-            raise NotImplementedError("FusedTrainer: label_style='node' trains on one rank (distributed=False or a one-rank group)")
+        if self._node and self.world > 1 and dist.get_backend(process_group) != "nccl":
+            # several ranks draw the loss rows of the global batch through NCCL collectives captured in the step graph
+            raise NotImplementedError("FusedTrainer: label_style='node' over several ranks needs an NCCL process group; with this "
+                                      "backend it trains on one rank (distributed=False or a one-rank group)")
         self.use_cuda_graph = use_cuda_graph
         # a captured graph bakes in the batch SHAPE (and, for resident batches, the batch object): cap how many are kept so a
         # stream of ever-new shapes (un-bucketed real data) degrades to eager launches instead of growing without bound
@@ -712,6 +720,8 @@ class FusedTrainer:
             self._status_host = torch.zeros(1, dtype=torch.int32).pin_memory()
             self._status_pending = None
             self._last_rows = None
+            if self.world > 1:
+                self._node_dp_setup(process_group)
         self.params = E.ParamPack.from_flat_list(pviews, K, nl)
         self.grads = E.ParamPack.from_flat_list(gviews, K, nl)
         self.loss_slot = self.flat_g[total:total + 1]          # this rank's share of the loss goes here (the kernels' loss_out)
@@ -869,11 +879,42 @@ class FusedTrainer:
         self._draw.fill_(v)
 
     def last_loss_rows(self) -> torch.Tensor:
-        """int32 device tensor: the nodes the last step's loss was taken over, ascending (reads S: one synchronisation)."""
+        """int32 device tensor: the nodes the last step's loss was taken over, ascending (reads S: one synchronisation).  With
+        several ranks: the rows of this rank's shard, in local node ids (add :meth:`last_node_offset` for global ids)."""
         self._require_node("last_loss_rows")
         if self._last_rows is None:
             return torch.zeros(0, dtype=torch.int32, device=self.device)
         return self._last_rows[:int(self._num_rows.item())].clone()
+
+    def last_node_offset(self) -> int:
+        """The first node of this rank's shard in the last step's global batch (the shards concatenated in rank order): the
+        number of valid nodes on the ranks before it.  0 on one rank.  Reads a device word: one synchronisation."""
+        self._require_node("last_node_offset")
+        return int(self._node_off.item()) if self.world > 1 else 0
+
+    def last_num_rows_global(self) -> int:
+        """S of the last step over the global batch, the divisor of its mean loss: the loss rows of all ranks.  On one rank
+        ``last_loss_rows().numel()``.  Reads a device word: one synchronisation."""
+        self._require_node("last_num_rows_global")
+        return int((self._s_global if self.world > 1 else self._num_rows).item())
+
+    def _node_dp_setup(self, process_group):
+        """Several ranks, node style: every rank must draw with the same seed (checked here, collectively: every rank raises
+        alike); the device words of the global row count and the shard's node offset; the side stream the draw runs on."""
+        seed = self.node_sample_seed
+        lo, hi = seed & 0xFFFFFFFF, seed >> 32
+        t = torch.tensor([lo, hi, -lo, -hi], dtype=torch.int64, device=self.device)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX, group=process_group)     # max == own on every word: the same seed on every rank
+        if t.tolist() != [lo, hi, -lo, -hi]:
+            raise ValueError(f"node_sample_seed differs between the ranks (this rank: {seed}); every rank draws the loss rows of the "
+                             "global batch with the same Philox keys")
+        self._s_global = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._node_off = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._sample_stream = torch.cuda.Stream(device=self.device)
+        self._node_rank = dist.get_rank(process_group)
+
+    def _sum_ints(self, t: torch.Tensor) -> None:
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.pg)
 
     def _node_step_done(self, rows):
         """After a node-style step: remembers its row list and sends the sampler's status word to the host behind it."""
@@ -970,6 +1011,8 @@ class FusedTrainer:
     def _global_batch(self, global_batch: Optional[int], local_graphs: int) -> int:
         """The divisor of the mean BCE (base_module.py:74,183).  Ranks generally hold different numbers of graphs
         (batched_graph.split_batch balances by nodes), so with more than one rank the caller must say what the global batch is."""
+        if self._node:            # node style: the loss is a mean over rows, whose global count the step exchanges itself
+            return int(local_graphs)
         if global_batch is not None:
             return int(global_batch)
         if self.world > 1:
@@ -1051,25 +1094,55 @@ class FusedTrainer:
             L.call(name, *args, stream)
 
     def _enqueue_node(self, dg, idx, vuln, eng, pw, valid_nodes, phase):
-        """label_style="node" (one rank): GGNN forward without the readout, the loss rows drawn on the device, the head and
-        the BCE over them, the head backward into dh_T / dx, the GGNN backward from there, the update (or, inside an
-        accumulation window, the gradient into the window's sum)."""
+        """label_style="node": GGNN forward without the readout, the loss rows drawn on the device, the head and the BCE over
+        them, the head backward into dh_T / dx, the GGNN backward from there, the update (or, inside an accumulation window, the
+        gradient into the window's sum).  Several ranks: the rows are those of the global batch's draw that fall in this shard
+        (``engine.NodeDrawDP``), drawn with their collectives on a side stream under the GGNN forward, and the BCE divides by
+        the global row count."""
         m, ws = self.module, self.ws
         N = dg.num_nodes
+        factor = m.hparams.undersample_node_on_loss_factor
         if vuln.dtype != torch.int32:
             vuln = vuln.to(torch.int32)
+        if self.world > 1:
+            return self._enqueue_node_dp(dg, idx, vuln, eng, pw, valid_nodes, phase)
         x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False,
                                   grad_ggnn=self._grad_ggnn)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
             valid_nodes.fill_(N)
         rows = ws.get("node_rows", (N,), torch.int32)
-        E.node_sample(vuln, valid_nodes, m.hparams.undersample_node_on_loss_factor, self.node_sample_seed, self._draw, rows,
-                      self._num_rows, self._sample_status, alloc=ws)
+        E.node_sample(vuln, valid_nodes, factor, self.node_sample_seed, self._draw, rows, self._num_rows, self._sample_status, alloc=ws)
         logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
         self._last_logits = logits
         dlogits = E.node_bce(logits, vuln, rows, self._num_rows, pw, self.loss_slot, alloc=ws,
                              grad_scale=None if self._k == 1 else 1.0 / self._k)
+        return self._node_backward(dg, saved, eng, dlogits, x, h_T, rows, act, phase)
+
+    def _enqueue_node_dp(self, dg, idx, vuln, eng, pw, valid_nodes, phase):
+        m, ws = self.module, self.ws
+        N = dg.num_nodes
+        if valid_nodes is None:
+            valid_nodes = ws.get("node_valid", (1,), torch.int32)
+            valid_nodes.fill_(N)
+        rows = ws.get("node_rows", (N,), torch.int32)
+        draw = E.NodeDrawDP(vuln, valid_nodes, m.hparams.undersample_node_on_loss_factor, self.node_sample_seed, self._draw, rows,
+                            self._num_rows, self._sample_status, self._s_global, self._node_off, self._node_rank, self.world, alloc=ws)
+        main = torch.cuda.current_stream()
+        self._sample_stream.wait_stream(main)
+        with torch.cuda.stream(self._sample_stream):      # it needs _VULN and the valid count only: under the GGNN forward
+            draw.run(self._sum_ints)
+        x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False,
+                                  grad_ggnn=self._grad_ggnn)
+        main.wait_stream(self._sample_stream)
+        logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
+        self._last_logits = logits
+        dlogits = E.node_bce_global(logits, vuln, rows, self._num_rows, self._s_global, pw,
+                                    self._loss_local if self.exchange == "p2p" else self.loss_slot, grad_scale=1.0 / self._k, alloc=ws)
+        return self._node_backward(dg, saved, eng, dlogits, x, h_T, rows, act, phase)
+
+    def _node_backward(self, dg, saved, eng, dlogits, x, h_T, rows, act, phase):
+        ws = self.ws
         dh, dx = E.node_head_bwd(self.params, self.grads, dlogits, x, h_T, rows, self._num_rows, act, alloc=ws,
                                  input_grads=self._grad_ggnn)
         if self._grad_ggnn:
@@ -1264,28 +1337,40 @@ class FusedTrainer:
     # ------------------------------------------------------------------------------------
     @staticmethod
     def dp_self_check(engine: str, device, rank: int, world: int, steps: int = 5, graphs_per_rank: int = 24, nodes: int = 60,
-                      exchange: str = "auto") -> dict:
+                      exchange: str = "auto", label_style: str = "graph", factor: Optional[float] = None) -> dict:
         """On-hardware data-parallel parity (SURVEY.md §8(e) "Determinism"): ``steps`` optimisation steps of a global batch
         sharded over the ``world`` ranks (node-balanced shards of different sizes, NCCL all-reduce) against the same steps of
         the UNSHARDED batch on this rank alone, same seeds.  fp32 summation order is the only difference.  Collective: every
-        rank must call it.  Returns the loss curves and the largest parameter difference after the last step."""
+        rank must call it.  Returns the loss curves and the largest parameter difference after the last step.
+        ``label_style="node"`` (``factor``: ``undersample_node_on_loss_factor``) also checks that every step's loss rows of
+        this rank, mapped to the global batch, are the unsharded run's rows inside this shard (``rows_identical``)."""
         from . import synth
         from .batched_graph import split_batch
         feat = "_ABS_DATAFLOW_api_all_limitall_1000_limitsubkeys_1000"
+        node = label_style == "node"
+        style = dict(label_style="node", undersample_node_on_loss_factor=factor) if node else {}
 
         def make(distributed):
             torch.manual_seed(4321)
-            m = FlowGNNGGNNModule(feat, 1002, 32, 8, 2, concat_all_absdf=True, positive_weight=4.0, engine=engine).to(device)
+            m = FlowGNNGGNNModule(feat, 1002, 32, 8, 2, concat_all_absdf=True, positive_weight=4.0, engine=engine, **style).to(device)
             return m, FusedTrainer(m, distributed=distributed, exchange=exchange if distributed else "nccl")
         m_dp, tr_dp = make(True)
         m_1, tr_1 = make(False)
-        l_dp, l_1 = [], []
+        l_dp, l_1, rows_ok = [], [], True
         for i in range(steps):
             b = synth.make_batch(graphs_per_rank * world, nodes, seed=900 + i, variable=True, vuln_rate=0.3)
             shard = split_batch(b, world)[rank]
             l_dp.append(float(tr_dp.step(shard.to(device), global_batch=b.batch_size)))
             l_1.append(float(tr_1.step(b.to(device), global_batch=b.batch_size)))
+            if node:
+                off, n = tr_dp.last_node_offset(), shard.num_nodes()
+                r1 = tr_1.last_loss_rows().long()
+                mine = r1[(r1 >= off) & (r1 < off + n)] - off
+                rows_ok = rows_ok and torch.equal(tr_dp.last_loss_rows().long(), mine)
         dparam = max(float((p.data - q.data).abs().max()) for p, q in zip(m_dp.param_list(), m_1.param_list()))
-        return {"steps": steps, "world": world, "global_batch": graphs_per_rank * world, "loss_sharded": l_dp, "loss_single_rank": l_1,
-                "max_abs_loss_diff": max(abs(a - b) for a, b in zip(l_dp, l_1)), "max_abs_param_diff": dparam,
-                "shard_sizes_differ": True, "exchange": exchange}
+        out = {"steps": steps, "world": world, "global_batch": graphs_per_rank * world, "loss_sharded": l_dp, "loss_single_rank": l_1,
+               "max_abs_loss_diff": max(abs(a - b) for a, b in zip(l_dp, l_1)), "max_abs_param_diff": dparam,
+               "shard_sizes_differ": True, "exchange": exchange}
+        if node:
+            out.update(label_style="node", factor=factor, rows_identical=bool(rows_ok))
+        return out

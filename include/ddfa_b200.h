@@ -405,6 +405,51 @@ int ddfa_node_bce(const float *logits, const int32_t *vuln, const int32_t *rows,
  * micro-batches passes 1 / k).  loss_out is the unscaled mean; grad_scale = 1 gives results bit-identical to ddfa_node_bce. */
 int ddfa_node_bce_scaled(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows,
                          int32_t num_nodes, float pos_weight, float grad_scale, float *loss_out, float *dlogits, void *stream);
+
+/* Several ranks (data parallel): the draw ddfa_node_sample makes over the GLOBAL batch — the ranks' shards concatenated in rank
+ * order — taken in phases, each rank keeping the rows that fall in its shard (local node ids).  Every phase reads and writes
+ * device words only (capturable); between phases the caller runs an in-place int32 SUM all-reduce over the ranks of one region
+ * of the rank's exchange buffer (ddfa_node_dp_exchange_words(world) int32 words):
+ *   words [0, 256)                histogram of the current radix digit
+ *   words [256, 256 + 2 world)    [n_vuln, n_nonvuln] of every rank (rank q writes its pair at 256 + 2q, the others are 0)
+ *   words [256 + 2 world, + world) the ties at the threshold key of every rank (rank q writes word q)
+ * Sequence (workspace: ddfa_node_sample_workspace_bytes(N), the same for every phase; num_valid as for ddfa_node_sample):
+ *   ddfa_node_dp_count     clears the workspace's control words and the exchange buffer, counts this rank's valid vulnerable and
+ *                          non-vulnerable nodes; factor < 0 also writes the local rows (every valid node) and *num_rows.
+ *                          -> SUM the counts region.
+ *   ddfa_node_dp_plan      global counts, *node_offset = sum over q < rank of rank q's valid nodes, *num_rows_global = S of the
+ *                          global batch (n_vuln + k, or every valid node for factor < 0); factor >= 0: k, *status and *draw as
+ *                          ddfa_node_sample computes them from the global counts (every rank advances its draw word alike).
+ *                          factor < 0 ends here.
+ *   4 x (ddfa_node_dp_radix_hist(pass) -> SUM the histogram region -> ddfa_node_dp_radix_pick(pass)): local histogram of the
+ *                          keys' digit `pass`, bin pick on the global one.  Node n's key is that of node *node_offset + n of the
+ *                          global batch: the keys one rank over the concatenated batch gives it.
+ *   ddfa_node_dp_ties      per-CTA counts; this rank's ties at the threshold key into its tie word.  -> SUM the ties region.
+ *   ddfa_node_dp_rows      the ties of ranks q < rank are taken first (global node order); compacts the local rows, *num_rows.
+ * Integer counts only: the union over the ranks of node_offset + rows is ddfa_node_sample's row list of the global batch, bit
+ * for bit, with the same status and draw.  One rank (world = 1, no exchange) is ddfa_node_sample itself.
+ * ddfa_node_bce_global: ddfa_node_bce_scaled over this rank's S rows with the global row count *num_rows_global as the divisor:
+ *   loss_out[0] = sum over the local rows of bce / S_global (this rank's share of the global mean; the shares of all ranks sum
+ *   to it) and dlogits[s] = (1.f / S_global) * grad_scale * d bce (bit-identical to the one-rank rows' for the same S). */
+size_t ddfa_node_dp_exchange_words(int32_t world);
+int ddfa_node_dp_count(const int32_t *vuln, const int32_t *num_valid, int32_t num_nodes, double factor, int32_t rank,
+                       int32_t world, int32_t *rows, int32_t *num_rows, void *workspace, size_t workspace_bytes,
+                       int32_t *exchange, void *stream);
+int ddfa_node_dp_plan(int32_t num_nodes, double factor, int32_t rank, int32_t world, int64_t *draw, int32_t *status,
+                      int32_t *num_rows_global, int32_t *node_offset, void *workspace, size_t workspace_bytes,
+                      const int32_t *exchange, void *stream);
+int ddfa_node_dp_radix_hist(const int32_t *vuln, const int32_t *num_valid, int32_t num_nodes, uint64_t seed, int32_t pass,
+                            void *workspace, size_t workspace_bytes, int32_t *exchange, void *stream);
+int ddfa_node_dp_radix_pick(int32_t num_nodes, int32_t pass, void *workspace, size_t workspace_bytes, int32_t *exchange,
+                            void *stream);
+int ddfa_node_dp_ties(const int32_t *vuln, const int32_t *num_valid, int32_t num_nodes, uint64_t seed, int32_t rank,
+                      int32_t world, void *workspace, size_t workspace_bytes, int32_t *exchange, void *stream);
+int ddfa_node_dp_rows(const int32_t *vuln, const int32_t *num_valid, int32_t num_nodes, uint64_t seed, int32_t rank,
+                      int32_t world, int32_t *rows, int32_t *num_rows, void *workspace, size_t workspace_bytes,
+                      const int32_t *exchange, void *stream);
+int ddfa_node_bce_global(const float *logits, const int32_t *vuln, const int32_t *rows, const int32_t *num_rows,
+                         const int32_t *num_rows_global, int32_t num_nodes, float pos_weight, float grad_scale,
+                         float *loss_out, float *dlogits, void *stream);
 size_t ddfa_node_head_bwd_workspace_bytes(int32_t num_nodes, int32_t dim);
 int ddfa_node_head_bwd(const float *dlogits, const float *h_final, const float *x, const int32_t *rows,
                        const int32_t *num_rows, int32_t num_nodes, int32_t dim, const float *const *mlp_w,
