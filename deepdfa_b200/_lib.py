@@ -118,6 +118,12 @@ _SIGNATURES = {
     "ddfa_eval_metrics_workspace_bytes": (_sz, []),
     "ddfa_eval_metrics_graph": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, C.c_double, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
     "ddfa_eval_metrics_rows": (_int, [_vp, _vp, _vp, _vp, _i32, _f32, C.c_double, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
+    "ddfa_stmt_metric_workspace_bytes": (_sz, []),
+    "ddfa_stmt_metric": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _sz, _vp]),
+    "ddfa_stmt_attention": (_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp]),
+    "ddfa_stmt_input_grad_score": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _vp, _vp]),
+    "ddfa_stmt_scale_input": (_int, [_vp, _f32, _i32, _i32, _vp, _vp, _vp]),
+    "ddfa_stmt_node_probability": (_int, [_vp, _vp, _i32, _vp, _vp]),
     "ddfa_grad_accumulate": (_int, [_vp, _vp, _i64, _i64, _i32, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
 }
@@ -129,8 +135,12 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
               "ddfa_build_csr_workspace_bytes", "ddfa_arena_batch_workspace_bytes", "ddfa_gru_step_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes_steps",
               "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes",
               "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
-              "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes"}
+              "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes",
+              "ddfa_stmt_metric_workspace_bytes"}
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
+STMT_STATE_WORDS = 16         # DDFA_STMT_STATE_WORDS: fp64 words of the statement metric state
+STMT_MODE_VULN_ONLY, STMT_MODE_FULL = 0, 1    # DDFA_STMT_MODE_*: modes of ddfa_stmt_metric
+STMT_SCORE_ABS, STMT_SCORE_X_TIMES = 0, 1     # DDFA_STMT_SCORE_*: rules of ddfa_stmt_input_grad_score
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
 GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate
 ADAM_GROUP_WORDS = 8          # DDFA_ADAM_GROUP_WORDS: fp32 words per row of the parameter-group table

@@ -286,13 +286,18 @@ def node_indices(g: BatchedCFG, concat_all_absdf: bool, feature_key: str, device
 # ------------------------------------------------------------------------------------------
 def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps: int, *, training: bool,
             engine: int = ENGINE_SIMT, alloc=None, oob_counter: Optional[torch.Tensor] = None, head: bool = True,
-            grad_ggnn: bool = True):
+            grad_ggnn: bool = True, x_in: Optional[torch.Tensor] = None, x_scale: float = 1.0,
+            attention: Optional[torch.Tensor] = None):
     """Returns (pooled [B,2D], logits [B] or None, Saved or None).  ``head=False`` stops before the readout and returns
     (x [N,D], h_T [N,D], Saved or None) instead: the label_style="node" trainer runs its own head over a row list
     (``node_head_fwd``); Saved then holds no readout state.
     ``training=True, grad_ggnn=False`` (frozen embedding tables and GGNN): the GGNN runs in its inference form — no per-step
     h / s images or gates are kept — and Saved holds only x, h_T and the readout state, enough for
-    ``backward(..., grad_ggnn=False)``."""
+    ``backward(..., grad_ggnn=False)``.
+    ``x_in`` ([N, D] fp32, e.g. the embedding output ``alloc`` holds as "x" after an earlier forward): the pass starts from
+    ``x_scale * x_in`` instead of the embedding lookup — h_0 and the readout's concat half both see the scaled rows, which are
+    written to the buffer "x_scaled" (and, for the tcgen05 engine, to h_0's activation image) by ``ddfa_stmt_scale_input``.
+    ``attention`` ([N] fp32): receives the readout's per-node softmax gate α_n (``ddfa_stmt_attention``)."""
     _require_cuda(*params.flat_list(), dg.indptr, *idx)
     L = _lib.lib()
     _lib.apply_deterministic_mode()
@@ -307,11 +312,20 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
 
     use_images = engine == ENGINE_TCGEN05     # activations travel as MMA-ready bf16 hi/lo images (include/ddfa_b200.h)
     ggnn_train = training and grad_ggnn       # keep the per-step state the GGNN backward reads
-    x = alloc.get("x", (N, D))
+    if x_in is not None and tuple(x_in.shape) != (N, D):
+        raise DdfaError(f"forward: x_in of shape {tuple(x_in.shape)}, need ({N}, {D})")
+    x = alloc.get("x" if x_in is None else "x_scaled", (N, D))
     h_imgs = None
-    if use_images and OPTIONS["packed_state"]:
+    img_bytes = L.call("ddfa_act_image_bytes", N) if use_images else 0
+    if x_in is not None:
+        img = None
+        if use_images and OPTIONS["packed_state"]:
+            n_img = T if ggnn_train else 2
+            h_imgs = [alloc.get_image(f"h_img{i}", img_bytes) for i in range(max(n_img, 1))]
+            img = h_imgs[0]
+        _call("ddfa_stmt_scale_input", _p(x_in), float(x_scale), N, D, _p(x), _p(img), st)
+    elif use_images and OPTIONS["packed_state"]:
         # the embedding kernel writes h_0 = x as fp32 rows AND as its activation image (one pass instead of embed + ddfa_act_to_image)
-        img_bytes = L.call("ddfa_act_image_bytes", N)
         n_img = T if ggnn_train else 2        # training keeps the image of every h_t (the weight-gradient GEMM reads it)
         h_imgs = [alloc.get_image(f"h_img{i}", img_bytes, tail_unwritten=i == 0) for i in range(max(n_img, 1))]
         _call("ddfa_embed_concat_fwd_image", ptr_array([_p(t) for t in idx]), ptr_array([_p(t) for t in params.tables]),
@@ -386,6 +400,8 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     if training and not grad_ggnn:
         hs, ss, gs, h_imgs = [x] + [None] * (T - 1) + [h_cur], [], [], None     # h[T] = h_T for the readout backward
     if not head:
+        if attention is not None:
+            raise DdfaError("forward: attention needs the readout (head=True)")
         saved = None
         if training:
             saved = Saved(T, D, x, hs, ss, gs, w_fold, b_fold, None, None, None, None, None, idx,
@@ -393,14 +409,17 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
         return x, h_cur, saved
     pooled = alloc.get("pooled", (B, 2 * D))
     logits = alloc.get("logits", (B,)) if nl > 0 else None
-    gate_logit = alloc.get("gate_logit", (N,)) if training else None
-    seg_max = alloc.get("seg_max", (B,)) if training else None
-    seg_sum = alloc.get("seg_sum", (B,)) if training else None
+    keep_gate = training or attention is not None
+    gate_logit = alloc.get("gate_logit", (N,)) if keep_gate else None
+    seg_max = alloc.get("seg_max", (B,)) if keep_gate else None
+    seg_sum = alloc.get("seg_sum", (B,)) if keep_gate else None
     mlp_act = alloc.get("mlp_act", (max(nl - 1, 1), B, 2 * D)) if (training and nl > 1) else None
     _call("ddfa_readout_mlp_fwd", _p(h_cur), _p(x), _p(dg.graph_ptr), B, D, _p(params.w_gate), _p(params.b_gate),
            ptr_array([_p(t) for t in params.mlp_w]) if nl else None,
            ptr_array([_p(t) for t in params.mlp_b]) if nl else None,
            nl, _p(pooled), _p(logits), _p(gate_logit), _p(seg_max), _p(seg_sum), _p(mlp_act), st)
+    if attention is not None:
+        _call("ddfa_stmt_attention", _p(gate_logit), _p(seg_max), _p(seg_sum), _p(dg.graph_ptr), B, _p(attention), st)
     saved = None
     if training:
         saved = Saved(T, D, x, hs, ss, gs, w_fold, b_fold, pooled, gate_logit, seg_max, seg_sum, mlp_act, idx,
@@ -411,7 +430,7 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
 def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack, *, dlogits: Optional[torch.Tensor] = None,
              dpooled: Optional[torch.Tensor] = None, engine: int = ENGINE_SIMT, alloc=None, on_small_grads_ready=None,
              dh_final: Optional[torch.Tensor] = None, dx_direct: Optional[torch.Tensor] = None, grad_ggnn: bool = True,
-             grad_tables: bool = True):
+             grad_tables: bool = True, grad_weights: bool = True):
     """Accumulates (+=) parameter gradients into ``grads``.  Exactly one of dlogits / dpooled / (dh_final, dx_direct) is given.
     ``dh_final`` / ``dx_direct`` ([N, D] each, from ``node_head_bwd``): the gradients of h_T and of the direct use of x; the
     GGNN backward starts from them and the MLP / readout backward is skipped (their gradients are left alone).  ``dh_final``
@@ -421,7 +440,12 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     trainer can start reducing them while that launch runs.
     ``grad_ggnn=False`` (frozen embedding tables and GGNN; ``saved`` may come from ``forward(..., grad_ggnn=False)``): stops after
     the readout — the gate gradients only, no GGNN gradient, no transposed gather, no embedding backward.
-    ``grad_tables=False`` (frozen embedding tables): the full GGNN backward without the embedding backward."""
+    ``grad_tables=False`` (frozen embedding tables): the full GGNN backward without the embedding backward.
+    ``grad_weights=False`` (input attribution): the dgrad chain only, returning ``(dh_0, dx_direct)``, whose sum is the gradient
+    of the logits (or of h_T / pooled) with respect to the embedding output x.  No weight-gradient GEMM (the tcgen05 step kernels
+    still keep their operands, but ``ddfa_gru_bwd_wgrad_batched`` / ``_finish`` are not launched), no ``ddfa_fold_weights_bwd``,
+    no embedding backward.  The gradients the MLP, readout and step kernels compute inline (the SIMT step kernel's weight
+    gradient among them) still go to ``grads``, which the caller then passes as scratch."""
     L = _lib.lib()
     det = _lib.apply_deterministic_mode()
     dev = dg.device
@@ -434,6 +458,8 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     st = _stream_ptr()
     if dg.indptr_t is None and grad_ggnn:
         raise DdfaError("backward needs the transposed CSR (prepare_graph(need_transpose=True))")
+    if not grad_weights and not grad_ggnn:
+        raise DdfaError("backward: grad_weights=False needs the GGNN backward (grad_ggnn=True)")
 
     if dh_final is not None or dx_direct is not None:
         if dh_final is None or dx_direct is None or dlogits is not None or dpooled is not None:
@@ -506,6 +532,8 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
         dh, dh_alt = dh_alt, dh
     if engine == ENGINE_TCGEN05 and T > 0 and fuse_gather:     # the gather of the last ds (step 0) has no following step to ride on
         _call("ddfa_gather_sum", _p(dg.indptr_t), _p(dg.indices_t), _p(ds_prev), N, D, _p(dh), 1, st, tag="gather_bwd")
+    if not grad_weights:
+        return dh, dx_direct
     # the deterministic form's scratch (sort keys and partial sums): allocated only in that mode, the default form does not read it
     if grad_tables:
         emb_bytes = L.call("ddfa_embed_concat_bwd_workspace_bytes", K, V, H, N) if det else 0

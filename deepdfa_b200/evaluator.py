@@ -11,6 +11,11 @@ The batch paths are those of :class:`~deepdfa_b200.trainer.FusedTrainer` and sha
 per-shape buffers (two sets, ``prefetch``) with optional shape bucketing, resident device batches (one captured graph per
 object), graph ids of a :class:`~deepdfa_b200.arena.GraphArena` assembled inside the captured graph, and eager launches beyond
 ``max_graph_shapes``.
+
+Statement-level localisation (``statements=``): per batch, a score per node (CFG node = statement) and IVDetect's top-k statement
+metric over them (DDFA/sastvd/helpers/evaluate.py:262-322), added by ``ddfa_stmt_metric`` to a second fp64 state.  The scores are
+the node head's probability (node style), or, for the function logit of graph style, the readout's attention α_n, the saliency
+Σ_d |∂logit/∂x_{n,d}| or the integrated gradients Σ_d x_{n,d} · mean_k ∂logit/∂x_{n,d}(α_k x) of the embedding output x.
 """
 from __future__ import annotations
 
@@ -26,6 +31,11 @@ from .module import FlowGNNGGNNModule, _ENGINES
 
 # the fp64 words of the metric state (include/ddfa_b200.h, DDFA_EVAL_STATE_WORDS)
 TP, FP, TN, FN, SAMPLES, BATCHES, LOSS_W, WEIGHT, STORED, OVERFLOW = range(10)
+# the fp64 words of the statement metric state (DDFA_STMT_STATE_WORDS): hits at k = 1..10 are words S_HIT1 + k - 1
+S_FUNCTIONS, S_VULN, S_HIT1, S_RANK_SUM, S_CLEAN, S_NAN, S_BATCHES = 0, 1, 2, 12, 13, 14, 15
+STMT_TOP_K = 10
+# statements= -> the label style it scores
+STATEMENT_MODES = {"probability": "node", "attention": "graph", "saliency": "graph", "integrated_gradients": "graph"}
 
 
 def _ratio(num: float, den: float) -> float:
@@ -51,15 +61,48 @@ def metrics_from_state(state, prefix: str = "val_") -> dict:
             f"{prefix}num_samples": int(n)}
 
 
+def _share(num: float, den: float) -> float:
+    return num / den if den > 0 else float("nan")
+
+
+def statement_metrics_from_state(state, prefix: str = "val_", node_style: bool = False) -> dict:
+    """The statement metrics of a statement state (any float64 tensor or sequence of ``STMT_STATE_WORDS`` values, e.g. a sum over
+    ranks), with the keys of evaluate.py:262-322: ``{prefix}stmt_top{k}`` (k = 1..10, ``eval_statements_list(..., vo=True)``: the
+    share of vulnerable functions whose first vulnerable statement ranks among the first k), ``{prefix}stmt_ifa`` (the mean number
+    of statements ranked above it, the initial false alarms), ``{prefix}stmt_vuln_functions`` and ``{prefix}stmt_functions``.
+    ``node_style`` (scores are probabilities) adds ``{prefix}stmt_nonvuln_clean`` (the share of non-vulnerable functions with no
+    probability > 0.5) and ``{prefix}stmt_all_top{k}`` (its product with top-k, ``vo=False``).  Unlike :func:`metrics_from_state`
+    (0 wherever a denominator is 0), a share over no function is NaN: the reference divides by zero there."""
+    s = [float(v) for v in (state.tolist() if torch.is_tensor(state) else state)]
+    nv = s[S_VULN]
+    out = {f"{prefix}stmt_top{k}": _share(s[S_HIT1 + k - 1], nv) for k in range(1, STMT_TOP_K + 1)}
+    out[f"{prefix}stmt_ifa"] = _share(s[S_RANK_SUM], nv)
+    out[f"{prefix}stmt_vuln_functions"] = int(nv)
+    out[f"{prefix}stmt_functions"] = int(s[S_FUNCTIONS])
+    if node_style:
+        clean = _share(s[S_CLEAN], s[S_FUNCTIONS] - nv - s[S_NAN])
+        out[f"{prefix}stmt_nonvuln_clean"] = clean
+        out.update({f"{prefix}stmt_all_top{k}": out[f"{prefix}stmt_top{k}"] * clean for k in range(1, STMT_TOP_K + 1)})
+    return out
+
+
 class FusedEvaluator:
     def __init__(self, model: FlowGNNGGNNModule, use_cuda_graph: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
-                 max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64):
+                 max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64,
+                 statements: Optional[str] = None, ig_steps: int = 50):
         """``max_predictions`` > 0 keeps the first that many probabilities and labels (``predictions()``; the reference's
         ``test_preds`` / ``test_labels``); more samples than that make :meth:`compute` raise, the counts stay complete.
         ``bucket_nodes`` / ``bucket_edges``: shape bucketing of host batches under ``use_cuda_graph``, as in ``FusedTrainer``
         (one padding graph, excluded from every metric).  The evaluator reads the module's parameters where they live when a
         batch runs and never writes them; graphs captured over other parameter storage (a ``FusedTrainer`` built later moves
-        the parameters into its flat buffer) are recaptured."""
+        the parameters into its flat buffer) are recaptured.
+        ``statements``: the per-statement score of :meth:`last_scores` and of the statement metrics (``STATEMENT_MODES``):
+        ``"probability"`` (node style: the node head's sigmoid), ``"attention"`` (graph style: the readout's softmax gate α_n,
+        summing to 1 over each function), ``"saliency"`` (graph style: Σ_d |∂logit/∂x_{n,d}| of the embedding output x, captum's
+        ``Saliency(abs=True)``) or ``"integrated_gradients"`` (graph style: Σ_d x_{n,d} · (1/m) Σ_{k<m} ∂logit/∂x_{n,d} at
+        ((k + ½)/m)·x, m = ``ig_steps``, zero baseline: captum's ``IntegratedGradients(method="riemann_middle")``).  The target is
+        each function's own logit; one backward with dlogits = 1 serves every function of the batch.  None (the default)
+        enqueues nothing beyond the classification metrics."""
         if model.device.type != "cuda":
             raise _lib.DdfaError("FusedEvaluator needs the module on a CUDA device (no CPU fallback)")
         hp = model.hparams
@@ -69,6 +112,16 @@ class FusedEvaluator:
             raise ValueError(f"FusedEvaluator: label_style={hp.label_style!r} is not supported ('graph' or 'node')")
         if int(max_predictions) < 0:
             raise ValueError(f"max_predictions must be >= 0, got {max_predictions!r}")
+        if statements is not None:
+            if statements not in STATEMENT_MODES:
+                raise ValueError(f"FusedEvaluator: statements={statements!r} is not one of {sorted(STATEMENT_MODES)} or None")
+            if STATEMENT_MODES[statements] != hp.label_style:
+                raise ValueError(f"FusedEvaluator: statements={statements!r} scores label_style={STATEMENT_MODES[statements]!r} "
+                                 f"modules, this one has label_style={hp.label_style!r}")
+        if int(ig_steps) < 1:
+            raise ValueError(f"ig_steps must be >= 1, got {ig_steps!r}")
+        self.statements = statements
+        self.ig_steps = int(ig_steps)
         self.module = model
         self.device = model.device
         self._node = hp.label_style == "node"
@@ -87,6 +140,12 @@ class FusedEvaluator:
             self._labels = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
             self._oob = torch.zeros(1, dtype=torch.int32, device=dev)        # out-of-range embedding indices (compute() raises)
             self._num_rows = torch.zeros(1, dtype=torch.int32, device=dev) if self._node else None
+            self._stmt_state = torch.zeros(_lib.STMT_STATE_WORDS, dtype=torch.float64, device=dev)
+            self._stmt_ws = torch.empty(L.call("ddfa_stmt_metric_workspace_bytes"), dtype=torch.uint8, device=dev) if statements else None
+            # the gradients the dgrad chain computes inline (MLP, gate, GRU biases / w_hh) land here, never in the module's .grad
+            self._grad_scratch = E.ParamPack.from_flat_list([torch.zeros_like(p) for p in model.param_list()], len(model._tables()),
+                                                            model._num_layers) if self._attributes else None
+        self._last_scores = None
         self.ws = E.Workspace(dev)
         self._slots = {}
         self._graphs = {}
@@ -95,9 +154,14 @@ class FusedEvaluator:
         self._param_key = None
 
     # ---- the metric state ------------------------------------------------------------------------------------------------
+    @property
+    def _attributes(self) -> bool:
+        return self.statements in ("saliency", "integrated_gradients")
+
     def reset(self) -> None:
-        """Zeroes the metric state in stream order (the prediction store starts over at position 0)."""
+        """Zeroes the metric state and the statement state in stream order (the prediction store starts over at position 0)."""
         self._state.zero_()
+        self._stmt_state.zero_()
 
     def state(self) -> torch.Tensor:
         """The float64 device metric state (``EVAL_STATE_WORDS`` words, layout in include/ddfa_b200.h), a view: the evaluator
@@ -106,6 +170,22 @@ class FusedEvaluator:
         return self._state
 
     metrics_from_state = staticmethod(metrics_from_state)
+    statement_metrics_from_state = staticmethod(statement_metrics_from_state)
+
+    def statement_state(self) -> torch.Tensor:
+        """The float64 device statement state (``STMT_STATE_WORDS`` words, layout in include/ddfa_b200.h, DDFA_STMT_STATE_WORDS),
+        a view, separate from :meth:`state`.  Every word is an integer count, so ``dist.all_reduce(ev.statement_state())`` adds
+        ranks exactly and :meth:`statement_metrics_from_state` turns the sum into the global statement metrics."""
+        return self._stmt_state
+
+    def last_scores(self) -> torch.Tensor:
+        """The fp32 device scores ``[N]`` of the last batch's statements, in the batch's node order (without the padding graph's
+        nodes under bucketing).  The next :meth:`update` overwrites them: copy them per batch to keep them."""
+        if self.statements is None:
+            raise ValueError("FusedEvaluator.last_scores: built with statements=None (no per-statement score)")
+        if self._last_scores is None:
+            raise ValueError("FusedEvaluator.last_scores: no batch was evaluated yet")
+        return self._last_scores
 
     def compute(self, prefix: str = "val_") -> dict:
         """The metrics of everything evaluated since the last :meth:`reset` (one synchronisation).  Raises ``ValueError`` when
@@ -122,7 +202,14 @@ class FusedEvaluator:
         if self._probs is not None and s[OVERFLOW] > 0:
             raise ValueError(f"FusedEvaluator.compute: {n} predictions, max_predictions={self.max_predictions}: build the "
                              f"evaluator with max_predictions >= {n}")
-        return metrics_from_state(s, prefix)
+        out = metrics_from_state(s, prefix)
+        if self.statements is not None:
+            ss = self._stmt_state.cpu()
+            if ss[S_NAN] > 0:
+                raise ValueError(f"FusedEvaluator.compute: {int(ss[S_NAN])} functions had a NaN statement score "
+                                 f"(statements={self.statements!r})")
+            out.update(statement_metrics_from_state(ss, prefix, node_style=self._node))
+        return out
 
     def predictions(self):
         """``(probs, labels)``: fp32 device tensors of the first ``min(stored, max_predictions)`` samples in evaluation order
@@ -148,21 +235,24 @@ class FusedEvaluator:
         return E.ParamPack.from_flat_list(plist, len(m._tables()), m._num_layers)
 
     def _prepare(self, graph):
-        """The device graph without the transposed CSR (inference reads none), the per-node view in node style, and the
-        embedding indices."""
+        """The device graph without the transposed CSR (inference reads none; saliency and integrated gradients run the
+        backward and ask for it), the per-node view in node style, the function-level graph_ptr and the embedding indices."""
         m = self.module
         g = as_batched_cfg(graph)
-        dg = E.prepare_graph(g, self.device, need_transpose=False)
+        dg = E.prepare_graph(g, self.device, need_transpose=self._attributes)
+        fptr = dg.graph_ptr
         if self._node:
             dg = E.per_node_view(g, dg)
         idx = E.node_indices(g, m.concat_all_absdf, m.feature_keys["feature"], self.device)
-        return g, dg, idx
+        return g, dg, idx, fptr
 
-    def _enqueue(self, params, dg, idx, vuln, num_graphs: int, num_valid: Optional[int] = None,
+    def _enqueue(self, params, dg, idx, vuln, fptr, num_graphs: int, num_valid: Optional[int] = None,
                  valid_nodes: Optional[torch.Tensor] = None):
-        """Enqueues one batch: the inference forward and the metric kernel.  ``num_graphs``: the batch's graph count (its
-        weight in the loss mean); ``num_valid``: graphs [num_valid, B) are bucket padding; ``valid_nodes``: the int32 device
-        word of the valid node count in node style under bucketing."""
+        """Enqueues one batch: the inference forward and the metric kernel, then, with ``statements``, the per-node scores and
+        the statement metric.  ``num_graphs``: the batch's graph count (its weight in the loss mean); ``num_valid``: graphs
+        [num_valid, B) are bucket padding; ``valid_nodes``: the int32 device word of the valid node count in node style under
+        bucketing; ``fptr``: the function-level graph_ptr.  Returns (node-style rows, scores): the scores are a fresh [N] tensor,
+        which a captured graph keeps writing on every replay."""
         m, ws = self.module, self.ws
         eng = _ENGINES[m.engine]
         pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
@@ -171,13 +261,19 @@ class FusedEvaluator:
         store = (E._p(self._probs), E._p(self._labels), self.max_predictions)
         mws = (self._metric_ws.data_ptr(), self._metric_ws.numel(), E._stream_ptr())
         L = _lib.lib()
+        N = dg.num_nodes
+        scores = torch.empty(N, dtype=torch.float32, device=self.device) if self.statements else None
         if not self._node:
-            _, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, oob_counter=self._oob)
+            att = scores if self.statements == "attention" else None
+            _, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, oob_counter=self._oob,
+                                     attention=att)
             B = dg.batch_size
             L.call("ddfa_eval_metrics_graph", E._p(logits), E._p(vuln), E._p(dg.graph_ptr), B, B if num_valid is None else int(num_valid),
                    pw, float(num_graphs), self._state.data_ptr(), *store, *mws)
-            return None
-        N = dg.num_nodes
+            if self._attributes:
+                self._attribute(params, dg, idx, scores)
+            self._statement_metric(scores, vuln, fptr, num_valid)
+            return None, scores
         x, h_T, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, head=False, oob_counter=self._oob)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
@@ -187,7 +283,44 @@ class FusedEvaluator:
         logits, _ = E.node_head_fwd(params, x, h_T, rows, self._num_rows, alloc=ws)
         L.call("ddfa_eval_metrics_rows", E._p(logits), E._p(vuln), E._p(rows), self._num_rows.data_ptr(), N, pw, float(num_graphs),
                self._state.data_ptr(), *store, *mws)
-        return rows
+        if self.statements:          # rows = every valid node in order, so logits[n] is node n's
+            E._call("ddfa_stmt_node_probability", E._p(logits), self._num_rows.data_ptr(), N, E._p(scores), E._stream_ptr())
+            self._statement_metric(scores, vuln, fptr, num_valid)
+        return rows, scores
+
+    def _statement_metric(self, scores, vuln, fptr, num_valid: Optional[int]) -> None:
+        if self.statements is None:
+            return
+        B = fptr.numel() - 1
+        mode = _lib.STMT_MODE_FULL if self._node else _lib.STMT_MODE_VULN_ONLY
+        E._call("ddfa_stmt_metric", E._p(scores), E._p(vuln), E._p(fptr), B, B if num_valid is None else int(num_valid), mode, 0.5,
+                self._stmt_state.data_ptr(), self._stmt_ws.data_ptr(), self._stmt_ws.numel(), E._stream_ptr())
+
+    def _attribute(self, params, dg, idx, scores) -> None:
+        """Saliency / integrated gradients of every function's logit with respect to the embedding output x: training-form
+        forwards and dgrad-only backwards (``grad_weights=False``) with dlogits = 1, the gradients of the weights going to a
+        scratch pack.  Integrated gradients start the m forwards from α_k·x (x: the inference forward's embedding output, still
+        in the workspace) and accumulate x·g / m."""
+        m, ws = self.module, self.ws
+        eng = _ENGINES[m.engine]
+        T = m.hparams.n_steps
+        N, B = dg.num_nodes, dg.batch_size
+        ones = ws.get("stmt_dlogits", (B,))
+        ones.fill_(1.0)
+        if self.statements == "saliency":
+            _, _, saved = E.forward(params, dg, idx, T, training=True, engine=eng, alloc=ws)
+            dh, dxd = E.backward(params, dg, saved, self._grad_scratch, dlogits=ones, engine=eng, alloc=ws, grad_weights=False)
+            E._call("ddfa_stmt_input_grad_score", None, E._p(dh), E._p(dxd), N, dh.shape[1], _lib.STMT_SCORE_ABS, 1.0, 0,
+                    E._p(scores), E._stream_ptr())
+            return
+        D = len(params.tables) * params.tables[0].shape[1]
+        x0 = ws.get("x", (N, D))             # written by the inference forward of this batch; no later pass writes "x"
+        steps = self.ig_steps
+        for k in range(steps):
+            _, _, saved = E.forward(params, dg, idx, T, training=True, engine=eng, alloc=ws, x_in=x0, x_scale=(k + 0.5) / steps)
+            dh, dxd = E.backward(params, dg, saved, self._grad_scratch, dlogits=ones, engine=eng, alloc=ws, grad_weights=False)
+            E._call("ddfa_stmt_input_grad_score", E._p(x0), E._p(dh), E._p(dxd), N, D, _lib.STMT_SCORE_X_TIMES, 1.0 / steps,
+                    int(k > 0), E._p(scores), E._stream_ptr())
 
     def _slot(self, g):
         N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
@@ -247,15 +380,17 @@ class FusedEvaluator:
 
             def enqueue():
                 gs = BatchedCFG(st["src"], st["dst"], st["bnn"], dict(st["ndata"]), num_nodes=N)   # no cached device CSR
-                _, dg, idx = self._prepare(gs)
+                _, dg, idx, fptr = self._prepare(gs)
                 vuln = gs.ndata["_VULN"]
                 if vuln.dtype != torch.int32:
                     vuln = vuln.to(torch.int32)
-                st["rows"] = self._enqueue(params, dg, idx, vuln.contiguous(), B, num_valid=slot["valid"], valid_nodes=st["valid_nodes"])
+                st["rows"], st["scores"] = self._enqueue(params, dg, idx, vuln.contiguous(), fptr, B, num_valid=slot["valid"],
+                                                         valid_nodes=st["valid_nodes"])
                 st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
 
             st["graph"] = T.graph_step(self.device, st["graph"], slot["warm"], enqueue)
             slot["warm"] = True
+            self._keep_scores(st["scores"], g.num_nodes())
             ev = torch.cuda.Event()
             ev.record(main)
             st["free"] = ev
@@ -279,16 +414,17 @@ class FusedEvaluator:
 
             def enqueue():
                 g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
-                _, dg, idx = self._prepare(g)
-                slot["rows"] = self._enqueue(params, dg, idx, g.ndata["_VULN"], B)
+                _, dg, idx, fptr = self._prepare(g)
+                slot["rows"], slot["scores"] = self._enqueue(params, dg, idx, g.ndata["_VULN"], fptr, B)
                 slot["keep"] = (g, dg, idx)
 
             slot["graph"] = T.graph_step(self.device, slot["graph"], slot["warm"], enqueue)
             slot["warm"] = True
+            self._keep_scores(slot["scores"], N)
 
     def _update_eager(self, batch):
         """Device-resident batch objects (one captured graph per object when ``use_cuda_graph``), or plain eager launches."""
-        g, dg, idx = self._prepare(batch)
+        g, dg, idx, fptr = self._prepare(batch)
         vuln = g.ndata["_VULN"]
         if vuln.device != self.device or vuln.dtype != torch.int32:
             key = "vuln_dev"
@@ -309,8 +445,12 @@ class FusedEvaluator:
             out = {}
 
             def enqueue():
-                out["rows"] = self._enqueue(params, dg, idx, vuln, B)
+                out["rows"], out["scores"] = self._enqueue(params, dg, idx, vuln, fptr, B)
             cg = T.graph_step(self.device, entry[0] if entry else None, capturable and shape_key in self._warm_shapes, enqueue)
             if entry is None and cg is not None:
-                self._graphs[graph_key] = (cg, g, idx, vuln, out["rows"])     # keep the captured tensors alive
+                self._graphs[graph_key] = entry = (cg, g, idx, vuln, out["rows"], out["scores"])     # keep the captured tensors alive
             self._warm_shapes.add(shape_key)
+            self._keep_scores(entry[5] if entry is not None else out["scores"], dg.num_nodes)
+
+    def _keep_scores(self, scores, num_nodes: int) -> None:
+        self._last_scores = None if scores is None else scores[:num_nodes]

@@ -495,6 +495,49 @@ int ddfa_eval_metrics_rows(const float *logits, const int32_t *vuln, const int32
                            float *labels_out, int64_t capacity, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K9'  statement-level localisation (csrc/statements.cu): per-node scores of a batch and IVDetect's top-k statement metric
+ * over them (DDFA/sastvd/helpers/evaluate.py:262-322, eval_statements_list), accumulated on the device like K9.
+ *
+ * ddfa_stmt_metric: function b < num_valid owns nodes [graph_ptr[b], graph_ptr[b+1]) (label_style="node": the function-level
+ *   graph_ptr, not the one-node-per-graph view); functions [num_valid, num_graphs) are bucket padding and are ignored.  A function
+ *   is vulnerable when one of its nodes has vuln != 0.  Its statements are ranked by score, descending, equal scores in node order
+ *   (Python's stable sorted(..., reverse=True)); rank = the number of statements ahead of the first-ranked vulnerable one (the
+ *   vulnerable node of maximum score, lowest node id among equal scores).  top-k is hit iff rank < k.
+ *   state: DDFA_STMT_STATE_WORDS fp64 words, zero-initialised by the caller, 8-byte aligned, every word an integer count:
+ *     [0] functions  [1] vulnerable functions  [2 + k - 1] vulnerable functions with rank < k, k = 1..10  [12] sum of rank over the
+ *     vulnerable functions  [13] non-vulnerable functions without a score > threshold (DDFA_STMT_MODE_FULL only; the strict
+ *     comparison of evaluate.py:276)  [14] functions with a NaN score (counted here and in [0] only)  [15] batches
+ *   One CTA per function (grid-stride over a grid of min(num_graphs, 264) CTAs), two passes over its nodes, integer partials per
+ *   CTA added in CTA order by a second one-thread launch: the state is bit-reproducible in both DDFA_TUNE_DETERMINISTIC modes.
+ *   workspace: ddfa_stmt_metric_workspace_bytes() bytes, 8-byte aligned, scratch.  Two launches.
+ * ddfa_stmt_attention: alpha[n] = exp(gate_logit[n] - seg_max[b]) / seg_sum[b] for the nodes of every graph b < num_graphs — the
+ *   softmax gate of GlobalAttentionPooling (DGL's get_attention=True) from the three arrays ddfa_readout_mlp_fwd writes when given,
+ *   with the expression of ddfa_readout_bwd.  One launch.
+ * ddfa_stmt_input_grad_score: score[n] = weight * sum_d f(x, g)[n, d] (accumulate != 0: score[n] = fmaf(weight, sum, score[n])), with
+ *   g = dh + dx ([N, dim] each: the gradient of h_0 through the GGNN and of the direct use of x in the readout concat, which
+ *   the embedding backward would add) and f = |g| (DDFA_STMT_SCORE_ABS; x may be NULL) or x * g (DDFA_STMT_SCORE_X_TIMES).  Warp
+ *   per node, a fixed shuffle tree: bit-reproducible.  One launch.
+ * ddfa_stmt_scale_input: out = alpha * x (fp32 [N, dim], out must not alias x) and, when image != NULL (dim == 128), its
+ *   activation image as ddfa_act_to_image writes it: the start of a forward from a scaled embedding output.  One or two launches.
+ * ddfa_stmt_node_probability: scores[n] = 1.f / (1.f + expf(-logits[n])) for n < S = *num_rows (clamped to [0, num_nodes]), 0
+ *   beyond: the probabilities of ddfa_eval_metrics_rows when the rows are every valid node in order.  One launch.
+ * ------------------------------------------------------------------------------------- */
+#define DDFA_STMT_STATE_WORDS 16
+#define DDFA_STMT_MODE_VULN_ONLY 0
+#define DDFA_STMT_MODE_FULL 1
+#define DDFA_STMT_SCORE_ABS 0
+#define DDFA_STMT_SCORE_X_TIMES 1
+size_t ddfa_stmt_metric_workspace_bytes(void);
+int ddfa_stmt_metric(const float *scores, const int32_t *vuln, const int32_t *graph_ptr, int32_t num_graphs, int32_t num_valid,
+                     int32_t mode, float threshold, double *state, void *workspace, size_t workspace_bytes, void *stream);
+int ddfa_stmt_attention(const float *gate_logit, const float *seg_max, const float *seg_sum, const int32_t *graph_ptr,
+                        int32_t num_graphs, float *alpha, void *stream);
+int ddfa_stmt_input_grad_score(const float *x, const float *dh, const float *dx, int32_t num_nodes, int32_t dim, int32_t rule,
+                               float weight, int32_t accumulate, float *score, void *stream);
+int ddfa_stmt_scale_input(const float *x, float alpha, int32_t num_nodes, int32_t dim, float *out, void *image, void *stream);
+int ddfa_stmt_node_probability(const float *logits, const int32_t *num_rows, int32_t num_nodes, float *scores, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K10  torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 (DDFA/configs/
  * config_default.yaml:43-47) over one flat parameter buffer.  step_count: int32[1] device
  * counter, incremented by the kernel (graph-capture safe).
