@@ -63,6 +63,9 @@ _SIGNATURES = {
     "ddfa_gru_step_fwd": (_int, [_vp] * 8 + [_i32, _i32, _vp, _vp, _vp, _sz, _int, _vp]),
     "ddfa_act_image_bytes": (_sz, [_i64]),
     "ddfa_act_to_image": (_int, [_vp, _i32, _i32, _vp, _vp]),
+    "ddfa_gru_tc_wide_gemm_workspace_bytes": (_sz, [_int, _i32, _i32]),
+    "ddfa_gru_tc_wide_gemm": (_int, [_int, _vp, _vp, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "ddfa_gru_tc_wide_wgrad_slices": (_sz, [_i32, _i32]),
     "ddfa_gather_sum_image": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_gru_step_fwd_image": (_int, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ddfa_gather_sum_image_src": (_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
@@ -136,7 +139,7 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
               "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes",
               "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
               "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes",
-              "ddfa_stmt_metric_workspace_bytes"}
+              "ddfa_stmt_metric_workspace_bytes", "ddfa_gru_tc_wide_gemm_workspace_bytes", "ddfa_gru_tc_wide_wgrad_slices"}
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
 STMT_STATE_WORDS = 16         # DDFA_STMT_STATE_WORDS: fp64 words of the statement metric state
 STMT_MODE_VULN_ONLY, STMT_MODE_FULL = 0, 1    # DDFA_STMT_MODE_*: modes of ddfa_stmt_metric

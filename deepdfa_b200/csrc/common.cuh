@@ -122,6 +122,21 @@ int scan_counts(int32_t *a0, int32_t *a1, int32_t n, int32_t *s0, int32_t *s1, c
 // gru_tc_fwd3.cu — tensor-core engine, forward (D == 128): activation images
 size_t act_image_bytes(int64_t n);
 int act_to_image(const float *x, int32_t N, void *image, cudaStream_t stream);
+int act_to_image(const float *x, int32_t N, int32_t D, void *image, cudaStream_t stream);   // D columns, D % 64 == 0 (tc_common.cuh: image_offset_w)
+// gru_tc_wide.cu — tensor-core GEMMs of the GRU step at the wide widths (192 <= D <= 512, D % 64 == 0), SIMT data flow around them.
+// Both step workspaces start with the W' and Whh operand images (gru_tcw_weights_bytes(D), written by gru_tcw_prepare); the
+// scratch is the images of the step's GEMM operands (and, backward, the split-K slices of the weight gradient).
+bool gru_tcw_width(int32_t D);
+size_t gru_tcw_weights_bytes(int32_t D);
+size_t gru_tcw_fwd_scratch_bytes(int32_t N, int32_t D);
+size_t gru_tcw_bwd_scratch_bytes(int32_t N, int32_t D);
+int gru_tcw_prepare(const float *w_fold, const float *w_hh, int32_t D, void *weights, cudaStream_t stream);
+// gi = s W'^T, gh = h Whh^T   ([N, 3D] fp32)
+int gru_tcw_fwd_gemms(const float *s, const float *h, int32_t N, int32_t D, const void *weights, void *scratch, float *gi, float *gh,
+                      cudaStream_t stream);
+// ds = dgi W', dh += dgh Whh, dw_fold += dgi^T s, dw_hh += dgh^T h   (weight gradients: split-K slices added in slice order)
+int gru_tcw_bwd_gemms(const float *dgi, const float *dgh, const float *s, const float *h, int32_t N, int32_t D, const void *weights,
+                      void *scratch, float *ds, float *dh, float *dw_fold, float *dw_hh, cudaStream_t stream);
 // gru_tc_fwd3.cu — forward, weights resident in shared memory (wgmma)
 size_t gru_tc3_packed_bytes();
 int gru_tc3_prepare(const float *w_fold, const float *b_fold, const float *b_ih, const float *w_hh, const float *b_hh, void *packed,

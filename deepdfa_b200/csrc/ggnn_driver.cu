@@ -20,7 +20,7 @@ inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 GgnnLayout make_layout(int32_t N, int32_t D, int32_t T, int engine, int training) {
   GgnnLayout L = {};
-  const bool tc = engine == DDFA_ENGINE_TCGEN05;
+  const bool tc = engine == DDFA_ENGINE_TCGEN05 && D == 128;     // the image path; at the wide widths tcgen05 keeps SIMT's layout
   L.plane = align256((size_t)N * D * sizeof(float));
   L.img = tc ? align256(ddfa_act_image_bytes(N)) : 0;
   size_t off = 0;
@@ -66,7 +66,7 @@ extern "C" {
 
 size_t ddfa_ggnn_workspace_bytes(int32_t N, int32_t D, int32_t T, int engine, int training) {
   if (N < 0 || D <= 0 || T < 0) return 0;
-  if (engine == DDFA_ENGINE_TCGEN05 && D != 128) return 0;
+  if (engine == DDFA_ENGINE_TCGEN05 && D != 128 && !ddfa::gru_tcw_width(D)) return 0;
   return ddfa::make_layout(N, D, T, engine, training).total;
 }
 
@@ -81,8 +81,8 @@ int ddfa_ggnn_fwd(const int32_t *indptr, const int32_t *indices, const float *x,
                   void *workspace, size_t workspace_bytes, int training, int engine, void *stream) {
   using namespace ddfa;
   DDFA_REQUIRE(N >= 0 && D > 0 && D % 4 == 0 && T >= 0, "ddfa_ggnn_fwd: bad sizes (N=%d D=%d T=%d)", N, D, T);
-  DDFA_REQUIRE(engine == DDFA_ENGINE_SIMT || (engine == DDFA_ENGINE_TCGEN05 && D == 128),
-               "ddfa_ggnn_fwd: the tcgen05 engine supports D == 128 only (engine=%d D=%d)", engine, D);
+  DDFA_REQUIRE(engine == DDFA_ENGINE_SIMT || (engine == DDFA_ENGINE_TCGEN05 && (D == 128 || gru_tcw_width(D))),
+               "ddfa_ggnn_fwd: the tcgen05 engine supports D = 128, 192, 256, 320, 384, 448 and 512 only (engine=%d D=%d)", engine, D);
   DDFA_REQUIRE(indptr && indices && x && w_msg && b_msg && w_ih && w_hh && b_ih && b_hh && h_out, "ddfa_ggnn_fwd: NULL pointer");
   DDFA_REQUIRE(h_out != x, "ddfa_ggnn_fwd: h_out must not alias x");
   const GgnnLayout L = make_layout(N, D, T, engine, training);
@@ -96,7 +96,7 @@ int ddfa_ggnn_fwd(const int32_t *indptr, const int32_t *indices, const float *x,
     DDFA_CUDA(cudaMemcpyAsync(h_out, x, (size_t)N * D * sizeof(float), cudaMemcpyDeviceToDevice, cs));
     return DDFA_OK;
   }
-  const bool tc = engine == DDFA_ENGINE_TCGEN05;
+  const bool tc = engine == DDFA_ENGINE_TCGEN05 && D == 128;
   float *w_fold = f32_at(workspace, L.w_fold), *b_fold = f32_at(workspace, L.b_fold);
   void *gws = u8_at(workspace, L.gru_ws);
   GGNN_TRY(ddfa_fold_weights_fwd(w_msg, b_msg, w_ih, D, w_fold, b_fold, stream));
@@ -134,8 +134,8 @@ int ddfa_ggnn_bwd(const int32_t *indptr, const int32_t *indptr_t, const int32_t 
                   size_t workspace_bytes, int engine, void *stream) {
   using namespace ddfa;
   DDFA_REQUIRE(N >= 0 && D > 0 && D % 4 == 0 && T >= 0, "ddfa_ggnn_bwd: bad sizes (N=%d D=%d T=%d)", N, D, T);
-  DDFA_REQUIRE(engine == DDFA_ENGINE_SIMT || (engine == DDFA_ENGINE_TCGEN05 && D == 128),
-               "ddfa_ggnn_bwd: the tcgen05 engine supports D == 128 only (engine=%d D=%d)", engine, D);
+  DDFA_REQUIRE(engine == DDFA_ENGINE_SIMT || (engine == DDFA_ENGINE_TCGEN05 && (D == 128 || gru_tcw_width(D))),
+               "ddfa_ggnn_bwd: the tcgen05 engine supports D = 128, 192, 256, 320, 384, 448 and 512 only (engine=%d D=%d)", engine, D);
   DDFA_REQUIRE(indptr && indptr_t && indices_t && x && w_msg && b_msg && w_ih && w_hh && dh_T && dx && dw_msg && db_msg && dw_ih && dw_hh &&
                    db_ih && db_hh,
                "ddfa_ggnn_bwd: NULL pointer");
@@ -151,7 +151,7 @@ int ddfa_ggnn_bwd(const int32_t *indptr, const int32_t *indptr_t, const int32_t 
     DDFA_CUDA(cudaMemcpyAsync(dx, dh_T, (size_t)N * D * sizeof(float), cudaMemcpyDeviceToDevice, cs));
     return DDFA_OK;
   }
-  const bool tc = engine == DDFA_ENGINE_TCGEN05;
+  const bool tc = engine == DDFA_ENGINE_TCGEN05 && D == 128;
   const bool batched = tc && T <= DDFA_WGRAD_MAX_STEPS;
   float *w_fold = f32_at(workspace, L.w_fold);
   float *dw_fold = f32_at(workspace, L.dw_fold), *db_fold = f32_at(workspace, L.db_fold);

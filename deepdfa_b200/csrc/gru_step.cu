@@ -7,7 +7,8 @@
 // which equals GRUCell(a, h) for a_v = sum_{u->v} (W h_u + b).
 //
 // This file holds the engine dispatch, the SIMT engine (fp32 FFMA GEMMs from sgemm.cu + fused
-// gate kernels) and the weight-folding helpers.  The tcgen05 engine lives in gru_tc_fwd.cu / gru_tc_bwd.cu.
+// gate kernels) and the weight-folding helpers.  The tcgen05 engine lives in gru_tc_fwd3.cu / gru_tc_bwd.cu (D == 128) and
+// gru_tc_wide.cu (D = 192 .. 512, D % 64 == 0: the SIMT data flow below with tensor-core GEMMs in place of the sgemm calls).
 #include "common.cuh"
 
 namespace ddfa {
@@ -236,8 +237,12 @@ size_t ddfa_gru_step_workspace_bytes(int32_t N, int32_t D, int engine) {
   if (N < 0 || D <= 0) return 0;
   // tcgen05: [packed per-slice weight images + biases][s image][h image]; the two images are only used by the
   // fp32-in/fp32-out entry ddfa_gru_step_fwd (N = 0 gives the size ddfa_gru_step_fwd_image needs).
-  if (engine == DDFA_ENGINE_TCGEN05) return D == 128 ? ddfa::gru_tc2_workspace_bytes() + 2 * ddfa::act_image_bytes(N) : 16;
-  return sizeof(float) * 2 * (size_t)N * 3 * (size_t)D;  // gi|gh
+  if (engine == DDFA_ENGINE_TCGEN05 && D == 128) return ddfa::gru_tc2_workspace_bytes() + 2 * ddfa::act_image_bytes(N);
+  if (engine == DDFA_ENGINE_TCGEN05 && !ddfa::gru_tcw_width(D)) return 16;
+  // tcgen05 at the wide widths: [W' and Whh operand images (ddfa_gru_step_prepare)][gi|gh][s and h images]
+  const size_t planes = sizeof(float) * 2 * (size_t)N * 3 * (size_t)D;  // gi|gh
+  if (engine == DDFA_ENGINE_TCGEN05) return ddfa::gru_tcw_weights_bytes(D) + planes + ddfa::gru_tcw_fwd_scratch_bytes(N, D);
+  return planes;
 }
 
 size_t ddfa_act_image_bytes(int64_t num_nodes) { return num_nodes < 0 ? 0 : ddfa::act_image_bytes(num_nodes); }
@@ -279,8 +284,8 @@ static int check_step_args(const char *who, int32_t N, int32_t D, int engine) {
   using namespace ddfa;
   DDFA_REQUIRE(N >= 0 && D > 0 && D % 4 == 0 && D <= 1024, "%s: unsupported shape N=%d D=%d", who, N, D);
   DDFA_REQUIRE(engine == DDFA_ENGINE_SIMT || engine == DDFA_ENGINE_TCGEN05, "%s: unknown engine %d", who, engine);
-  if (engine == DDFA_ENGINE_TCGEN05 && D != 128) {
-    set_error("%s: the tcgen05 engine supports D == 128 only (got %d); select DDFA_ENGINE_SIMT", who, D);
+  if (engine == DDFA_ENGINE_TCGEN05 && D != 128 && !gru_tcw_width(D)) {
+    set_error("%s: the tcgen05 engine supports D = 128, 192, 256, 320, 384, 448 and 512 only (got %d); select DDFA_ENGINE_SIMT", who, D);
     return DDFA_ERR_UNSUPPORTED;
   }
   return DDFA_OK;
@@ -293,6 +298,14 @@ int ddfa_gru_step_prepare(const float *w_fold, const float *b_fold, const float 
   if (rc) return rc;
   if (engine == DDFA_ENGINE_SIMT) return DDFA_OK;  // nothing to pre-pack
   DDFA_REQUIRE(w_fold && b_fold && b_ih && w_hh && b_hh, "ddfa_gru_step_prepare: NULL pointer");
+  if (D != 128) {      // the W' and Whh operand images at the head of the workspace
+    if (workspace == nullptr || workspace_bytes < gru_tcw_weights_bytes(D)) {
+      set_error("ddfa_gru_step_prepare: workspace too small (%zu < %zu)", workspace_bytes, gru_tcw_weights_bytes(D));
+      return DDFA_ERR_WORKSPACE;
+    }
+    DDFA_REQUIRE(aligned16(w_fold) && aligned16(w_hh), "ddfa_gru_step_prepare: w_fold / w_hh not 16-byte aligned");
+    return gru_tcw_prepare(w_fold, w_hh, D, workspace, as_stream(stream_));
+  }
   return gru_tc2_prepare(w_fold, b_fold, b_ih, w_hh, b_hh, workspace, workspace_bytes, as_stream(stream_));
 }
 
@@ -309,7 +322,7 @@ int ddfa_gru_step_fwd(const float *s, const float *h, const int32_t *indptr, con
     set_error("ddfa_gru_step_fwd: workspace too small (%zu < %zu)", workspace_bytes, ddfa_gru_step_workspace_bytes(N, D, engine));
     return DDFA_ERR_WORKSPACE;
   }
-  if (engine == DDFA_ENGINE_TCGEN05) {
+  if (engine == DDFA_ENGINE_TCGEN05 && D == 128) {
     // fp32-in / fp32-out convenience path (tests, tools): build the two operand images in the workspace, then run the
     // image kernel.  The training driver calls ddfa_gru_step_fwd_image with images written by the producer kernels.
     uint8_t *ws8 = static_cast<uint8_t *>(workspace);
@@ -321,11 +334,19 @@ int ddfa_gru_step_fwd(const float *s, const float *h, const int32_t *indptr, con
     if (rc) return rc;
     return gru_tc2_step_fwd(s_img, h_img, h, indptr, N, h_out, nullptr, save_gates, nullptr, workspace, workspace_bytes, stream);
   }
-  float *gi = static_cast<float *>(workspace);
+  const bool wide = engine == DDFA_ENGINE_TCGEN05;       // D = 192 .. 512: tensor-core GEMMs, the rest as SIMT
+  const size_t head = wide ? gru_tcw_weights_bytes(D) : 0;
+  float *gi = reinterpret_cast<float *>(static_cast<uint8_t *>(workspace) + head);
   float *gh = gi + (size_t)N * 3 * D;
-  rc = sgemm(0, 1, N, 3 * D, D, 1.f, s, D, w_fold, D, 0.f, gi, 3 * D, 1, stream);
-  if (rc) return rc;
-  rc = sgemm(0, 1, N, 3 * D, D, 1.f, h, D, w_hh, D, 0.f, gh, 3 * D, 1, stream);
+  if (wide) {
+    // s and h become operand images through 16-byte loads
+    DDFA_REQUIRE(aligned16(s) && aligned16(h), "ddfa_gru_step_fwd: s / h not 16-byte aligned");
+    rc = gru_tcw_fwd_gemms(s, h, N, D, workspace, gh + (size_t)N * 3 * D, gi, gh, stream);
+  } else {
+    rc = sgemm(0, 1, N, 3 * D, D, 1.f, s, D, w_fold, D, 0.f, gi, 3 * D, 1, stream);
+    if (rc) return rc;
+    rc = sgemm(0, 1, N, 3 * D, D, 1.f, h, D, w_hh, D, 0.f, gh, 3 * D, 1, stream);
+  }
   if (rc) return rc;
   const int64_t tot = (int64_t)N * (D / 4);
   gru_gate_fwd_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(gi, gh, h, indptr, b_fold, b_ih, b_hh, N, D, h_out, save_gates);
@@ -340,12 +361,16 @@ size_t ddfa_gru_step_bwd_workspace_bytes(int32_t N, int32_t D, int engine) {
 
 size_t ddfa_gru_step_bwd_workspace_bytes_steps(int32_t N, int32_t D, int engine, int32_t steps) {
   if (N < 0 || D <= 0) return 0;
-  if (engine == DDFA_ENGINE_TCGEN05) return D == 128 ? ddfa::gru_tc2_bwd_workspace_bytes(N, steps) : 16;   // layout: gru_tc_bwd.cu
+  if (engine == DDFA_ENGINE_TCGEN05 && D == 128) return ddfa::gru_tc2_bwd_workspace_bytes(N, steps);   // layout: gru_tc_bwd.cu
+  if (engine == DDFA_ENGINE_TCGEN05 && !ddfa::gru_tcw_width(D)) return 16;
   // dgi | dgh | bias slots of the gate-backward CTAs | split-K slices of one weight gradient (the last two: deterministic mode,
-  // reserved in both modes)
+  // reserved in both modes).  tcgen05 at the wide widths: [W' and Whh operand images] dgi | dgh | bias slots [operand images
+  // and weight-gradient slices: gru_tc_wide.cu] (the step count does not matter: the weight gradient is taken per step)
   const size_t slots = (size_t)((N + ddfa::kGateBwdRows - 1) / ddfa::kGateBwdRows) * 7 * D;
+  const size_t planes = sizeof(float) * (2 * (size_t)N * 3 * (size_t)D + slots);
+  if (engine == DDFA_ENGINE_TCGEN05) return ddfa::gru_tcw_weights_bytes(D) + planes + ddfa::gru_tcw_bwd_scratch_bytes(N, D);
   const size_t part = (size_t)ddfa::sgemm_splitk_ordered_slices(N, ddfa::simt_wgrad_split(N, D)) * 3 * D * D;
-  return sizeof(float) * (2 * (size_t)N * 3 * (size_t)D + slots + part);
+  return planes + sizeof(float) * part;
 }
 
 int ddfa_gru_bwd_wgrad_batched(const void *const *s_images, const void *const *h_images, int32_t steps, int32_t N, int32_t D,
@@ -411,6 +436,14 @@ int ddfa_gru_step_prepare_bwd(const float *w_fold, const float *w_hh, int32_t D,
   if (rc) return rc;
   if (engine == DDFA_ENGINE_SIMT) return DDFA_OK;
   DDFA_REQUIRE(w_fold && w_hh, "ddfa_gru_step_prepare_bwd: NULL pointer");
+  if (D != 128) {      // the W' and Whh operand images at the head of the workspace (read K-major forward, MN-major here)
+    if (workspace == nullptr || workspace_bytes < gru_tcw_weights_bytes(D)) {
+      set_error("ddfa_gru_step_prepare_bwd: workspace too small (%zu < %zu)", workspace_bytes, gru_tcw_weights_bytes(D));
+      return DDFA_ERR_WORKSPACE;
+    }
+    DDFA_REQUIRE(aligned16(w_fold) && aligned16(w_hh), "ddfa_gru_step_prepare_bwd: w_fold / w_hh not 16-byte aligned");
+    return gru_tcw_prepare(w_fold, w_hh, D, workspace, as_stream(stream_));
+  }
   return gru_tc2_prepare_bwd(w_fold, w_hh, workspace, workspace_bytes, as_stream(stream_));
 }
 
@@ -431,7 +464,7 @@ int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const
     set_error("ddfa_gru_step_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
     return DDFA_ERR_WORKSPACE;
   }
-  if (engine == DDFA_ENGINE_TCGEN05) {
+  if (engine == DDFA_ENGINE_TCGEN05 && D == 128) {
     // fp32-s convenience path (tests, tools): build the s image at the end of the workspace, then the image kernels
     void *s_img = gru_tc2_bwd_s_image_scratch(workspace, N);
     rc = act_to_image(s, N, s_img, stream);
@@ -439,12 +472,16 @@ int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const
     return gru_tc2_step_bwd(dh_out, nullptr, nullptr, nullptr, h, /*h_img_in=*/nullptr, s_img, gates, nullptr, indptr, N, ds, dh, dw_fold, db_fold, db_ih, dw_hh, db_hh,
                             workspace, workspace_bytes, /*wgrad_mode=*/0, stream);
   }
-  float *dgi = static_cast<float *>(workspace);
+  const bool wide = engine == DDFA_ENGINE_TCGEN05;       // D = 192 .. 512: tensor-core GEMMs, the rest as SIMT
+  // wide: s and h become operand images through 16-byte loads, ds / dh are written with 8-byte stores
+  DDFA_REQUIRE(!wide || (aligned16(s) && aligned16(h) && ((reinterpret_cast<uintptr_t>(ds) | reinterpret_cast<uintptr_t>(dh)) & 7) == 0),
+               "ddfa_gru_step_bwd: s / h must be 16-byte aligned, ds / dh 8-byte aligned");
+  float *dgi = reinterpret_cast<float *>(static_cast<uint8_t *>(workspace) + (wide ? gru_tcw_weights_bytes(D) : 0));
   float *dgh = dgi + (size_t)N * 3 * D;
   const bool det = deterministic();
   const int ctas = (N + kGateBwdRows - 1) / kGateBwdRows;
   float *bias_slots = dgh + (size_t)N * 3 * D;
-  float *wg_part = bias_slots + (size_t)ctas * 7 * D;
+  float *wg_part = bias_slots + (size_t)ctas * 7 * D;      // wide: the start of gru_tc_wide.cu's scratch
   dim3 block(D / 4, 256 / (D / 4) > 0 ? 256 / (D / 4) : 1);
   const size_t smem = sizeof(float) * block.y * 7 * D;
   gru_gate_bwd_kernel<<<ctas, block, smem, stream>>>(dh_out, h, gates, indptr, N, D, dgi, dgh, dh, db_fold, db_ih, db_hh,
@@ -453,6 +490,9 @@ int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const
   if (det) {
     bias_slots_sum_kernel<<<(7 * D + 255) / 256, 256, 0, stream>>>(bias_slots, ctas, D, db_fold, db_ih, db_hh);
     DDFA_CHECK_LAUNCH("bias_slots_sum_kernel");
+  }
+  if (wide) {
+    return gru_tcw_bwd_gemms(dgi, dgh, s, h, N, D, workspace, wg_part, ds, dh, dw_fold, dw_hh, stream);
   }
   // ds = dgi @ w_fold ; dh = dh_out*z + dgh @ w_hh
   rc = sgemm(0, 0, N, D, 3 * D, 1.f, dgi, 3 * D, w_fold, D, 0.f, ds, D, 1, stream);

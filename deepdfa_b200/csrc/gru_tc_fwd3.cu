@@ -298,36 +298,39 @@ int gru_tc3_step_fwd(const void *s_img, const void *h_img, const float *h, const
   return DDFA_OK;
 }
 
-// ---- fp32 [N,128] -> activation image (zero tail rows): h_0 enters the image pipeline here ------------------------------
+// ---- fp32 [N,D] -> image of D columns (tc_common.cuh: image_offset_w; zero tail rows): h_0 enters the image pipeline here, and
+// the wide-width engine (gru_tc_wide.cu) turns its GEMM operands into images with it --------------------------------------------
 namespace tc3 {
-__global__ void __launch_bounds__(256) to_image_kernel(const float *__restrict__ x, int32_t N, uint8_t *__restrict__ image) {
+__global__ void __launch_bounds__(256) to_image_kernel(const float *__restrict__ x, int32_t N, int32_t D, uint8_t *__restrict__ image) {
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;   // one thread = 8 consecutive columns of a row
+  const int units = D >> 3;
   const int64_t rows = ((int64_t)N + kTileM - 1) / kTileM * kTileM;
-  if (t >= rows * 16) return;
-  const int64_t node = t >> 4;
-  const int col = (int)(t & 15) * 8;
+  if (t >= rows * units) return;
+  const int64_t node = t / units;
+  const int col = (int)(t - node * units) * 8;
   float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (node < N) {
-    const float4 a = ldg_nc_f4(x + node * kD + col), b = ldg_nc_f4(x + node * kD + col + 4);
+    const float4 a = ldg_nc_f4(x + node * D + col), b = ldg_nc_f4(x + node * D + col + 4);
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
   }
   uint4 ph, pl;
   split8(v, ph, pl);
-  *reinterpret_cast<uint4 *>(image + image_offset(node, col, 0)) = ph;
-  *reinterpret_cast<uint4 *>(image + image_offset(node, col, 1)) = pl;
+  *reinterpret_cast<uint4 *>(image + image_offset_w(node, col, 0, D)) = ph;
+  *reinterpret_cast<uint4 *>(image + image_offset_w(node, col, 1, D)) = pl;
 }
 }  // namespace tc3
 
 size_t act_image_bytes(int64_t n) { return tcc::image_bytes(n); }
 
-int act_to_image(const float *x, int32_t N, void *image, cudaStream_t stream) {
+int act_to_image(const float *x, int32_t N, int32_t D, void *image, cudaStream_t stream) {
   const int64_t rows = ((int64_t)N + tcc::kTileM - 1) / tcc::kTileM * tcc::kTileM;
-  const int64_t total = rows * 16;
+  const int64_t total = rows * (D / 8);
   if (total == 0) return DDFA_OK;
-  tc3::to_image_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(x, N, static_cast<uint8_t *>(image));
+  tc3::to_image_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(x, N, D, static_cast<uint8_t *>(image));
   DDFA_CHECK_LAUNCH("to_image_kernel");
   return DDFA_OK;
 }
+int act_to_image(const float *x, int32_t N, void *image, cudaStream_t stream) { return act_to_image(x, N, tcc::kD, image, stream); }
 
 // workspace-checked entry points used by gru_step.cu (the forward workspace is exactly the packed weights)
 size_t gru_tc2_workspace_bytes() { return gru_tc3_packed_bytes(); }

@@ -159,6 +159,13 @@ __host__ __device__ __forceinline__ size_t image_offset(int64_t node, int col, i
   return (size_t)(node / kTileM) * kImageTileBytes + (size_t)((v * 2 + (col >> 6)) * kChunkBytes) +
          sw128_offset((int)(node % kTileM), col & 63);
 }
+// The same layout for a matrix of D columns (D a multiple of 64): a 128-row tile is [hi | lo][D / 64 column chunks] of 16 KB,
+// 128 x D x 4 bytes.  D = 128 is the activation image above.  The wide-width engine (gru_tc_wide.cu) keeps every GEMM operand so.
+__host__ __device__ __forceinline__ size_t image_bytes_w(int64_t n, int D) { return (size_t)((n + kTileM - 1) / kTileM) * kTileM * 4 * (size_t)D; }
+__host__ __device__ __forceinline__ size_t image_offset_w(int64_t node, int col, int v, int D) {
+  return (size_t)(node / kTileM) * ((size_t)kTileM * 4 * D) + (size_t)((v * (D >> 6) + (col >> 6)) * kChunkBytes) +
+         sw128_offset((int)(node % kTileM), col & 63);
+}
 
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16 &hi, __nv_bfloat16 &lo) {
   hi = __float2bfloat16_rn(x);

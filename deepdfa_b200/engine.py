@@ -310,7 +310,9 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     nl = len(params.mlp_w)
     st = _stream_ptr()
 
-    use_images = engine == ENGINE_TCGEN05     # activations travel as MMA-ready bf16 hi/lo images (include/ddfa_b200.h)
+    # activations travel as MMA-ready bf16 hi/lo images (include/ddfa_b200.h); at the other tcgen05 widths the step follows the
+    # SIMT call sequence and ddfa_gru_step_fwd runs its GEMMs on the tensor cores (csrc/gru_tc_wide.cu)
+    use_images = engine == ENGINE_TCGEN05 and D == 128
     ggnn_train = training and grad_ggnn       # keep the per-step state the GGNN backward reads
     if x_in is not None and tuple(x_in.shape) != (N, D):
         raise DdfaError(f"forward: x_in of shape {tuple(x_in.shape)}, need ({N}, {D})")
@@ -504,16 +506,18 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     dw_fold.zero_()
     db_fold.zero_()
     ds = alloc.get("ds", (N, D))
+    # the D == 128 tensor-core path (images, packed state, fused backward); at the wider tcgen05 widths the SIMT call sequence
+    images = engine == ENGINE_TCGEN05 and D == 128
     ds_prev = None                     # tcgen05 engine: ds of the step after t, folded into step t's call (dh' = dh + A^T ds)
-    ds_alt = alloc.get("ds_b", (N, D)) if engine == ENGINE_TCGEN05 else None
+    ds_alt = alloc.get("ds_b", (N, D)) if images else None
     fuse_gather = OPTIONS["fuse_gather_bwd"]
     # tcgen05: keep the q images of every step and run the weight-gradient GEMM of the whole pass as ONE launch at the end
-    batched_wgrad = engine == ENGINE_TCGEN05 and bool(saved.h_img) and 0 < T <= 16 and OPTIONS["batched_wgrad"]
+    batched_wgrad = images and bool(saved.h_img) and 0 < T <= 16 and OPTIONS["batched_wgrad"]
     ws_bytes = L.call("ddfa_gru_step_bwd_workspace_bytes_steps", N, D, engine, T if batched_wgrad else 1)
     ws = alloc.get("gru_ws_bwd", (max(ws_bytes, 16),), torch.uint8)
     L.call("ddfa_gru_step_prepare_bwd", _p(saved.w_fold), _p(params.w_hh), D, engine, _p(ws), ws_bytes, st)
     for t in range(T - 1, -1, -1):
-        if engine == ENGINE_TCGEN05:     # saved.s[t] is the activation image of s_t
+        if images:     # saved.s[t] is the activation image of s_t
             _call("ddfa_gru_step_bwd_image_v2" if saved.gates[t].dtype == torch.uint8 else "ddfa_gru_step_bwd_image",
                   _p(dh), _p(ds_prev), _p(dg.indptr_t), _p(dg.indices_t), _p(saved.h[t]),
                   _p(saved.h_img[t]), _p(saved.s[t]), _p(saved.gates[t]), _p(dg.indptr), N, D,
@@ -530,7 +534,7 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
         # dh_t += A^T ds   (gather over the transposed graph)
         _call("ddfa_gather_sum", _p(dg.indptr_t), _p(dg.indices_t), _p(ds), N, D, _p(dh_alt), 1, st, tag="gather_bwd")
         dh, dh_alt = dh_alt, dh
-    if engine == ENGINE_TCGEN05 and T > 0 and fuse_gather:     # the gather of the last ds (step 0) has no following step to ride on
+    if images and T > 0 and fuse_gather:     # the gather of the last ds (step 0) has no following step to ride on
         _call("ddfa_gather_sum", _p(dg.indptr_t), _p(dg.indices_t), _p(ds_prev), N, D, _p(dh), 1, st, tag="gather_bwd")
     if not grad_weights:
         return dh, dx_direct
@@ -542,7 +546,7 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
               ptr_array([_p(t) for t in grads.tables]), _p(emb_ws), emb_bytes, st, tag="ddfa_embed_concat_bwd")
     if on_small_grads_ready is not None:
         on_small_grads_ready()
-    if engine == ENGINE_TCGEN05 and T > 0:
+    if images and T > 0:
         if batched_wgrad:
             _call("ddfa_gru_bwd_wgrad_batched", ptr_array([_p(saved.s[t]) for t in range(T)]), ptr_array([_p(saved.h_img[t]) for t in range(T)]),
                   T, N, D, _p(dw_fold), _p(grads.w_hh), _p(ws), ws_bytes, st, tag="wgrad_batched")

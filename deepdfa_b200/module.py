@@ -36,7 +36,10 @@ allfeats = ["api", "datatype", "literal", "operator"]  # reference ggnn.py:17-19
 
 _ENGINES = {"simt": ENGINE_SIMT, "tcgen05": ENGINE_TCGEN05}
 MAX_HIDDEN_WIDTH = 512      # readout.cu (kMaxChunks = 4: D <= 512) and the embedding backward (K * H <= 512)
-TCGEN05_WIDTH = 128         # the tensor-core GRU kernels are written for D == 128
+TCGEN05_WIDTH = 128         # the tensor-core GRU kernels with activation images and the fused backward are written for D == 128
+# every width the tensor-core engine runs: 128, and the multiples of 64 from 192 up (gru_tc_wide.cu: the SIMT engine's data flow
+# with its six GEMMs on the tensor cores)
+TCGEN05_WIDTHS = (TCGEN05_WIDTH,) + tuple(range(192, MAX_HIDDEN_WIDTH + 1, 64))
 
 
 def default_engine(hidden_width: int) -> str:
@@ -127,8 +130,8 @@ class FlowGNNGGNNModule(nn.Module):
 
     Extra keyword (not in the reference): ``engine`` = "simt" | "tcgen05" selects the GEMM engine of the
     GRU step (default: ``$DDFA_B200_ENGINE`` if set, else ``default_engine(W)``).  The hidden width W (``hidden_dim``, times 4
-    with ``concat_all_absdf``) must be a multiple of 4 and at most 512; "tcgen05" runs W = 128 only.  Both are checked here
-    (``ValueError``).
+    with ``concat_all_absdf``) must be a multiple of 4 and at most 512; "tcgen05" runs W = 128 and W = 192, 256, ..., 512
+    (``TCGEN05_WIDTHS``).  Both are checked here (``ValueError``).  The default stays "simt" at every width but 128.
     """
 
     def __init__(self, feat, input_dim, hidden_dim, n_steps, num_output_layers, label_style="graph",
@@ -209,8 +212,9 @@ class FlowGNNGGNNModule(nn.Module):
             engine = os.environ.get("DDFA_B200_ENGINE") or default_engine(hidden_dim)
         if engine not in _ENGINES:
             raise ValueError(f"engine must be one of {sorted(_ENGINES)}, got {engine!r}")
-        if engine == "tcgen05" and hidden_dim != TCGEN05_WIDTH:
-            raise ValueError(f"engine='tcgen05' (from the {source}) runs hidden width {TCGEN05_WIDTH} only, got {hidden_dim} ({config}); "
+        if engine == "tcgen05" and hidden_dim not in TCGEN05_WIDTHS:
+            widths = ", ".join(str(w) for w in TCGEN05_WIDTHS[:-1]) + f" and {TCGEN05_WIDTHS[-1]}"
+            raise ValueError(f"engine='tcgen05' (from the {source}) runs hidden widths {widths} only, got {hidden_dim} ({config}); "
                              "use engine='simt'")
         self.engine = engine
         # Input validation (the reference raises on an out-of-range embedding index; DGL rejects edge ids >= num_nodes):

@@ -40,7 +40,11 @@ typedef enum ddfa_status {
 
 /* GEMM engines for the dense GRU matmuls */
 #define DDFA_ENGINE_SIMT 0     /* fp32 FFMA reference kernels (any D % 4 == 0)              */
-#define DDFA_ENGINE_TCGEN05 1  /* tensor-core engine (name kept): Hopper wgmma, bf16x3 split operands, fp32 accumulate (D == 128) */
+#define DDFA_ENGINE_TCGEN05 1  /* tensor-core engine (name kept): Hopper wgmma, bf16x3 split operands, fp32 accumulate.
+                                  D == 128: activation images, packed saved gates, fused backward (the entry points marked
+                                  "tcgen05 engine" below).  D = 192, 256, 320, 384, 448, 512: the SIMT entry points' data flow
+                                  (fp32 planes, fp32 saved gates) with tensor-core GEMMs (ddfa_gru_tc_wide_gemm).  Any other D:
+                                  DDFA_ERR_UNSUPPORTED. */
 
 int ddfa_abi_version(void);
 const char *ddfa_last_error(void);
@@ -273,6 +277,10 @@ int ddfa_gru_bwd_wgrad_batched(const void *const *s_images, const void *const *h
  * prepared once per backward pass by ddfa_gru_step_prepare_bwd (transposed bf16 hi/lo weight
  * images) and is then reused by every step of that pass. */
 size_t ddfa_gru_step_bwd_workspace_bytes(int32_t num_nodes, int32_t dim, int engine);
+/* ddfa_gru_step_prepare / _prepare_bwd with engine = TCGEN05 at D = 192 .. 512 write the bf16 hi / lo operand images of W' and
+ * Whh at the head of the step workspace; ddfa_gru_step_fwd / _bwd then run their GEMMs on the tensor cores (the images of the
+ * step's activations are built inside the workspace).  The weight gradient is split over the nodes into slices that are added
+ * in slice order in every mode (bit-identical on repeat). */
 int ddfa_gru_step_prepare_bwd(const float *w_fold, const float *w_hh, int32_t dim, int engine,
                               void *workspace, size_t workspace_bytes, void *stream);
 int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const float *gates,
@@ -280,6 +288,17 @@ int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const
                       int32_t num_nodes, int32_t dim, float *ds, float *dh, float *dw_fold,
                       float *db_fold, float *db_ih, float *dw_hh, float *db_hh, void *workspace,
                       size_t workspace_bytes, int engine, void *stream);
+/* The tensor-core GEMMs of the step at the wide widths (D = 192 .. 512, D % 64 == 0), callable one by one (tests, tools); all
+ * operands fp32 row-major, N = num_nodes rows:
+ *   call 0: c[N,3D] = a[N,D] b[3D,D]^T      (gi = s W'^T, gh = h Whh^T)
+ *   call 1: c[N,D] = a[N,3D] b[3D,D]        (ds = dgi W')
+ *   call 2: c[N,D] += a[N,3D] b[3D,D]       (dh += dgh Whh)
+ *   call 3: c[3D,D] += a[N,3D]^T b[N,D]     (dW' += dgi^T s, dWhh += dgh^T h; ddfa_gru_tc_wide_wgrad_slices(N, D) slices)
+ * Rows of c past N are never written.  Other D: DDFA_ERR_UNSUPPORTED. */
+size_t ddfa_gru_tc_wide_gemm_workspace_bytes(int call, int32_t num_nodes, int32_t dim);
+int ddfa_gru_tc_wide_gemm(int call, const float *a, const float *b, int32_t num_nodes, int32_t dim, float *c, void *workspace,
+                          size_t workspace_bytes, void *stream);
+size_t ddfa_gru_tc_wide_wgrad_slices(int32_t num_nodes, int32_t dim);
 
 /* ---------------------------------------------------------------------------------------
  * K3+K4 over all T steps: the whole dgl.nn.GatedGraphConv (ggnn.py:57-60 construction, :95 call) behind one call each.
@@ -289,7 +308,7 @@ int ddfa_gru_step_bwd(const float *dh_out, const float *h, const float *s, const
  *   fwd: x = h_0 [N,D] (the embedding output; must stay valid until the backward) -> h_out = h_T [N,D].
  *   bwd: dh_T [N,D] -> dx [N,D] = dL/dh_0 (overwritten); dw_msg[D,D], db_msg[D], dw_ih[3D,D], dw_hh[3D,D], db_ih[3D],
  *        db_hh[3D] accumulated (+=).  w_msg / b_msg = GatedGraphConv.linears[0], the rest = GatedGraphConv.gru.
- * engine = DDFA_ENGINE_SIMT (any D % 4 == 0) or DDFA_ENGINE_TCGEN05 (D == 128). */
+ * engine = DDFA_ENGINE_SIMT (any D % 4 == 0) or DDFA_ENGINE_TCGEN05 (D = 128, 192, 256, 320, 384, 448, 512). */
 size_t ddfa_ggnn_workspace_bytes(int32_t num_nodes, int32_t dim, int32_t n_steps, int engine, int training);
 int ddfa_ggnn_fwd(const int32_t *indptr, const int32_t *indices, const float *x, int32_t num_nodes, int32_t dim,
                   int32_t n_steps, const float *w_msg, const float *b_msg, const float *w_ih, const float *w_hh,
