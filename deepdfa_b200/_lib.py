@@ -127,6 +127,9 @@ _SIGNATURES = {
     "ddfa_stmt_input_grad_score": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _vp, _vp]),
     "ddfa_stmt_scale_input": (_int, [_vp, _f32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_stmt_node_probability": (_int, [_vp, _vp, _i32, _vp, _vp]),
+    "ddfa_stmt_attribution_score": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _vp, _vp]),
+    "ddfa_stmt_shap_input": (_int, [_vp, _vp, _i32, _i32, _i32, _f32, _f32, _f32, C.c_uint64, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "ddfa_mlp_dgrad_rescale": (_int, [_vp] * 7 + [_i32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_grad_accumulate": (_int, [_vp, _vp, _i64, _i64, _i32, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
 }

@@ -301,6 +301,18 @@ __global__ void relu_mask_kernel(const float *in, const float *__restrict__ mask
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i < total) out[i] = (mask[i] > 0.f) ? in[i] : 0.f;
 }
+// DeepLift's rescale rule at a hidden ReLU (captum's `nonlinear`): with z = zg + bias and z' = zrg + bias the pre-activations of the
+// input and the reference pass, din *= (relu(z) - relu(z')) / (z - z'), or the plain derivative [act > 0] where |z - z'| < 1e-10
+__global__ void __launch_bounds__(256) rescale_relu_kernel(float *__restrict__ din, const float *__restrict__ zg, const float *__restrict__ zrg,
+                                                           const float *__restrict__ bias, const float *__restrict__ act, int64_t total,
+                                                           int32_t n) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float b = bias[i % n];
+  const float z = zg[i] + b, zr = zrg[i] + b;
+  const float dz = z - zr;
+  din[i] = fabsf(dz) < 1e-10f ? (act[i] > 0.f ? din[i] : 0.f) : din[i] * (fmaxf(z, 0.f) - fmaxf(zr, 0.f)) / dz;
+}
 // ---- MLP head over the whole batch (large training batches): hidden layers as one GEMM each + this epilogue, last layer below ----
 // a[m, n] = max(a[m, n] + bias[n], 0), 4 columns per thread (n % 4 == 0)
 __global__ void __launch_bounds__(256) bias_relu_kernel(float *__restrict__ a, const float *__restrict__ bias, int64_t total4, int32_t n4) {
@@ -435,6 +447,44 @@ int ddfa_mlp_bwd(const float *dlogits, const float *pooled, const float *mlp_act
       dout = din;
       out_dim = D2;
     }
+  }
+  return DDFA_OK;
+}
+
+int ddfa_mlp_dgrad_rescale(const float *dlogits, const float *pooled, const float *mlp_act, const float *pooled_ref,
+                           const float *mlp_act_ref, const float *const *mlp_w, const float *const *mlp_b, int32_t B, int32_t D,
+                           int32_t L, float *dpooled, float *scratch, void *stream_) {
+  using namespace ddfa;
+  DDFA_REQUIRE(B >= 0 && D > 0 && L >= 1 && L <= kMaxMlpLayers, "ddfa_mlp_dgrad_rescale: bad shape B=%d D=%d L=%d", B, D, L);
+  if (B == 0) return DDFA_OK;
+  DDFA_REQUIRE(dlogits && pooled && pooled_ref && mlp_w && dpooled && scratch, "ddfa_mlp_dgrad_rescale: NULL pointer");
+  DDFA_REQUIRE(L == 1 || (mlp_act && mlp_act_ref && mlp_b), "ddfa_mlp_dgrad_rescale: mlp_act, mlp_act_ref and mlp_b required for num_layers > 1");
+  cudaStream_t stream = as_stream(stream_);
+  const int D2 = 2 * D;
+  const size_t plane = (size_t)B * D2;
+  float *buf0 = scratch, *buf1 = scratch + plane, *z = scratch + 2 * plane, *zr = scratch + 3 * plane;
+  const float *dout = dlogits;
+  int out_dim = 1;
+  for (int i = L - 1; i >= 0; --i) {
+    // dIn[B,2D] = dOut[B,out] @ W_i[out,2D]: the call of ddfa_mlp_bwd
+    float *din = (i == 0) ? dpooled : (dout == buf0 ? buf1 : buf0);
+    int rc = sgemm(0, 0, B, D2, out_dim, 1.f, dout, out_dim, mlp_w[i], D2, 0.f, din, D2, 1, stream);
+    if (rc) return rc;
+    if (i == 0) break;
+    // in_i = relu(z_{i-1}): the pre-activations of both passes, recomputed from the inputs of layer i - 1 (the forward's hidden-layer
+    // GEMM when the batch ran the batched head)
+    const float *in = (i == 1) ? pooled : mlp_act + (size_t)(i - 2) * plane;
+    const float *in_ref = (i == 1) ? pooled_ref : mlp_act_ref + (size_t)(i - 2) * plane;
+    rc = sgemm(0, 1, B, D2, D2, 1.f, in, D2, mlp_w[i - 1], D2, 0.f, z, D2, 1, stream);
+    if (rc) return rc;
+    rc = sgemm(0, 1, B, D2, D2, 1.f, in_ref, D2, mlp_w[i - 1], D2, 0.f, zr, D2, 1, stream);
+    if (rc) return rc;
+    const int64_t tot = (int64_t)plane;
+    rescale_relu_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(din, z, zr, mlp_b[i - 1], mlp_act + (size_t)(i - 1) * plane,
+                                                                           tot, D2);
+    DDFA_CHECK_LAUNCH("rescale_relu_kernel");
+    dout = din;
+    out_dim = D2;
   }
   return DDFA_OK;
 }

@@ -152,6 +152,70 @@ __global__ void __launch_bounds__(256) node_probability_kernel(const float *__re
     scores[n] = n < S ? 1.f / (1.f + expf(-logits[n])) : 0.f;    // eval_metrics.cu's p: what predictions() stores
 }
 
+// ---- DeepLift / DeepLiftShap / GradientShap inputs ----------------------------------------------------------------------------
+// Philox4x32-10 (Salmon et al., SC'11), key = the 64-bit seed, counter (batch, sample, index, column word): all four output words
+__device__ __forceinline__ uint4 philox4(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint64_t seed) {
+  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+  }
+  return make_uint4(c0, c1, c2, c3);
+}
+
+// the column word of the counter: the noise of column quad q is q, the baseline's q | kBaseWord, the function's alpha kAlphaWord
+constexpr uint32_t kBaseWord = 0x40000000u, kAlphaWord = 0x80000000u;
+
+__device__ __forceinline__ float uniform24(uint32_t w) { return (float)(w >> 8) * 0x1p-24f; }       // [0, 1), exact
+
+// Box-Muller on the words (a, b): u1 = ((a >> 8) + 1) 2^-24 in (0, 1], u2 = (b >> 8) 2^-24
+__device__ __forceinline__ float2 gauss2(uint32_t a, uint32_t b) {
+  const float r = sqrtf(-2.f * logf((float)((a >> 8) + 1u) * 0x1p-24f));
+  float s, c;
+  sincospif(2.f * uniform24(b), &s, &c);
+  return make_float2(r * c, r * s);
+}
+
+__device__ __forceinline__ float4 gauss4(uint4 w) {
+  const float2 p = gauss2(w.x, w.y), q = gauss2(w.z, w.w);
+  return make_float4(p.x, p.y, q.x, q.y);
+}
+
+// one CTA per function (grid-stride): alpha_b (given, or drawn from word 0 of the function's counter), then per column quad of its
+// nodes x~ = x + noise_stdev eps, b = baseline_stdev eps', diff = x~ - b, input = fmaf(alpha_b, diff, b)
+__global__ void __launch_bounds__(256) shap_input_kernel(const float *__restrict__ x, const int32_t *__restrict__ graph_ptr, int32_t B,
+                                                        int32_t D, float alpha, float noise_stdev, float base_stdev, uint64_t seed,
+                                                        const int64_t *__restrict__ counter, uint32_t sample, float *__restrict__ input,
+                                                        float *__restrict__ diff) {
+  const uint32_t batch = (uint32_t)(uint64_t)*counter;
+  const int32_t quads = D / 4;
+  for (int32_t b = blockIdx.x; b < B; b += gridDim.x) {
+    const float a = alpha >= 0.f ? alpha : uniform24(philox4(batch, sample, (uint32_t)b, kAlphaWord, seed).x);
+    const int32_t n0 = graph_ptr[b], n1 = graph_ptr[b + 1];
+    const int64_t units = (int64_t)(n1 - n0) * quads;
+    for (int64_t i = threadIdx.x; i < units; i += 256) {
+      const int32_t n = n0 + (int32_t)(i / quads), q = (int32_t)(i % quads);
+      const int64_t off = (int64_t)n * D + 4 * q;
+      float4 xt = *reinterpret_cast<const float4 *>(x + off);
+      float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (noise_stdev > 0.f) {
+        const float4 e = gauss4(philox4(batch, sample, (uint32_t)n, (uint32_t)q, seed));
+        xt.x += noise_stdev * e.x; xt.y += noise_stdev * e.y; xt.z += noise_stdev * e.z; xt.w += noise_stdev * e.w;
+      }
+      if (base_stdev > 0.f) {
+        const float4 e = gauss4(philox4(batch, sample, (uint32_t)n, (uint32_t)q | kBaseWord, seed));
+        bv = make_float4(base_stdev * e.x, base_stdev * e.y, base_stdev * e.z, base_stdev * e.w);
+      }
+      const float4 d = make_float4(xt.x - bv.x, xt.y - bv.y, xt.z - bv.z, xt.w - bv.w);
+      *reinterpret_cast<float4 *>(diff + off) = d;
+      *reinterpret_cast<float4 *>(input + off) = make_float4(fmaf(a, d.x, bv.x), fmaf(a, d.y, bv.y), fmaf(a, d.z, bv.z), fmaf(a, d.w, bv.w));
+    }
+  }
+}
+
 inline int grid_for(int64_t units, int per_cta) {
   const int64_t c = (units + per_cta - 1) / per_cta;
   return (int)(c < 1 ? 1 : (c > 8 * kNumSMs ? 8 * kNumSMs : c));
@@ -228,6 +292,42 @@ int ddfa_stmt_scale_input(const float *x, float alpha, int32_t num_nodes, int32_
   scale_rows_kernel<<<grid_for(numel, 256), 256, 0, as_stream(stream_)>>>(x, alpha, numel, out);
   DDFA_CHECK_LAUNCH("stmt_scale_rows_kernel");
   if (image) return ddfa_act_to_image(out, num_nodes, dim, image, stream_);
+  return DDFA_OK;
+}
+
+int ddfa_stmt_attribution_score(const float *diff, const float *dh, const float *dx, int32_t num_nodes, int32_t dim, float weight,
+                                int32_t accumulate, float *score, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::stmt;
+  DDFA_REQUIRE(num_nodes >= 0 && dim > 0, "ddfa_stmt_attribution_score: need num_nodes (%d) >= 0 and dim (%d) > 0", num_nodes, dim);
+  if (num_nodes == 0) return DDFA_OK;
+  DDFA_REQUIRE(diff && dh && dx && score, "ddfa_stmt_attribution_score: NULL pointer");
+  // the x * g rule of ddfa_stmt_input_grad_score with the difference tensor in place of x: the same sums, bit for bit
+  input_grad_score_kernel<DDFA_STMT_SCORE_X_TIMES><<<(num_nodes + 7) / 8, 256, 0, as_stream(stream_)>>>(diff, dh, dx, num_nodes, dim,
+                                                                                                     weight, accumulate, score);
+  DDFA_CHECK_LAUNCH("stmt_attribution_score_kernel");
+  return DDFA_OK;
+}
+
+int ddfa_stmt_shap_input(const float *x, const int32_t *graph_ptr, int32_t num_graphs, int32_t num_nodes, int32_t dim, float alpha,
+                         float noise_stdev, float baseline_stdev, uint64_t seed, const int64_t *counter, int32_t sample, float *input,
+                         float *diff, void *image, void *stream_) {
+  using namespace ddfa;
+  using namespace ddfa::stmt;
+  DDFA_REQUIRE(num_graphs >= 0 && num_nodes >= 0 && dim > 0 && dim % 4 == 0,
+               "ddfa_stmt_shap_input: need num_graphs (%d) >= 0, num_nodes (%d) >= 0 and dim (%d) a positive multiple of 4", num_graphs,
+               num_nodes, dim);
+  DDFA_REQUIRE(alpha <= 1.f && noise_stdev >= 0.f && baseline_stdev >= 0.f && sample >= 0,
+               "ddfa_stmt_shap_input: need alpha <= 1 (negative: drawn), stdevs >= 0 and sample >= 0");
+  DDFA_REQUIRE(image == nullptr || dim == 128, "ddfa_stmt_shap_input: activation images exist for dim == 128 only (dim=%d)", dim);
+  if (num_nodes == 0 || num_graphs == 0) return DDFA_OK;
+  DDFA_REQUIRE(x && graph_ptr && counter && input && diff, "ddfa_stmt_shap_input: NULL pointer");
+  DDFA_REQUIRE(x != input && x != diff && input != diff, "ddfa_stmt_shap_input: input, diff and x must not alias");
+  DDFA_REQUIRE(aligned16(x) && aligned16(input) && aligned16(diff), "ddfa_stmt_shap_input: 16-byte alignment required");
+  shap_input_kernel<<<num_graphs < 8 * kNumSMs ? num_graphs : 8 * kNumSMs, 256, 0, as_stream(stream_)>>>(
+      x, graph_ptr, num_graphs, dim, alpha, noise_stdev, baseline_stdev, seed, counter, (uint32_t)sample, input, diff);
+  DDFA_CHECK_LAUNCH("stmt_shap_input_kernel");
+  if (image) return ddfa_act_to_image(input, num_nodes, dim, image, stream_);
   return DDFA_OK;
 }
 

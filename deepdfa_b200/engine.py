@@ -287,7 +287,7 @@ def node_indices(g: BatchedCFG, concat_all_absdf: bool, feature_key: str, device
 def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps: int, *, training: bool,
             engine: int = ENGINE_SIMT, alloc=None, oob_counter: Optional[torch.Tensor] = None, head: bool = True,
             grad_ggnn: bool = True, x_in: Optional[torch.Tensor] = None, x_scale: float = 1.0,
-            attention: Optional[torch.Tensor] = None):
+            attention: Optional[torch.Tensor] = None, x_fill=None):
     """Returns (pooled [B,2D], logits [B] or None, Saved or None).  ``head=False`` stops before the readout and returns
     (x [N,D], h_T [N,D], Saved or None) instead: the label_style="node" trainer runs its own head over a row list
     (``node_head_fwd``); Saved then holds no readout state.
@@ -297,7 +297,9 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     ``x_in`` ([N, D] fp32, e.g. the embedding output ``alloc`` holds as "x" after an earlier forward): the pass starts from
     ``x_scale * x_in`` instead of the embedding lookup — h_0 and the readout's concat half both see the scaled rows, which are
     written to the buffer "x_scaled" (and, for the tcgen05 engine, to h_0's activation image) by ``ddfa_stmt_scale_input``.
-    ``attention`` ([N] fp32): receives the readout's per-node softmax gate α_n (``ddfa_stmt_attention``)."""
+    ``attention`` ([N] fp32): receives the readout's per-node softmax gate α_n (``ddfa_stmt_attention``).
+    ``x_fill`` (instead of ``x_in``): ``x_fill(out, image)`` writes the pass's h_0 rows into ``out`` (the buffer "x_scaled", [N, D])
+    and, when ``image`` is not None (tcgen05 engine at D = 128), their activation image — ``ddfa_stmt_shap_input`` does both."""
     _require_cuda(*params.flat_list(), dg.indptr, *idx)
     L = _lib.lib()
     _lib.apply_deterministic_mode()
@@ -316,16 +318,21 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     ggnn_train = training and grad_ggnn       # keep the per-step state the GGNN backward reads
     if x_in is not None and tuple(x_in.shape) != (N, D):
         raise DdfaError(f"forward: x_in of shape {tuple(x_in.shape)}, need ({N}, {D})")
-    x = alloc.get("x" if x_in is None else "x_scaled", (N, D))
+    if x_in is not None and x_fill is not None:
+        raise DdfaError("forward: x_in and x_fill are alternatives")
+    x = alloc.get("x" if x_in is None and x_fill is None else "x_scaled", (N, D))
     h_imgs = None
     img_bytes = L.call("ddfa_act_image_bytes", N) if use_images else 0
-    if x_in is not None:
+    if x_in is not None or x_fill is not None:
         img = None
         if use_images and OPTIONS["packed_state"]:
             n_img = T if ggnn_train else 2
             h_imgs = [alloc.get_image(f"h_img{i}", img_bytes) for i in range(max(n_img, 1))]
             img = h_imgs[0]
-        _call("ddfa_stmt_scale_input", _p(x_in), float(x_scale), N, D, _p(x), _p(img), st)
+        if x_fill is not None:
+            x_fill(x, img)
+        else:
+            _call("ddfa_stmt_scale_input", _p(x_in), float(x_scale), N, D, _p(x), _p(img), st)
     elif use_images and OPTIONS["packed_state"]:
         # the embedding kernel writes h_0 = x as fp32 rows AND as its activation image (one pass instead of embed + ddfa_act_to_image)
         n_img = T if ggnn_train else 2        # training keeps the image of every h_t (the weight-gradient GEMM reads it)
@@ -432,7 +439,7 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
 def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack, *, dlogits: Optional[torch.Tensor] = None,
              dpooled: Optional[torch.Tensor] = None, engine: int = ENGINE_SIMT, alloc=None, on_small_grads_ready=None,
              dh_final: Optional[torch.Tensor] = None, dx_direct: Optional[torch.Tensor] = None, grad_ggnn: bool = True,
-             grad_tables: bool = True, grad_weights: bool = True):
+             grad_tables: bool = True, grad_weights: bool = True, mlp_ref: Optional[tuple] = None):
     """Accumulates (+=) parameter gradients into ``grads``.  Exactly one of dlogits / dpooled / (dh_final, dx_direct) is given.
     ``dh_final`` / ``dx_direct`` ([N, D] each, from ``node_head_bwd``): the gradients of h_T and of the direct use of x; the
     GGNN backward starts from them and the MLP / readout backward is skipped (their gradients are left alone).  ``dh_final``
@@ -463,9 +470,18 @@ def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack,
     if not grad_weights and not grad_ggnn:
         raise DdfaError("backward: grad_weights=False needs the GGNN backward (grad_ggnn=True)")
 
+    if mlp_ref is not None and dlogits is None:
+        raise DdfaError("backward: mlp_ref goes with dlogits")
     if dh_final is not None or dx_direct is not None:
         if dh_final is None or dx_direct is None or dlogits is not None or dpooled is not None:
             raise DdfaError("backward: dh_final and dx_direct go together, without dlogits / dpooled")
+    elif dlogits is not None and mlp_ref is not None:
+        if nl == 0 or grad_weights:
+            raise DdfaError("backward: mlp_ref needs an MLP head and grad_weights=False (the rescaled pass computes no weight gradient)")
+        dpooled = alloc.get("dpooled", (B, 2 * D))
+        scratch = alloc.get("mlp_rescale_scratch", (4, B, 2 * D))
+        _call("ddfa_mlp_dgrad_rescale", _p(dlogits), _p(saved.pooled), _p(saved.mlp_act), _p(mlp_ref[0]), _p(mlp_ref[1]),
+              ptr_array([_p(t) for t in params.mlp_w]), ptr_array([_p(t) for t in params.mlp_b]), B, D, nl, _p(dpooled), _p(scratch), st)
     elif dlogits is not None:
         if nl == 0:
             raise DdfaError("dlogits given but the module has no MLP head")

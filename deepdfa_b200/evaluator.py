@@ -15,10 +15,13 @@ object), graph ids of a :class:`~deepdfa_b200.arena.GraphArena` assembled inside
 Statement-level localisation (``statements=``): per batch, a score per node (CFG node = statement) and IVDetect's top-k statement
 metric over them (DDFA/sastvd/helpers/evaluate.py:262-322), added by ``ddfa_stmt_metric`` to a second fp64 state.  The scores are
 the node head's probability (node style), or, for the function logit of graph style, the readout's attention α_n, the saliency
-Σ_d |∂logit/∂x_{n,d}| or the integrated gradients Σ_d x_{n,d} · mean_k ∂logit/∂x_{n,d}(α_k x) of the embedding output x.
+Σ_d |∂logit/∂x_{n,d}|, the integrated gradients Σ_d x_{n,d} · mean_k ∂logit/∂x_{n,d}(α_k x), DeepLift / DeepLiftShap
+Σ_d (x − x̄)_{n,d} · g̃_{n,d} (g̃: the gradient with the MLP head's ReLUs under the rescale rule, against a baseline forward on x̄) or
+GradientShap's mean over samples of Σ_d (x̃ − b)_{n,d} · ∂logit/∂x_{n,d}(b + α(x̃ − b)), of the embedding output x.
 """
 from __future__ import annotations
 
+import numbers
 from typing import Optional
 
 import torch
@@ -35,7 +38,11 @@ TP, FP, TN, FN, SAMPLES, BATCHES, LOSS_W, WEIGHT, STORED, OVERFLOW = range(10)
 S_FUNCTIONS, S_VULN, S_HIT1, S_RANK_SUM, S_CLEAN, S_NAN, S_BATCHES = 0, 1, 2, 12, 13, 14, 15
 STMT_TOP_K = 10
 # statements= -> the label style it scores
-STATEMENT_MODES = {"probability": "node", "attention": "graph", "saliency": "graph", "integrated_gradients": "graph"}
+STATEMENT_MODES = {"probability": "node", "attention": "graph", "saliency": "graph", "integrated_gradients": "graph",
+                   "deeplift": "graph", "deeplift_shap": "graph", "gradient_shap": "graph"}
+# the modes that run the dgrad-only backward, and those whose default sample count is captum's / the reference's
+_GRADIENT_MODES = ("saliency", "integrated_gradients", "deeplift", "deeplift_shap", "gradient_shap")
+_SHAP_SAMPLES = {"deeplift_shap": 16, "gradient_shap": 5}
 
 
 def _ratio(num: float, den: float) -> float:
@@ -89,7 +96,8 @@ def statement_metrics_from_state(state, prefix: str = "val_", node_style: bool =
 class FusedEvaluator:
     def __init__(self, model: FlowGNNGGNNModule, use_cuda_graph: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
                  max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64,
-                 statements: Optional[str] = None, ig_steps: int = 50):
+                 statements: Optional[str] = None, ig_steps: int = 50, shap_samples: Optional[int] = None,
+                 baseline_stdev: float = 0.0, noise_stdev: float = 0.0, attribution_seed: int = 0):
         """``max_predictions`` > 0 keeps the first that many probabilities and labels (``predictions()``; the reference's
         ``test_preds`` / ``test_labels``); more samples than that make :meth:`compute` raise, the counts stay complete.
         ``bucket_nodes`` / ``bucket_edges``: shape bucketing of host batches under ``use_cuda_graph``, as in ``FusedTrainer``
@@ -102,7 +110,18 @@ class FusedEvaluator:
         ``Saliency(abs=True)``) or ``"integrated_gradients"`` (graph style: Σ_d x_{n,d} · (1/m) Σ_{k<m} ∂logit/∂x_{n,d} at
         ((k + ½)/m)·x, m = ``ig_steps``, zero baseline: captum's ``IntegratedGradients(method="riemann_middle")``).  The target is
         each function's own logit; one backward with dlogits = 1 serves every function of the batch.  None (the default)
-        enqueues nothing beyond the classification metrics."""
+        enqueues nothing beyond the classification metrics.
+        ``"deeplift"`` (graph style): captum's ``DeepLift(multiply_by_inputs=True)`` with a zero baseline x̄: Σ_d (x − x̄)_{n,d} ·
+        g̃_{n,d}, g̃ the input gradient with each hidden ReLU of the MLP head under the rescale rule — its derivative replaced by
+        (relu(z) − relu(z̄)) / (z − z̄), z̄ the pre-activation of a full forward of the same graph from x̄ — and every other
+        nonlinearity (GRU gates, pooling softmax, gate products) a plain gradient at the input pass's activations, as captum
+        hooks only ``nn.ReLU`` modules.  ``"deeplift_shap"``: captum's ``DeepLiftShap``, the mean of DeepLift over the baselines
+        b_j = ``baseline_stdev`` · ε_j, j < ``shap_samples`` (default 16); with ``baseline_stdev`` = 0 (the default) every baseline
+        is zero and DeepLift runs once, bit-identical to ``"deeplift"``.  ``"gradient_shap"``: captum's ``GradientShap``, the mean
+        over ``shap_samples`` (default 5) samples s of Σ_d (x̃ − b) · ∂logit/∂x at b + α(x̃ − b), x̃ = x + ``noise_stdev`` · ε,
+        b = ``baseline_stdev`` · ε' (zero by default) and α uniform in [0, 1) per function.  The draws are Philox4x32-10 with key
+        ``attribution_seed`` and a device batch counter (``ddfa_stmt_shap_input``, :attr:`attribution_draws`), advanced once per
+        batch these three modes attribute, so captured replays draw fresh values."""
         if model.device.type != "cuda":
             raise _lib.DdfaError("FusedEvaluator needs the module on a CUDA device (no CPU fallback)")
         hp = model.hparams
@@ -120,8 +139,23 @@ class FusedEvaluator:
                                  f"modules, this one has label_style={hp.label_style!r}")
         if int(ig_steps) < 1:
             raise ValueError(f"ig_steps must be >= 1, got {ig_steps!r}")
+        if shap_samples is not None and int(shap_samples) < 1:
+            raise ValueError(f"shap_samples must be >= 1, got {shap_samples!r}")
+        for name, v in (("baseline_stdev", baseline_stdev), ("noise_stdev", noise_stdev)):
+            if not float(v) >= 0.0 or float(v) == float("inf"):
+                raise ValueError(f"{name} must be a finite value >= 0, got {v!r}")
+        if float(baseline_stdev) > 0 and statements not in ("deeplift_shap", "gradient_shap"):
+            raise ValueError(f"baseline_stdev applies to statements='deeplift_shap' / 'gradient_shap', not {statements!r}")
+        if float(noise_stdev) > 0 and statements != "gradient_shap":
+            raise ValueError(f"noise_stdev applies to statements='gradient_shap', not {statements!r}")
+        if isinstance(attribution_seed, bool) or not isinstance(attribution_seed, numbers.Integral) or \
+                not 0 <= int(attribution_seed) < 2 ** 64:
+            raise ValueError(f"attribution_seed must be an integer in [0, 2**64), got {attribution_seed!r}")
         self.statements = statements
         self.ig_steps = int(ig_steps)
+        self.shap_samples = int(shap_samples) if shap_samples is not None else _SHAP_SAMPLES.get(statements, 1)
+        self.baseline_stdev, self.noise_stdev = float(baseline_stdev), float(noise_stdev)
+        self.attribution_seed = int(attribution_seed)
         self.module = model
         self.device = model.device
         self._node = hp.label_style == "node"
@@ -145,8 +179,12 @@ class FusedEvaluator:
             # the gradients the dgrad chain computes inline (MLP, gate, GRU biases / w_hh) land here, never in the module's .grad
             self._grad_scratch = E.ParamPack.from_flat_list([torch.zeros_like(p) for p in model.param_list()], len(model._tables()),
                                                             model._num_layers) if self._attributes else None
+            # the batch counter of the attribution draws (advanced once per attributed batch, inside a captured graph too)
+            self._draws = torch.zeros(1, dtype=torch.int64, device=dev)
         self._last_scores = None
         self.ws = E.Workspace(dev)
+        # DeepLift's baseline forwards keep their readout state here, apart from the input pass's saved state in self.ws
+        self._ref_ws = E.Workspace(dev) if statements in ("deeplift", "deeplift_shap") else None
         self._slots = {}
         self._graphs = {}
         self._warm_shapes = set()
@@ -156,7 +194,21 @@ class FusedEvaluator:
     # ---- the metric state ------------------------------------------------------------------------------------------------
     @property
     def _attributes(self) -> bool:
-        return self.statements in ("saliency", "integrated_gradients")
+        return self.statements in _GRADIENT_MODES
+
+    @property
+    def attribution_draws(self) -> int:
+        """Batches attributed so far by "deeplift", "deeplift_shap" or "gradient_shap" (the Philox batch counter of the next one).
+        Reading it synchronises.
+        Setting it writes the device word in stream order, so a run that restores it draws what an earlier run drew."""
+        return int(self._draws.item())
+
+    @attribution_draws.setter
+    def attribution_draws(self, value: int):
+        v = int(value)
+        if v < 0:
+            raise ValueError(f"attribution_draws must be >= 0, got {value!r}")
+        self._draws.fill_(v)
 
     def reset(self) -> None:
         """Zeroes the metric state and the statement state in stream order (the prediction store starts over at position 0)."""
@@ -297,10 +349,11 @@ class FusedEvaluator:
                 self._stmt_state.data_ptr(), self._stmt_ws.data_ptr(), self._stmt_ws.numel(), E._stream_ptr())
 
     def _attribute(self, params, dg, idx, scores) -> None:
-        """Saliency / integrated gradients of every function's logit with respect to the embedding output x: training-form
-        forwards and dgrad-only backwards (``grad_weights=False``) with dlogits = 1, the gradients of the weights going to a
-        scratch pack.  Integrated gradients start the m forwards from α_k·x (x: the inference forward's embedding output, still
-        in the workspace) and accumulate x·g / m."""
+        """Saliency / integrated gradients / DeepLift(Shap) / GradientShap of every function's logit with respect to the
+        embedding output x: training-form forwards and dgrad-only backwards (``grad_weights=False``) with dlogits = 1, the
+        gradients of the weights going to a scratch pack.  Integrated gradients start the m forwards from α_k·x (x: the
+        inference forward's embedding output, still in the workspace) and accumulate x·g / m; the others start them from the
+        rows ``ddfa_stmt_shap_input`` writes and accumulate (x̃ − b)·g over their samples."""
         m, ws = self.module, self.ws
         eng = _ENGINES[m.engine]
         T = m.hparams.n_steps
@@ -314,13 +367,46 @@ class FusedEvaluator:
                     E._p(scores), E._stream_ptr())
             return
         D = len(params.tables) * params.tables[0].shape[1]
-        x0 = ws.get("x", (N, D))             # written by the inference forward of this batch; no later pass writes "x"
-        steps = self.ig_steps
-        for k in range(steps):
-            _, _, saved = E.forward(params, dg, idx, T, training=True, engine=eng, alloc=ws, x_in=x0, x_scale=(k + 0.5) / steps)
-            dh, dxd = E.backward(params, dg, saved, self._grad_scratch, dlogits=ones, engine=eng, alloc=ws, grad_weights=False)
-            E._call("ddfa_stmt_input_grad_score", E._p(x0), E._p(dh), E._p(dxd), N, D, _lib.STMT_SCORE_X_TIMES, 1.0 / steps,
-                    int(k > 0), E._p(scores), E._stream_ptr())
+        x0 = ws.get("x", (N, D))             # written by the inference forward of this batch; later passes write the same rows or none
+        if self.statements == "integrated_gradients":
+            steps = self.ig_steps
+            for k in range(steps):
+                _, _, saved = E.forward(params, dg, idx, T, training=True, engine=eng, alloc=ws, x_in=x0, x_scale=(k + 0.5) / steps)
+                dh, dxd = E.backward(params, dg, saved, self._grad_scratch, dlogits=ones, engine=eng, alloc=ws, grad_weights=False)
+                E._call("ddfa_stmt_input_grad_score", E._p(x0), E._p(dh), E._p(dxd), N, D, _lib.STMT_SCORE_X_TIMES, 1.0 / steps,
+                        int(k > 0), E._p(scores), E._stream_ptr())
+            return
+        diff = ws.get("attr_diff", (N, D))
+
+        def shap_input(x_src, alpha, noise, sample):
+            def fill(out, image):
+                E._call("ddfa_stmt_shap_input", E._p(x_src), E._p(dg.graph_ptr), B, N, D, float(alpha), float(noise),
+                        self.baseline_stdev, self.attribution_seed, self._draws.data_ptr(), sample, E._p(out), E._p(diff),
+                        E._p(image), E._stream_ptr())
+            return fill
+
+        if self.statements == "gradient_shap":
+            # sample s: the plain gradient at b + α(x̃ − b) (x̃, b and α drawn), times x̃ − b
+            S = self.shap_samples
+            for s in range(S):
+                _, _, saved = E.forward(params, dg, idx, T, training=True, engine=eng, alloc=ws,
+                                        x_fill=shap_input(x0, -1.0, self.noise_stdev, s))
+                dh, dxd = E.backward(params, dg, saved, self._grad_scratch, dlogits=ones, engine=eng, alloc=ws, grad_weights=False)
+                E._call("ddfa_stmt_attribution_score", E._p(diff), E._p(dh), E._p(dxd), N, D, 1.0 / S, int(s > 0), E._p(scores),
+                        E._stream_ptr())
+        else:
+            # DeepLift: one input pass; per baseline a forward from it (GGNN in its inference form, readout state kept in _ref_ws)
+            # and the backward of the input pass with the head's ReLUs rescaled against it
+            _, _, saved = E.forward(params, dg, idx, T, training=True, engine=eng, alloc=ws)
+            J = self.shap_samples if self.statements == "deeplift_shap" and self.baseline_stdev > 0 else 1
+            for j in range(J):
+                _, _, ref = E.forward(params, dg, idx, T, training=True, grad_ggnn=False, engine=eng, alloc=self._ref_ws,
+                                      x_fill=shap_input(saved.x, 0.0, 0.0, j))
+                dh, dxd = E.backward(params, dg, saved, self._grad_scratch, dlogits=ones, engine=eng, alloc=ws, grad_weights=False,
+                                     mlp_ref=(ref.pooled, ref.mlp_act))
+                E._call("ddfa_stmt_attribution_score", E._p(diff), E._p(dh), E._p(dxd), N, D, 1.0 / J, int(j > 0), E._p(scores),
+                        E._stream_ptr())
+        self._draws.add_(1)
 
     def _slot(self, g):
         N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size

@@ -342,6 +342,16 @@ int ddfa_mlp_bwd(const float *dlogits, const float *pooled, const float *mlp_act
                  const float *const *mlp_w, int32_t num_graphs, int32_t dim, int32_t num_layers,
                  float *dpooled, float *const *dmlp_w, float *const *dmlp_b, float *scratch,
                  void *stream);
+/* MLP input gradient under DeepLift's rescale rule (captum DeepLift, the `nonlinear` rule at each nn.ReLU of the head):
+ * dlogits[B] -> dpooled[B,2D], no weight or bias gradient.  pooled / mlp_act are the input pass's (as ddfa_readout_mlp_fwd wrote
+ * them), pooled_ref / mlp_act_ref the reference (baseline) pass's.  At each hidden layer the pre-activations z, z' of both passes
+ * are recomputed from the layer's inputs (one GEMM each) and the derivative [z > 0] is replaced by
+ * (relu(z) - relu(z')) / (z - z'), or kept ([mlp_act > 0], the input pass's branch) where |z - z'| < 1e-10.  num_layers == 1: the
+ * dpooled of ddfa_mlp_bwd.  mlp_b: HOST array of num_layers device pointers (read for layers < num_layers - 1).
+ * scratch: fp32[4][B][2D]. */
+int ddfa_mlp_dgrad_rescale(const float *dlogits, const float *pooled, const float *mlp_act, const float *pooled_ref,
+                           const float *mlp_act_ref, const float *const *mlp_w, const float *const *mlp_b, int32_t num_graphs,
+                           int32_t dim, int32_t num_layers, float *dpooled, float *scratch, void *stream);
 /* Readout backward: dpooled[B,2D] -> dh_final[N,D], dx[N,D] (both overwritten);
  * accumulates dw_gate[2D], db_gate[1] (+=).  dpooled, pooled, h_final, x, w_gate, dh_final and dx
  * must be 16-byte aligned. */
@@ -540,6 +550,18 @@ int ddfa_eval_metrics_rows(const float *logits, const int32_t *vuln, const int32
  *   activation image as ddfa_act_to_image writes it: the start of a forward from a scaled embedding output.  One or two launches.
  * ddfa_stmt_node_probability: scores[n] = 1.f / (1.f + expf(-logits[n])) for n < S = *num_rows (clamped to [0, num_nodes]), 0
  *   beyond: the probabilities of ddfa_eval_metrics_rows when the rows are every valid node in order.  One launch.
+ * ddfa_stmt_attribution_score: score[n] = weight * sum_d diff[n, d] * (dh + dx)[n, d] (accumulate != 0: fmaf(weight, sum,
+ *   score[n])): the DDFA_STMT_SCORE_X_TIMES rule of ddfa_stmt_input_grad_score over a given difference tensor (x - baseline), the
+ *   same sums bit for bit.  One launch.
+ * ddfa_stmt_shap_input: the input of one DeepLift / GradientShap pass.  Per function b < num_graphs (nodes [graph_ptr[b],
+ *   graph_ptr[b+1])) and element (n, d): x~ = x + noise_stdev * eps, base = baseline_stdev * eps', diff = x~ - base and
+ *   input = fmaf(a_b, diff, base), with a_b = alpha when alpha >= 0 (0: the baseline itself) and otherwise drawn uniform in [0, 1).
+ *   The draws are Philox4x32-10 with key `seed` and counter (c0, c1, c2, c3) = (low word of *counter, sample, index, column
+ *   word): a_b = (w0 >> 8) * 2^-24 of (batch, sample, b, 0x80000000); eps of columns 4q..4q+3 of node n from the words of
+ *   (batch, sample, n, q) — for eps', q | 0x40000000 — by Box-Muller on the pairs (w0, w1), (w2, w3): r = sqrt(-2 ln u1),
+ *   u1 = ((w_a >> 8) + 1) 2^-24, u2 = (w_b >> 8) 2^-24, (r cos 2 pi u2, r sin 2 pi u2).  A stdev of 0 draws nothing.  *counter
+ *   (int64, device) is read, not advanced.  dim % 4 == 0; x, input and diff fp32 [N, dim], 16-byte aligned, not aliased.  When
+ *   image != NULL (dim == 128) input is also written as its activation image (ddfa_act_to_image).  One or two launches.
  * ------------------------------------------------------------------------------------- */
 #define DDFA_STMT_STATE_WORDS 16
 #define DDFA_STMT_MODE_VULN_ONLY 0
@@ -555,6 +577,11 @@ int ddfa_stmt_input_grad_score(const float *x, const float *dh, const float *dx,
                                float weight, int32_t accumulate, float *score, void *stream);
 int ddfa_stmt_scale_input(const float *x, float alpha, int32_t num_nodes, int32_t dim, float *out, void *image, void *stream);
 int ddfa_stmt_node_probability(const float *logits, const int32_t *num_rows, int32_t num_nodes, float *scores, void *stream);
+int ddfa_stmt_attribution_score(const float *diff, const float *dh, const float *dx, int32_t num_nodes, int32_t dim, float weight,
+                                int32_t accumulate, float *score, void *stream);
+int ddfa_stmt_shap_input(const float *x, const int32_t *graph_ptr, int32_t num_graphs, int32_t num_nodes, int32_t dim, float alpha,
+                         float noise_stdev, float baseline_stdev, uint64_t seed, const int64_t *counter, int32_t sample, float *input,
+                         float *diff, void *image, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * K10  torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 (DDFA/configs/
