@@ -83,7 +83,7 @@ int ddfa_debug_set(int key, int value) {
 
 int ddfa_debug_read(int key, void *host_out, size_t bytes) {
   DDFA_REQUIRE(host_out != nullptr, "ddfa_debug_read: null output");
-  switch (key) {   // [132 CTAs][12 tiles][12 events] int64 SM-clock stamps
+  switch (key) {   // [132 CTAs][12 tiles][16 events] int64 SM-clock stamps
     case 2: return ddfa::gru_tc2b_trace_read(host_out, bytes);    // dgrad3_kernel / bwd_step_fused_kernel / wgrad_kernel
     case 3: return ddfa::gru_tc3_trace_read(host_out, bytes);     // gru_fwd3_kernel
     case 4: {                                                     // int32: bounded-wait failures of the TMA-staged gather variants

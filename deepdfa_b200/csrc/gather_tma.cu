@@ -142,12 +142,17 @@ __global__ void __launch_bounds__(kWarps * 32) gather_sum_staged_kernel(const __
   }
 }
 
+static int *g_err_flag = nullptr;    // one int in device memory: bounded-wait failures of the last launches (development aid)
+
+}  // namespace gtma
+
 // cuTensorMapEncodeTiled through the runtime's driver entry point (libcuda is not linked)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-static int encode_row_map(const float *h, int32_t N, CUtensorMap *tm) {
+int tcc::encode_f32_rows_map(const float *base, int32_t rows, uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle,
+                             CUtensorMap *tm) {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     void *p = nullptr;
@@ -156,20 +161,15 @@ static int encode_row_map(const float *h, int32_t N, CUtensorMap *tm) {
     DDFA_REQUIRE(p != nullptr && q == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled is not available from this driver");
     fn = reinterpret_cast<EncodeTiledFn>(p);
   }
-  const cuuint64_t gdim[2] = {128, (cuuint64_t)N};
+  const cuuint64_t gdim[2] = {128, (cuuint64_t)rows};
   const cuuint64_t gstride[1] = {512};
-  const cuuint32_t box[2] = {128, 1};       // one row per copy
+  const cuuint32_t box[2] = {box_cols, box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult rc = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(h), gdim, gstride, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult rc = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), gdim, gstride, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   DDFA_REQUIRE(rc == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
   return DDFA_OK;
 }
-
-static int *g_err_flag = nullptr;    // one int in device memory: bounded-wait failures of the last launches (development aid)
-
-}  // namespace gtma
 
 int launch_gather_tma(int variant, const int32_t *indptr, const int32_t *indices, const float *h, int32_t N, float *out,
                       int accumulate, cudaStream_t stream) {
@@ -186,7 +186,7 @@ int launch_gather_tma(int variant, const int32_t *indptr, const int32_t *indices
     DDFA_CUDA(cudaFuncSetAttribute(gather_sum_staged_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     gather_sum_staged_kernel<0><<<blocks, kWarps * 32, kSmemBytes, stream>>>(tm, indptr, indices, h, N, out, accumulate, g_err_flag);
   } else {
-    int rc = encode_row_map(h, N, &tm);
+    int rc = tcc::encode_f32_rows_map(h, N, 128, 1, CU_TENSOR_MAP_SWIZZLE_NONE, &tm);      // one row per copy
     if (rc) return rc;
     DDFA_CUDA(cudaFuncSetAttribute(gather_sum_staged_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     gather_sum_staged_kernel<1><<<blocks, kWarps * 32, kSmemBytes, stream>>>(tm, indptr, indices, h, N, out, accumulate, g_err_flag);

@@ -417,6 +417,9 @@ int ddfa_gru_step_bwd_image_v2(const float *dh_out, const float *ds_prev, const 
   DDFA_REQUIRE(ds_prev == nullptr || (indptr_t && indices_t), "ddfa_gru_step_bwd_image_v2: ds_prev given without the transposed CSR");
   DDFA_REQUIRE(ds_prev == nullptr || ds_prev != ds, "ddfa_gru_step_bwd_image_v2: ds must not alias ds_prev");
   DDFA_REQUIRE(ds_prev == nullptr || ds_prev != dh, "ddfa_gru_step_bwd_image_v2: dh must not alias ds_prev");
+  // moved by TMA bulk and tensor-map copies, which address 16-byte units
+  DDFA_REQUIRE(aligned16(dh_out) && aligned16(ds) && aligned16(dh) && aligned16(gates_packed) && (h == nullptr || aligned16(h)),
+               "ddfa_gru_step_bwd_image_v2: dh_out, ds, dh, gates_packed and h must be 16-byte aligned");
   return gru_tc2_step_bwd(dh_out, ds_prev, indptr_t, indices_t, h, h_image, s_image, nullptr, gates_packed, indptr, N, ds, dh, dw_fold, db_fold,
                           db_ih, dw_hh, db_hh, workspace, workspace_bytes, wgrad_mode, as_stream(stream_));
 }

@@ -208,7 +208,7 @@ constexpr int kD3WChunkBytes = 64 * 128;                     // [64 columns x 64
 constexpr int kD3WBytes = 12 * kD3WChunkBytes;               // [g][hi|lo][kb] = 96 KB per (role, column half)
 constexpr int kD3OffStage = kD3WBytes;
 constexpr int kD3OffBar = kD3OffStage + kD3Stages * kD3StageBytes;   // 224 KB
-constexpr int kD3SmemAlloc = kD3OffBar + (2 * kD3Stages + 1) * 8 + 1024;   // + slack for the 1024-byte round-up below
+constexpr int kD3SmemAlloc = kD3OffBar + (2 * kD3Stages + 1) * 8 + 8 + 1024;   // barriers, one trace word; + slack for the 1024-byte round-up below
 constexpr int kD3Threads = 32 * kEpiWarps + 32;              // two consumer warpgroups + one producer warp
 constexpr size_t kD3PackedBytes = (size_t)4 * kD3WBytes;     // [role][column half] = 384 KB
 static_assert(kD3SmemAlloc <= 232448, "shared memory budget");
@@ -370,9 +370,9 @@ __global__ void __launch_bounds__(kD3Threads, 1) dgrad3_kernel(const uint8_t *__
 //   handover every writer fences its generic-proxy stores against the async proxy (the q tiles are read back by TMA, dh' * z
 //            is added to by bulk reductions), then the cluster barrier (arrive.release / wait.acquire);
 //   phase B  dgrad3_kernel's MMA loop, unchanged: the three q tiles of the role by bulk copy (L2 hits: written microseconds
-//            earlier), m64n64k16 bf16x3, the same MMA order.  The accumulator leaves through shared memory: ds by bulk copies,
-//            dh by bulk fp32 add-reductions onto dh' * z (one rounding to nearest, as the register add of the two-kernel path),
-//            so ds and dh are bit-identical to the two-kernel path.
+//            earlier), m64n64k16 bf16x3, the same MMA order.  The accumulator leaves through shared memory: ds by tensor-map
+//            stores, dh by tensor-map fp32 add-reductions onto dh' * z (one rounding to nearest, as the register add of the
+//            two-kernel path), so ds and dh are bit-identical to the two-kernel path.
 // The phase-A operands of a tile and the q tiles share the two 64 KB stages as one ring, four uses per tile (A, q0, q1, q2):
 // the next tile's phase-A copy goes into the stage that q1 releases, so it streams from HBM while phase B runs.  q2's stage
 // then holds the staged output until the end of the next tile's phase A, while its copies drain.
@@ -393,34 +393,33 @@ __device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.c
 __device__ __forceinline__ void mbar_arrive_n(uint32_t bar, uint32_t n) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory");
 }
-// Bulk copies shared -> global, tracked per issuing thread in bulk groups: a plain copy, and one that adds the fp32 values onto the
-// destination at L2 (UBLKRED.G.S.ADD.F32.RN: round to nearest even, and on the H100 subnormal inputs and results kept, the bits
-// of an fp32 register add in every probed case; DESIGN §3)
-__device__ __forceinline__ void bulk_s2g_hint(float *dst, uint32_t src, uint32_t bytes, uint64_t pol) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst), "r"(src), "r"(bytes), "l"(pol)
+// Tensor-map copies of one box shared -> global, tracked per issuing thread in bulk groups: a plain store, and one that adds the
+// fp32 values onto the destination at L2 (round to nearest even, subnormals kept: the bits of an fp32 register add; DESIGN §3).
+// Box rows past the map's row count are not written.
+__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap *tm, uint32_t src, int32_t x, int32_t y, uint64_t pol) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2}], [%3], %4;" ::"l"(tm), "r"(x), "r"(y),
+               "r"(src), "l"(pol)
                : "memory");
 }
-__device__ __forceinline__ void bulk_s2g_add_f32_hint(float *dst, uint32_t src, uint32_t bytes, uint64_t pol) {
-  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.L2::cache_hint.add.f32 [%0], [%1], %2, %3;" ::"l"(dst), "r"(src),
-               "r"(bytes), "l"(pol)
+__device__ __forceinline__ void tma_reduce_add_2d_hint(const CUtensorMap *tm, uint32_t src, int32_t x, int32_t y, uint64_t pol) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group.L2::cache_hint [%0, {%1, %2}], [%3], %4;" ::"l"(tm),
+               "r"(x), "r"(y), "r"(src), "l"(pol)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }   // sources read
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }             // writes done
 
-// Phase B's output goes out through the stage that held q2 (always stage 1: four ring uses per tile over two stages), as [64 rows
-// x 64 fp32] per warpgroup, rows padded from 256 to 272 bytes: the 8 rows of one warp store instruction start 4 banks apart, so
-// each bank is hit twice by the 256 bytes of a v2 store (the minimum).  Row r of warpgroup wg lies at (r / 16) x 16 KB + wg x 8 KB
-// + (r % 16) x 272 — inside the bytes of q2 that wg's own MMAs read (rows 64 wg .. 64 wg + 63 of each 16 KB chunk), so a
-// warpgroup may overwrite them as soon as all of its last MMAs have completed.
+// Phase B's output goes out through the stage that held q2 (always stage 1: four ring uses per tile over two stages).  Warpgroup
+// wg's [64 rows x 64 fp32] is two boxes of [64 rows x 32 fp32] in the SWIZZLE_128B layout of the ds / dh tensor maps: row r at
+// r x 128 bytes, its 16-byte unit u at (u ^ (r & 7)) x 16.  Box b lies at b x 16 KB + wg x 8 KB, 1024-byte aligned and inside the
+// bytes of q2 that wg's own MMAs read (rows 64 wg .. 64 wg + 63 of chunk b), so a warpgroup may overwrite them as soon as all of
+// its last MMAs have completed.  The 8 rows of one warp's v2 store cover all 8 unit positions twice: 2 wavefronts per 256 bytes.
 constexpr int kD3OutStage = 3 % kD3Stages;
 static_assert(4 % kD3Stages == 0, "q2 lands in the same stage every tile");
-constexpr int kStRowBytes = 64 * 4 + 16;
-static_assert(16 * kStRowBytes <= kChunkBytes / 2, "16 staged rows fit in a warpgroup's half of a chunk");
-__device__ __forceinline__ uint32_t staged_row(uint32_t stage, int wg, int r) {
-  return stage + (uint32_t)((r >> 4) * kChunkBytes + wg * (kChunkBytes / 2) + (r & 15) * kStRowBytes);
-}
+constexpr uint32_t kOutBoxCols = 32, kOutBoxRows = 64;
+static_assert(kOutBoxCols * 4 == 128 && kOutBoxRows * 128 == kChunkBytes / 2, "a box is one warpgroup's half of a chunk");
+constexpr int kD3OffPhaseAEnd = kD3OffBar + (2 * kD3Stages + 1) * 8;      // trace: SM clock at which the CTA's last warp ended phase A
 
 template <bool HF32, bool CSRP>
 __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const float *__restrict__ dh_out, const float *__restrict__ h,
@@ -428,7 +427,8 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
                                                                        const int32_t *__restrict__ indptr, const float *__restrict__ ds_in,
                                                                        const int32_t *__restrict__ indptr_t, const int32_t *__restrict__ indices_t,
                                                                        int32_t N, uint8_t *__restrict__ q_img, size_t img_stride,
-                                                                       const uint8_t *__restrict__ packed3, float *__restrict__ ds, float *__restrict__ dh,
+                                                                       const uint8_t *__restrict__ packed3, const __grid_constant__ CUtensorMap tm_ds,
+                                                                       const __grid_constant__ CUtensorMap tm_dh, float *__restrict__ dh,
                                                                        float *__restrict__ db_fold, float *__restrict__ db_ih, float *__restrict__ db_hh,
                                                                        float *__restrict__ bias_slots, int hints) {
   extern __shared__ uint8_t smem_raw[];
@@ -439,6 +439,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
   auto empty = [&](int i) { return bar0 + 8u * (kD3Stages + i); };
   const uint32_t w_full = bar0 + 8u * (2 * kD3Stages);
   const int tron = (g_trace_on == 1);
+  unsigned long long *phase_a_end = reinterpret_cast<unsigned long long *>(smem + kD3OffPhaseAEnd);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rh = blockIdx.x & 3, role = rh >> 1, half = rh & 1;      // rh = the CTA's rank in its cluster
@@ -452,6 +453,7 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
     for (int i = 0; i < kD3Stages; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), kEpiWarps); }
     mbar_init(w_full, 1);
     mbar_fence_init();
+    *phase_a_end = 0ull;
   }
   __syncthreads();
   if (threadIdx.x == 0) trace_stamp(tron, 0, 0);
@@ -648,7 +650,10 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
           split4(qnr, ph, pl); *reinterpret_cast<uint2 *>(q_img + 3 * img_stride + o_hi) = ph; *reinterpret_cast<uint2 *>(q_img + 3 * img_stride + o_lo) = pl;
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(empty(stage));      // this warp has read its rows of the stage
+        if (lane == 0) {
+          mbar_arrive(empty(stage));      // this warp has read its rows of the stage
+          if (tron) atomicMax(phase_a_end, (unsigned long long)clock64());      // clock64 only grows: no reset between tiles
+        }
       }
       // the previous tile's output has been read out of its stage (long ago: its copies drained during this phase A): hand the
       // stage back for this tile's first q copy, which the producer issues only after the handover below — four arrivals per
@@ -662,7 +667,10 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
       fence_proxy_async_global();
       cluster_arrive_release();
       cluster_wait_acquire();
-      if (tr) trace_stamp(tron, k, 11);      // 11: handover done
+      if (tr) {
+        trace_stamp(tron, k, 11);                                   // 11: handover done
+        trace_put(tron, k, 14, (long long)*(volatile unsigned long long *)phase_a_end);      // 14: the CTA's last warp ended phase A
+      }
       if ((warp & 3) == 0 && role == 1) fence_proxy_async_global();      // dh' * z (generic stores of the cluster) is added to by the async proxy
       // ---------------- phase B: dgrad3_kernel's loop ----------------
       if (k == 0) mbar_wait_bounded(w_full, 0);
@@ -696,35 +704,44 @@ __global__ void __launch_bounds__(kD3Threads, 1) bwd_step_fused_kernel(const flo
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (tr) { trace_stamp(tron, k, 6); trace_stamp(tron, k, 8); trace_stamp(tron, k, 9); }
-      // ds = acc; dh = acc + dh' * z, the elementwise term phase A wrote into dh's rows.  The fragment goes into q2's stage (see
-      // staged_row), then one bulk copy per row leaves the SM — for dh one that adds onto dh' * z in L2, so the SM never reads it
-      // back.  Rows >= N are never written: ds and dh are unpadded [N, 128] planes.
+      // ds = acc; dh = acc + dh' * z, the elementwise term phase A wrote into dh's rows.  The fragment goes into q2's stage as two
+      // swizzled boxes per warpgroup (see kOutBoxCols), then one tensor-map copy per box leaves the SM — for dh one that adds onto
+      // dh' * z in L2, so the SM never reads it back.  The maps end at row N: ds and dh are unpadded [N, 128] planes.
       const uint32_t st_base = sbase + kD3OffStage + kD3OutStage * kD3StageBytes;      // == pending
       // a warp's wait covers the rows of q2 its own MMAs read (16 per chunk); it stages into rows its siblings read
       if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
       else asm volatile("bar.sync 3, 128;" ::: "memory");
       uint32_t tid;      // re-read here: addresses derived from it and kept across the tile loop made the kernel spill
       asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+      // fragment row (tid >> 5 & 3) x 16 + (tid >> 2 & 7) + 8 hh; its row & 7 is tid >> 2 & 7.  Column 8 j + 2 (tid & 3) + e lies
+      // in box j / 4, unit 2 (j % 4) + (tid >> 1 & 1), byte 8 (tid & 1) + 4 e of the unit.
+      const uint32_t sw = ((tid >> 1 & 1) ^ (tid >> 2)) & 7;      // the unit's low bit and the row's swizzle, folded
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const uint32_t rowp = staged_row(st_base, wg, (tid >> 5 & 3) * 16 + (tid >> 2 & 7) + 8 * hh) + 8 * (tid & 3);
+        const uint32_t rowp = st_base + (tid >> 7) * (kChunkBytes / 2) + ((tid >> 5 & 3) * 16 + (tid >> 2 & 7) + 8 * hh) * 128 + 8 * (tid & 1);
 #pragma unroll
         for (int j = 0; j < 8; ++j)
-          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(rowp + 32 * j), "f"(acc[4 * j + 2 * hh]), "f"(acc[4 * j + 2 * hh + 1]) : "memory");
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(rowp + (j >> 2) * kChunkBytes + (((2 * (j & 3)) ^ sw) << 4)),
+                       "f"(acc[4 * j + 2 * hh]), "f"(acc[4 * j + 2 * hh + 1])
+                       : "memory");
       }
       fence_proxy_async_shared();
       if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");      // the warpgroup's 64 rows are staged
       else asm volatile("bar.sync 3, 128;" ::: "memory");
       if ((warp & 3) == 0 && elect_one()) {      // one thread per warpgroup issues its copies (uniform operands: straight-line issue)
-        const uint64_t pol_tmp = DDFA_POL_TMP;
-        const int64_t node0 = (int64_t)tile * kTileM + wg * 64;
-        float *out = (role == 0 ? ds : dh) + node0 * kD + half * 64;
-        const int rows = (int)min((int64_t)64, (int64_t)N - node0);
-        for (int r = 0; r < rows; ++r) {
-          if (role == 0) bulk_s2g_hint(out + (int64_t)r * kD, staged_row(st_base, wg, r), 64 * 4, pol_tmp);
-          else bulk_s2g_add_f32_hint(out + (int64_t)r * kD, staged_row(st_base, wg, r), 64 * 4, pol_tmp);
+        const int32_t y = tile * kTileM + wg * 64;
+        if (y < N) {      // the map clips a partial box; a box wholly past N is not issued
+          const uint64_t pol_tmp = DDFA_POL_TMP;
+          const uint32_t src = st_base + wg * (kChunkBytes / 2);
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {
+            const int32_t x = half * 64 + b * (int)kOutBoxCols;
+            if (role == 0) tma_store_2d_hint(&tm_ds, src + b * kChunkBytes, x, y, pol_tmp);
+            else tma_reduce_add_2d_hint(&tm_dh, src + b * kChunkBytes, x, y, pol_tmp);
+          }
         }
         bulk_commit();
+        trace_stamp(tron, k, 12 + wg);      // 12 / 13: warpgroup 0 / 1 has issued its copies
       }
       __syncwarp();
       if (tr) trace_stamp(tron, k, 10);
@@ -1006,11 +1023,16 @@ static int launch_bwd_fused(int tiles, cudaStream_t stream, const float *dh_out,
   *ctas = clusters * 4;
   DDFA_REQUIRE(bias_slots == nullptr || *ctas <= tc2b::kBiasSlots, "tcgen05 engine (bwd): %d CTAs exceed the %d bias-gradient slots",
                *ctas, tc2b::kBiasSlots);
+  // ds and dh leave the kernel as [64 x 32] boxes; encoded per call, so a captured graph keeps the addresses of its capture
+  CUtensorMap tm_ds, tm_dh;
+  int rc_map = tcc::encode_f32_rows_map(ds, N, tc2b::kOutBoxCols, tc2b::kOutBoxRows, CU_TENSOR_MAP_SWIZZLE_128B, &tm_ds);
+  if (rc_map == DDFA_OK) rc_map = tcc::encode_f32_rows_map(dh, N, tc2b::kOutBoxCols, tc2b::kOutBoxRows, CU_TENSOR_MAP_SWIZZLE_128B, &tm_dh);
+  if (rc_map != DDFA_OK) return rc_map;
   DDFA_CUDA(cudaFuncSetAttribute(tc2b::bwd_step_fused_kernel<HF32, CSRP>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2b::kD3SmemAlloc));
   DDFA_CUDA(launch_chain_cluster(4, 4, tc2b::bwd_step_fused_kernel<HF32, CSRP>, dim3(clusters * 4), dim3(tc2b::kD3Threads), tc2b::kD3SmemAlloc,
                                  stream, dh_out, h, static_cast<const uint8_t *>(h_img_in), static_cast<const uint2 *>(gates_packed), indptr,
-                                 ds_in, ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, packed, ds, dh, db_fold, db_ih, db_hh, bias_slots,
-                                 l2_hints()));
+                                 ds_in, ds_in ? indptr_t : nullptr, indices_t, N, q_img, img, packed, tm_ds, tm_dh, dh, db_fold, db_ih, db_hh,
+                                 bias_slots, l2_hints()));
   DDFA_CHECK_LAUNCH("tc2b::bwd_step_fused_kernel");
   return DDFA_OK;
 }

@@ -9,12 +9,18 @@
 //   exactly the bytes of the fp32 matrix — so producer kernels write it instead of / next to fp32 and the GEMM
 //   kernels stream it with plain 1-D TMA bulk copies (no in-kernel conversion pass).
 #pragma once
+#include <cuda.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 
 namespace ddfa {
 namespace tcc {
+
+// gather_tma.cu: the tensor map of an fp32 [rows, 128] row-major plane (512-byte rows) with a box of box_cols x box_rows elements,
+// encoded on the host (cuTensorMapEncodeTiled through the runtime's driver entry point).  Loads fill rows past `rows` with zeros;
+// stores and reductions skip them.
+int encode_f32_rows_map(const float *base, int32_t rows, uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle, CUtensorMap *tm);
 
 constexpr int kD = 128;
 constexpr int kTileM = 128;
@@ -242,14 +248,14 @@ __device__ __forceinline__ float fast_tanh(float x) {
 
 // ---- pipeline timeline (development aid; ddfa_debug_set key 2 switches it on, ddfa_debug_read fetches it) -----------
 // Each translation unit that includes this header gets its own buffer: [CTA][tile][event] SM-clock stamps.
-constexpr int kTraceCtas = 132, kTraceTiles = 12, kTraceEvents = 12;
+constexpr int kTraceCtas = 132, kTraceTiles = 12, kTraceEvents = 16;
 constexpr size_t kTraceWords = (size_t)kTraceCtas * kTraceTiles * kTraceEvents;
 static __device__ long long g_trace[kTraceWords];
 static __device__ int g_trace_on = 0;
-__device__ __forceinline__ void trace_stamp(int on, int tile_i, int ev) {
-  if (on && blockIdx.x < kTraceCtas && tile_i < kTraceTiles)
-    g_trace[((size_t)blockIdx.x * kTraceTiles + tile_i) * kTraceEvents + ev] = clock64();
+__device__ __forceinline__ void trace_put(int on, int tile_i, int ev, long long v) {
+  if (on && blockIdx.x < kTraceCtas && tile_i < kTraceTiles) g_trace[((size_t)blockIdx.x * kTraceTiles + tile_i) * kTraceEvents + ev] = v;
 }
+__device__ __forceinline__ void trace_stamp(int on, int tile_i, int ev) { trace_put(on, tile_i, ev, clock64()); }
 
 }  // namespace tcc
 }  // namespace ddfa

@@ -12,7 +12,11 @@ call from the kernel's SM-clock stamps (ddfa_debug_set(2, 1)), averaged over eve
   handover -> first q    waiting for the first q tile of phase B (event 4)
   first q -> last MMAs   the dgrad MMAs (events 6 / 8)
   accumulator -> end     the ds / dh epilogue (event 9 -> event 10)
-  period                 iteration end to iteration end"""
+  period                 iteration end to iteration end
+and where phase A and the epilogue's copy issue end:
+  start -> last phase A  the CTA's last warp has read its phase-A rows (event 14, an atomic max over the warps)
+  last phase A -> handover   the cluster barrier: the other CTAs' phase A and the q / dh' * z stores made visible
+  accumulator -> issued (wg 0 / wg 1)   warpgroup 0 / 1 has issued its ds / dh copies (events 12 / 13)"""
 import argparse
 import ctypes
 import json
@@ -30,7 +34,7 @@ from deepdfa_b200.engine import _p, prepare_graph  # noqa: E402
 
 DEV, D = "cuda:0", 128
 KEEP0 = 16                     # DDFA_WGRAD_KEEP(0): keep the q images, no weight-gradient launch inside the call
-CT, TL, EV = 132, 12, 12       # the trace buffer: [CTA][tile][event] (tc_common.cuh)
+CT, TL, EV = 132, 12, 16       # the trace buffer: [CTA][tile][event] (tc_common.cuh)
 
 
 def card():
@@ -45,7 +49,9 @@ def phases(t):
     ok = (t[:, k, 10] != 0) & (t[:, k - 1, 10] != 0)
     spans = {"start_to_handover": t[:, k, 11] - t[:, k - 1, 10], "handover_to_first_q": t[:, k, 4] - t[:, k, 11],
              "first_q_to_last_mmas": t[:, k, 6] - t[:, k, 4], "accumulator_to_end": t[:, k, 10] - t[:, k, 9],
-             "period": t[:, k, 10] - t[:, k - 1, 10]}
+             "period": t[:, k, 10] - t[:, k - 1, 10],
+             "start_to_last_phase_a": t[:, k, 14] - t[:, k - 1, 10], "last_phase_a_to_handover": t[:, k, 11] - t[:, k, 14],
+             "accumulator_to_issued_wg0": t[:, k, 12] - t[:, k, 9], "accumulator_to_issued_wg1": t[:, k, 13] - t[:, k, 9]}
     return {n: round(float(v[ok].mean()), 0) for n, v in spans.items()}, int(ok.sum())
 
 

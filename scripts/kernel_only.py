@@ -61,7 +61,7 @@ print("done", which, N)
 
 def dump_trace(key, label):
     import numpy as np
-    CT, TL, EV = 132, 12, 12
+    CT, TL, EV = 132, 12, 16
     buf = np.zeros(CT * TL * EV, dtype=np.int64)
     L.call("ddfa_debug_read", key, buf.ctypes.data, buf.nbytes)
     t = buf.reshape(CT, TL, EV).astype(np.float64)
@@ -111,9 +111,9 @@ if os.environ.get("DDFA_TRACE"):
                N, D, _p(ds), _p(dh), _p(acc[0]), _p(acc[1]), _p(acc[2]), _p(acc[3]), _p(acc[4]), _p(ws), wsb, 2, st)
         torch.cuda.synchronize()
         import numpy as np
-        buf = np.zeros(132 * 12 * 12, dtype=np.int64)
+        buf = np.zeros(132 * 12 * 16, dtype=np.int64)
         L.call("ddfa_debug_read", 2, buf.ctypes.data, buf.nbytes)
-        t = buf.reshape(132, 12, 12).astype(np.float64) / GHZ
+        t = buf.reshape(132, 12, 16).astype(np.float64) / GHZ
         print("---- wgrad_kernel (gate block 0 of dW'): ns since kernel start: B issue | A issue | B landed | A landed | A landed | tile MMAs issued")
         for cta in (0, 1, 11, 21):
             t0 = t[cta, 0, 0]
