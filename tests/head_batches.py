@@ -361,3 +361,85 @@ def sampler_cases():
     cases.append(("c1_tie_a", t["vuln"], len(t["vuln"]), t["factor_a"], t["seed"], 0))
     cases.append(("c1_tie_ab", t["vuln"], len(t["vuln"]), t["factor_ab"], t["seed"], 0))
     return cases
+
+
+# ---- node-style head (node_loss.cu: ddfa_node_head_fwd / _bwd) ----------------------------------------------------------------
+NODE_HEAD_BM, NODE_HEAD_BK = 64, 16     # head_gemm_kernel: 64-row tiles, K in steps of 16 (a ragged last step when 2D % 16 != 0)
+NODE_HEAD_CHUNKS = 32                   # kHeadChunks: row chunks of the weight / bias gradient, added in chunk order
+NODE_HEAD_WARP_ROWS = 8                 # head_out_kernel: a warp per row, 8 rows per CTA
+NODE_HEAD_WIDTHS = (20, 32, 64, 128, 192, 256, 320, 384, 448, 512)    # D: the SIMT widths and the tensor-core wide widths
+NODE_SMALL_S = (0, 1, 5, 31, 32, 33, -1)                              # row counts at the hub node count; -1: every node
+NODE_VULN_RATE, NODE_FACTOR = 0.15, 1.0                               # the C1 row list: every vulnerable node + as many others
+
+
+def node_head_chunks(S: int):
+    """The rows [r0, r1) of each weight-gradient chunk (head_wgrad_kernel / head_bias_partial_kernel): ceil(S / 32) rows each."""
+    c = -(-S // NODE_HEAD_CHUNKS)
+    return [(min(S, i * c), min(S, min(S, i * c) + c)) for i in range(NODE_HEAD_CHUNKS)]
+
+
+def node_head_ws_bytes(N: int, D: int) -> int:
+    """ddfa_node_head_bwd_workspace_bytes: two [N, 2D] planes and 32 chunk partials of a [2D, 2D] gradient plus its bias."""
+    K = 2 * D
+    return 4 * (2 * N * K + NODE_HEAD_CHUNKS * (K * K + K))
+
+
+def node_rows_trainer(N: int, seed: int) -> np.ndarray:
+    """A row list as FusedTrainer draws it (sample_ref: every vulnerable node plus rint(n_vuln * factor) non-vulnerable ones by
+    Philox key), over NODE_VULN_RATE labels with node 0 and node N - 1 vulnerable, so both ends of the planes are in it."""
+    vuln = (np.random.default_rng(seed).random(N) < NODE_VULN_RATE).astype(np.int32)
+    vuln[[0, N - 1]] = 1
+    return sample_ref(vuln, N, NODE_FACTOR, seed, 0)[0]
+
+
+def node_rows(N: int, S: int, seed: int) -> np.ndarray:
+    """S sorted unique rows of N (S < 0: all of them); node N - 1 first, then node 0, then random ones."""
+    if S < 0 or S >= N:
+        return np.arange(N, dtype=np.int32)
+    fixed = [N - 1, 0][:S]
+    rest = np.random.default_rng(seed).choice(np.arange(1, N - 1), max(S - len(fixed), 0), replace=False)
+    return np.sort(np.concatenate([fixed, rest])).astype(np.int32)
+
+
+def node_head_ref(ins0, acts, ws, bs, dl, dw0, db0):
+    """The node head's forward and backward in float64 from the kernel's own fp32 inputs to each stage, with every hidden ReLU on
+    the side of its kink the kernel's forward took (mask = act > 0): the autograd of [h | x][rows] -> Linear/ReLU ... ->
+    Linear(2D, 1) with relu(z) read as z * mask.  ins0: [S, 2D] gathered rows; acts: the kernel's hidden activations [S, 2D]
+    each; dl: [S] dlogits; dw0 / db0: the gradients' start values (the kernel accumulates).
+
+    Returns name -> (ref, mag, tau) with |got - ref| <= tau * mag the a-priori bound of each output (u = 2^-24, every count
+    doubled as in linear_ref): mag is the same computation on absolute values.  Forward: a length-(K + 1) dot product
+    (2 (K + 1) u).  Backward: the error of the incoming gradient (its own tau, carried by the absolute-value chain) plus, for
+    dIn, a length-K dot product (or one product for the last layer), and for dW / db a ceil(S / 32)-row chunk sum, the 32-way
+    chunk reduction and the add onto the start value (2 (ceil(S / 32) + 34) u)."""
+    L = len(ws)
+    K = ins0.shape[1]
+    S = ins0.shape[0]
+    chunk = -(-S // NODE_HEAD_CHUNKS)
+    f64 = lambda t: t.double()
+    ins = [f64(ins0)] + [f64(a) for a in acts]
+    masks = [f64(a > 0) for a in acts]
+    out = {}
+    fwd_tau = 2 * (K + 1) * U
+    for i in range(L):
+        W, b = f64(ws[i]), f64(bs[i])
+        z = ins[i] @ W.t() + b
+        mag = ins[i].abs() @ W.abs().t() + b.abs()
+        if i < L - 1:
+            out[f"act{i}"] = (torch.relu(z), mag, fwd_tau)
+        else:
+            out["logits"] = (z[:, 0], mag[:, 0], fwd_tau)
+    g, gmag, gtau = f64(dl)[:, None], f64(dl).abs()[:, None], 0.0
+    w_tau = 2 * (chunk + 34) * U
+    for i in range(L - 1, -1, -1):
+        W = f64(ws[i])
+        dw = g.t() @ ins[i] + f64(dw0[i])
+        dwm = gmag.t() @ ins[i].abs() + f64(dw0[i]).abs()
+        out[f"dw{i}"] = (dw, dwm, gtau + w_tau)
+        out[f"db{i}"] = (g.sum(0) + f64(db0[i]), gmag.sum(0) + f64(db0[i]).abs(), gtau + w_tau)
+        step = 2 * U if i == L - 1 else 2 * (K + 1) * U          # dlogits[s] * w[k] (one product) or a length-K dot product
+        g, gmag, gtau = g @ W, gmag @ W.abs(), gtau + step
+        if i > 0:
+            g, gmag = g * masks[i - 1], gmag * masks[i - 1]
+    out["din"] = (g, gmag, gtau)
+    return out

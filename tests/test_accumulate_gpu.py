@@ -8,6 +8,7 @@ sum and skips a non-finite window whole; frozen tensors stay put; an LR schedule
 flush() applies a partial window; and with two GPUs the exchange runs once per window."""
 import contextlib
 import copy
+import gc
 import math
 import os
 import socket
@@ -67,8 +68,11 @@ def assert_same(a, b):
 
 
 def cuda_kernels(fn):
-    """The names of the device activities ``fn`` enqueues (sorted) and the library's launch count over it."""
+    """The names of the device activities ``fn`` enqueues (sorted) and the library's launch count over it.  Earlier work
+    finishes and the garbage earlier tests left is collected first, so neither is recorded in the window."""
     from torch.profiler import ProfilerActivity, profile
+    gc.collect()
+    torch.cuda.synchronize()
     n0 = lib().call("ddfa_launch_count")
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
         fn()
@@ -91,7 +95,8 @@ def test_k1_enqueues_what_the_trainer_without_the_argument_enqueues(style):
         tr = D.FusedTrainer(module(style, factor=1.0), **kw)
         assert tr._acc is None and tr.accumulated == 0
         tr.step(b)                                            # warm-up: workspace growth
-        names, launches = cuda_kernels(lambda: tr.step(b))
+        tr.step(b)                                            # capture (its gc.collect / empty_cache stay out of the window)
+        names, launches = cuda_kernels(lambda: tr.step(b))    # the step every later step replays
         assert tr.accumulated == 0
         seen.append((names, launches))
     assert seen[0][1] > 0 and seen[0] == seen[1]

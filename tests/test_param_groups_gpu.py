@@ -10,6 +10,7 @@ coupled group over everything gives the default trainer's bits with the guard, a
 runs repeat; and without the new arguments the step enqueues the kernels it always did."""
 import contextlib
 import copy
+import gc
 import os
 import socket
 
@@ -456,8 +457,10 @@ def test_deterministic_adamw_runs_are_bit_identical(style):
 
 def cuda_kernels(fn):
     """The names of the device activities ``fn`` enqueues (sorted) and the library's launch count over it.  Work enqueued
-    before the call finishes first, so none of it is recorded in the window."""
+    before the call finishes first, so none of it is recorded in the window, and the garbage earlier tests left is collected
+    first, so none of it is released inside the window."""
     from torch.profiler import ProfilerActivity, profile
+    gc.collect()
     torch.cuda.synchronize()
     n0 = lib().call("ddfa_launch_count")
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
@@ -474,7 +477,8 @@ def test_without_the_arguments_the_step_enqueues_what_it_did(style):
     for kw in ({}, {"param_groups": None, "decoupled_weight_decay": False}, {"decoupled_weight_decay": True}):
         tr = D.FusedTrainer(module(style=style, factor=1.0), **kw)
         tr.step(b)                                            # warm-up: workspace growth
-        seen.append(cuda_kernels(lambda: tr.step(b)))
+        tr.step(b)                                            # capture (its gc.collect / empty_cache stay out of the window)
+        seen.append(cuda_kernels(lambda: tr.step(b)))         # the step every later step replays
     assert seen[0][1] > 0 and seen[0] == seen[1]
     assert any("adam_flat_kernel" in n for n in seen[0][0]) and not any("adam_flat_groups" in n for n in seen[0][0])
     # AdamW swaps the one update kernel for its grouped form and launches no more
