@@ -34,7 +34,7 @@ class ArenaBatch(BatchedCFG):
         empty = torch.empty(0, dtype=torch.int64, device=dg.device)
         super().__init__(empty, empty, bnn, ndata, None, num_nodes=dg.num_nodes)
         self._dg = dg
-        self._ws = ws                      # workspace of the producing call: [edge_ptr int32[B+1]][error counter int32]
+        self._ws = ws                      # workspace of the producing call: [edge_ptr int32[B+1]][error counter int32][node_ptr int32[B+1]]
         self._coo = None
         self._cache[f"devgraph:{dg.device}:1"] = dg
 
@@ -103,6 +103,8 @@ class GraphArena:
         big = BG.batch(singles)
         if big.num_nodes() >= 2 ** 31 or big.num_edges() >= 2 ** 31:
             raise ValueError("GraphArena: more than 2^31 nodes or edges")
+        if len([k for k in big.ndata if k != "_VULN"]) > 8:
+            raise ValueError("GraphArena: at most 8 node-feature vectors")
         nodes = big.batch_num_nodes().cpu().numpy().astype(np.int64)
         edges = big.batch_num_edges().cpu().numpy().astype(np.int64)
         dg = E.prepare_graph(big.to(device), device, need_transpose=True)
@@ -116,8 +118,6 @@ class GraphArena:
                 feats[k] = v.to(device).to(torch.int64).contiguous()
         if vuln is None:
             vuln = torch.zeros(big.num_nodes(), dtype=torch.int32, device=device)
-        if len(feats) > 8:
-            raise ValueError("GraphArena: at most 8 node-feature vectors")
         return cls(dg, node_off.to(device), feats, vuln, nodes, edges)
 
     @property

@@ -152,20 +152,28 @@ def batch(graphs: Sequence[BatchedCFG]) -> BatchedCFG:
 def unbatch(g: BatchedCFG, node_split=None) -> List[BatchedCFG]:
     """``dgl.unbatch`` (reference ``base_module.py:87``). Kept for compatibility; the CUDA path
     never unbatches (labels are a fused segment-max)."""
-    bnn = g.batch_num_nodes().tolist()
-    bne = g.batch_num_edges().tolist()
-    out = []
-    n0 = e0 = 0
-    # edges of a batched graph are grouped per graph only if it came from batch(); handle the general case
+    bnn_t = g.batch_num_nodes().cpu().to(torch.int64)
+    bnn = bnn_t.tolist()
+    B = len(bnn)
+    # edges of a batched graph are grouped per graph only if it came from batch(); handle the general case: an edge belongs to
+    # the graph that owns its dst (dst past the last node: to none), and one stable sort keeps each graph's edges in their order
     src, dst = g.edges()
-    ptr = torch.tensor([0] + bnn).cumsum(0)
+    ptr = torch.zeros(B + 1, dtype=torch.int64)
+    torch.cumsum(bnn_t, 0, out=ptr[1:])
     gid = torch.bucketize(dst.cpu().to(torch.int64), ptr[1:], right=True)
-    for b, (nn_, ne_) in enumerate(zip(bnn, bne)):
-        sel = (gid == b).nonzero().squeeze(-1).to(src.device)
+    bne_t = torch.bincount(gid, minlength=B + 1)[:B]
+    owned = int(bne_t.sum())
+    order = torch.sort(gid, stable=True).indices[:owned].to(src.device)
+    shift = torch.repeat_interleave(ptr[:-1], bne_t).to(device=src.device, dtype=src.dtype)   # first node of each edge's graph
+    src, dst = src[order] - shift, dst[order] - shift.to(dst.dtype)
+    eptr = [0] + bne_t.cumsum(0).tolist()
+    n0 = 0
+    out = []
+    for b, nn_ in enumerate(bnn):
+        e0, e1 = eptr[b], eptr[b + 1]
         nd = {k: v[n0:n0 + nn_] for k, v in g.ndata.items()}
-        out.append(BatchedCFG(src[sel] - n0, dst[sel] - n0, torch.tensor([nn_]), nd, torch.tensor([int(sel.numel())])))
+        out.append(BatchedCFG(src[e0:e1], dst[e0:e1], bnn_t[b:b + 1], nd, bne_t[b:b + 1], num_nodes=nn_))
         n0 += nn_
-        e0 += ne_
     return out
 
 

@@ -18,12 +18,13 @@ struct ArenaFeats {                     // device pointers, passed by value
   int64_t *out[kArenaMaxFeats];
 };
 
-// ws layout: int32 edge_ptr[B + 1], int32 err
+// ws layout: int32 edge_ptr[B + 1], int32 err, int32 node_ptr[B + 1].  The scan writes only the workspace: whether an id was bad
+// or the totals disagree is known after its last pass, so the outputs (graph_ptr included) are written by the assembler, which
+// runs only when err == 0.
 __global__ void __launch_bounds__(1024) arena_scan_kernel(const int32_t *__restrict__ ids, int32_t B, int32_t G,
                                                           const int32_t *__restrict__ node_off, const int32_t *__restrict__ indptr,
-                                                          int32_t n_expect, int32_t e_expect, int32_t *__restrict__ graph_ptr,
-                                                          int32_t *__restrict__ edge_ptr, int32_t *__restrict__ out_indptr,
-                                                          int32_t *__restrict__ out_indptr_t, int32_t *__restrict__ err) {
+                                                          int32_t n_expect, int32_t e_expect, int32_t *__restrict__ node_ptr,
+                                                          int32_t *__restrict__ edge_ptr, int32_t *__restrict__ err) {
   __shared__ int32_t sn[32], se[32];
   __shared__ int32_t carry_n, carry_e;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -62,19 +63,15 @@ __global__ void __launch_bounds__(1024) arena_scan_kernel(const int32_t *__restr
     __syncthreads();
     const int32_t pn = carry_n + (warp ? sn[warp - 1] : 0) + xn - n;     // exclusive prefix
     const int32_t pe = carry_e + (warp ? se[warp - 1] : 0) + xe - e;
-    if (b < B) { graph_ptr[b] = pn; edge_ptr[b] = pe; }
+    if (b < B) { node_ptr[b] = pn; edge_ptr[b] = pe; }
     __syncthreads();
     if (threadIdx.x == 1023) { carry_n += sn[31]; carry_e += se[31]; }
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    graph_ptr[B] = carry_n;
+    node_ptr[B] = carry_n;
     edge_ptr[B] = carry_e;
     if (carry_n != n_expect || carry_e != e_expect) atomicAdd(err, 1 << 16);   // host-side totals disagree with the arena
-    else {
-      out_indptr[carry_n] = carry_e;
-      out_indptr_t[carry_n] = carry_e;
-    }
   }
 }
 
@@ -82,17 +79,24 @@ __global__ void __launch_bounds__(128) arena_assemble_kernel(const int32_t *__re
                                                              const int32_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                                                              const int32_t *__restrict__ indptr_t, const int32_t *__restrict__ indices_t,
                                                              const ArenaFeats feats, int32_t K,
-                                                             const int32_t *__restrict__ vuln, const int32_t *__restrict__ graph_ptr,
+                                                             const int32_t *__restrict__ vuln, const int32_t *__restrict__ node_ptr,
                                                              const int32_t *__restrict__ edge_ptr, const int32_t *__restrict__ err,
-                                                             int32_t *__restrict__ out_indptr, int32_t *__restrict__ out_indices,
-                                                             int32_t *__restrict__ out_indptr_t, int32_t *__restrict__ out_indices_t,
-                                                             int32_t *__restrict__ out_vuln) {
+                                                             int32_t *__restrict__ out_graph_ptr, int32_t *__restrict__ out_indptr,
+                                                             int32_t *__restrict__ out_indices, int32_t *__restrict__ out_indptr_t,
+                                                             int32_t *__restrict__ out_indices_t, int32_t *__restrict__ out_vuln) {
   if (*err != 0) return;                      // bad id or inconsistent totals: leave the outputs alone, the host reports it
   const int b = blockIdx.x;
   const int32_t id = ids[b];
   const int32_t n0 = node_off[id], n = node_off[id + 1] - n0;
   const int32_t e0 = indptr[n0], e0t = indptr_t[n0], ne = indptr[n0 + n] - e0;
-  const int32_t o = graph_ptr[b], eo = edge_ptr[b];
+  const int32_t o = node_ptr[b], eo = edge_ptr[b];
+  if (threadIdx.x == 0) out_graph_ptr[b] = o;
+  if (b == (int)gridDim.x - 1 && threadIdx.x == 0) {   // the sentinels: graph_ptr[B] = N, indptr[N] = indptr_t[N] = E
+    const int32_t N = node_ptr[b + 1], E = edge_ptr[b + 1];
+    out_graph_ptr[b + 1] = N;
+    out_indptr[N] = E;
+    out_indptr_t[N] = E;
+  }
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     out_indptr[o + i] = indptr[n0 + i] - e0 + eo;
     out_indptr_t[o + i] = indptr_t[n0 + i] - e0t + eo;
@@ -112,7 +116,7 @@ __global__ void __launch_bounds__(128) arena_assemble_kernel(const int32_t *__re
 
 extern "C" {
 
-size_t ddfa_arena_batch_workspace_bytes(int32_t batch_size) { return sizeof(int32_t) * ((size_t)(batch_size < 0 ? 0 : batch_size) + 2); }
+size_t ddfa_arena_batch_workspace_bytes(int32_t batch_size) { return sizeof(int32_t) * (2 * (size_t)(batch_size < 0 ? 0 : batch_size) + 3); }
 
 int ddfa_arena_batch(const int32_t *graph_ids, int32_t batch_size, int32_t num_graphs, const int32_t *node_off, const int32_t *indptr,
                      const int32_t *indices, const int32_t *indptr_t, const int32_t *indices_t, const int64_t *const *feats,
@@ -138,13 +142,14 @@ int ddfa_arena_batch(const int32_t *graph_ids, int32_t batch_size, int32_t num_g
   cudaStream_t stream = as_stream(stream_);
   int32_t *edge_ptr = static_cast<int32_t *>(workspace);
   int32_t *err = edge_ptr + batch_size + 1;
+  int32_t *node_ptr = err + 1;
   DDFA_CUDA(cudaMemsetAsync(err, 0, sizeof(int32_t), stream));
-  arena_scan_kernel<<<1, 1024, 0, stream>>>(graph_ids, batch_size, num_graphs, node_off, indptr, batch_nodes, batch_edges, out_graph_ptr, edge_ptr,
-                                            out_indptr, out_indptr_t, err);
+  arena_scan_kernel<<<1, 1024, 0, stream>>>(graph_ids, batch_size, num_graphs, node_off, indptr, batch_nodes, batch_edges, node_ptr, edge_ptr,
+                                            err);
   DDFA_CHECK_LAUNCH("arena_scan_kernel");
   arena_assemble_kernel<<<batch_size, 128, 0, stream>>>(graph_ids, num_graphs, node_off, indptr, indices, indptr_t, indices_t, fp, num_feats,
-                                                        vuln, out_graph_ptr, edge_ptr, err, out_indptr, out_indices, out_indptr_t, out_indices_t,
-                                                        out_vuln);
+                                                        vuln, node_ptr, edge_ptr, err, out_graph_ptr, out_indptr, out_indices, out_indptr_t,
+                                                        out_indices_t, out_vuln);
   DDFA_CHECK_LAUNCH("arena_assemble_kernel");
   return DDFA_OK;
 }

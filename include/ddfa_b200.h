@@ -115,8 +115,10 @@ int ddfa_graph_ptr(const int64_t *batch_num_nodes, int32_t num_graphs, int32_t *
  * indices_t int32[E], the feature vectors and _VULN restricted to the batch — bit-identical to ddfa_build_csr +
  * ddfa_graph_ptr on the collated COO of the same graphs.  batch_nodes / batch_edges = N and E of the batch (the caller
  * knows them from its host copy of the graph sizes; they size the outputs).  A bad id or inconsistent totals leave the
- * outputs untouched and raise the int32 counter at workspace[(B + 1) * 4].  feats / out_feats: host arrays of device
- * pointers, num_feats <= 8. */
+ * outputs untouched and raise the int32 counter at workspace[(B + 1) * 4]: its low 16 bits count bad ids, bit 16 flags
+ * the totals.  Workspace layout (ddfa_arena_batch_workspace_bytes(B) bytes): int32 edge_ptr[B + 1] (first edge of every
+ * graph of the batch, then E), int32 counter, int32 node_ptr[B + 1] (graph_ptr staged until the ids are known to be good).
+ * feats / out_feats: host arrays of device pointers, num_feats <= 8. */
 size_t ddfa_arena_batch_workspace_bytes(int32_t batch_size);
 int ddfa_arena_batch(const int32_t *graph_ids, int32_t batch_size, int32_t num_graphs, const int32_t *node_off,
                      const int32_t *indptr, const int32_t *indices, const int32_t *indptr_t, const int32_t *indices_t,

@@ -101,13 +101,14 @@ def close_state(got, want, rtol=1e-6):
 
 
 def test_graph_kernel_against_fp64_with_padding_accumulation_and_reset():
-    k = Kernel(capacity=5000)
+    k = Kernel(capacity=12000)
     batches = []
-    for i, (B, nv) in enumerate([(300, 300), (1024, 1000), (17, 12)]):
+    # 2 113 graphs and more: past the 264 CTAs x 8 warps of graph_metrics_kernel, whose warps then stride over the batch
+    for i, (B, nv) in enumerate([(300, 300), (1024, 1000), (17, 12), (2112, 2112), (2113, 2100), (5000, 4990)]):
         logits, vuln, gptr, labels = graph_case(B, i)
         k.graph(logits, vuln, gptr, nv, 2.0, float(nv))
         batches.append((logits[:nv], labels[:nv], float(nv)))       # graphs [nv, B) are padding: ignored
-    want, probs = expected_state(batches, 2.0, C=5000)
+    want, probs = expected_state(batches, 2.0, C=k.C)
     close_state(k.state, want)
     assert k.state[TP].item() + k.state[FP].item() > 0
     n = int(want[SAMPLES])
@@ -117,7 +118,7 @@ def test_graph_kernel_against_fp64_with_padding_accumulation_and_reset():
     k.state.zero_()
     logits, vuln, gptr, labels = graph_case(50, 9)
     k.graph(logits, vuln, gptr, 50, 1.0, 50.0)
-    want, _ = expected_state([(logits, labels, 50.0)], 1.0, C=5000)
+    want, _ = expected_state([(logits, labels, 50.0)], 1.0, C=k.C)
     close_state(k.state, want)
 
 
