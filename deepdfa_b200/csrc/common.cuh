@@ -252,6 +252,12 @@ __device__ __forceinline__ float warp_max(float v) {
 
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// torch.relu: NaN stays NaN (fmaxf(NaN, 0) is 0, which would hide a non-finite activation from the loss, the gradients and the
+// non-finite step guard).  Every other input gives fmaxf's result bit for bit, the sign of a zero included.
+__device__ __forceinline__ float relu_nan(float y) { return y != y ? y : fmaxf(y, 0.f); }
+// ReLU's backward as torch's threshold_backward: the gradient is dropped where the activation is <= 0, so a NaN activation passes it
+__device__ __forceinline__ float relu_grad(float act, float g) { return act <= 0.f ? 0.f : g; }
+
 __device__ __forceinline__ void f4_add(float4 &a, const float4 &b) {
   a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
 }

@@ -316,7 +316,7 @@ __device__ __forceinline__ float load_a(const float *__restrict__ a, const float
 }
 
 // C[s, j] = sum_k A[s, k] * B(k, j) over the rows s < S, B(k, j) = TransB ? b[j * K + k] : b[k * Nout + j]; then the epilogue:
-// kBiasRelu out = max(C + bias, 0) (compact [S, Nout]); kMask out = mask > 0 ? C : 0 (compact); kScatter C into the two planes
+// kBiasRelu out = relu(C + bias) (compact [S, Nout]); kMask out = mask <= 0 ? 0 : C (compact); kScatter C into the two planes
 // dh (columns < D) and dx (columns >= D) at row rows[s]
 template <bool Gather, bool TransB, int E>
 __global__ void __launch_bounds__(256) head_gemm_kernel(const float *__restrict__ a, const float *__restrict__ h, const float *__restrict__ x,
@@ -369,8 +369,8 @@ __global__ void __launch_bounds__(256) head_gemm_kernel(const float *__restrict_
       const int32_t c = j0 + tx * 4 + j;
       if (c >= Nout) continue;
       const float v = acc[i][j];
-      if constexpr (E == kBiasRelu) out[(int64_t)s * Nout + c] = fmaxf(v + bias[c], 0.f);
-      else if constexpr (E == kMask) out[(int64_t)s * Nout + c] = mask[(int64_t)s * Nout + c] > 0.f ? v : 0.f;
+      if constexpr (E == kBiasRelu) out[(int64_t)s * Nout + c] = relu_nan(v + bias[c]);
+      else if constexpr (E == kMask) out[(int64_t)s * Nout + c] = relu_grad(mask[(int64_t)s * Nout + c], v);
       else {
         if (c < D) dh[r * D + c] = v;
         else dx[r * D + (c - D)] = v;
@@ -412,7 +412,7 @@ __global__ void __launch_bounds__(256) head_last_bwd_kernel(const float *__restr
     if (k < D) dh[r * D + k] = v;
     else dx[r * D + (k - D)] = v;
   } else {
-    out[i] = mask[i] > 0.f ? v : 0.f;
+    out[i] = relu_grad(mask[i], v);
   }
 }
 

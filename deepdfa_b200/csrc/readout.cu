@@ -115,7 +115,12 @@ __global__ void __launch_bounds__(kReadoutWarps * 32) readout_mlp_fwd_kernel(
       if (n < n1 && gate_logit && lane == 0) gate_logit[n] = g[u];
       m_new = fmaxf(m_new, g[u]);
     }
-    const float scale = expf(m - m_new);  // first iteration: exp(-inf) = 0  (m_new is finite: row nb exists)
+    // first iteration: exp(-inf) = 0 (m_new is finite when the gate logits are).  A NaN logit (skipped by fmaxf) has p = NaN, a +inf
+    // one p = exp(inf - inf) = NaN; the NaN reaches l and acc and, through fmaf(NaN, 0, .), the merge below even from a warp whose
+    // max stayed -inf: the graph pools to NaN, as in torch's softmax.  A -inf logit differs: torch gives its row weight 0, but a
+    // warp whose first group holds only -inf logits takes p = exp(-inf + inf) = NaN here and the graph pools to NaN.  With finite
+    // gate weights and bias a logit is -inf only when its row is not finite, and then torch's sum (0 * inf) is NaN as well
+    const float scale = expf(m - m_new);
     float p[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) p[u] = expf(g[u] - m_new);   // exp(-inf) = 0 for rows past the graph
@@ -203,7 +208,7 @@ __global__ void __launch_bounds__(kReadoutWarps * 32) readout_mlp_fwd_kernel(
         if (layer == L - 1) {
           logits[b] = y;
         } else {
-          y = fmaxf(y, 0.f);
+          y = relu_nan(y);
           s_out[r] = y;
           if (mlp_act) mlp_act[((int64_t)layer * B + b) * D2 + r] = y;
         }
@@ -296,10 +301,10 @@ __global__ void __launch_bounds__(kReadoutWarps * 32) readout_bwd_kernel(
 }
 
 // ---- small helpers for the MLP backward ---------------------------------------------------
-// out[m,n] = (mask == NULL || mask[m,n] > 0) ? in[m,n] : 0
+// out[m,n] = mask[m,n] <= 0 ? 0 : in[m,n]  (a NaN activation passes its gradient, as in torch)
 __global__ void relu_mask_kernel(const float *in, const float *__restrict__ mask, int64_t total, float *out) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < total) out[i] = (mask[i] > 0.f) ? in[i] : 0.f;
+  if (i < total) out[i] = relu_grad(mask[i], in[i]);
 }
 // DeepLift's rescale rule at a hidden ReLU (captum's `nonlinear`): with z = zg + bias and z' = zrg + bias the pre-activations of the
 // input and the reference pass, din *= (relu(z) - relu(z')) / (z - z'), or the plain derivative [act > 0] where |z - z'| < 1e-10
@@ -311,16 +316,16 @@ __global__ void __launch_bounds__(256) rescale_relu_kernel(float *__restrict__ d
   const float b = bias[i % n];
   const float z = zg[i] + b, zr = zrg[i] + b;
   const float dz = z - zr;
-  din[i] = fabsf(dz) < 1e-10f ? (act[i] > 0.f ? din[i] : 0.f) : din[i] * (fmaxf(z, 0.f) - fmaxf(zr, 0.f)) / dz;
+  din[i] = fabsf(dz) < 1e-10f ? relu_grad(act[i], din[i]) : din[i] * (relu_nan(z) - relu_nan(zr)) / dz;
 }
 // ---- MLP head over the whole batch (large training batches): hidden layers as one GEMM each + this epilogue, last layer below ----
-// a[m, n] = max(a[m, n] + bias[n], 0), 4 columns per thread (n % 4 == 0)
+// a[m, n] = relu(a[m, n] + bias[n]), 4 columns per thread (n % 4 == 0)
 __global__ void __launch_bounds__(256) bias_relu_kernel(float *__restrict__ a, const float *__restrict__ bias, int64_t total4, int32_t n4) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= total4) return;
   float4 v = *reinterpret_cast<const float4 *>(a + 4 * i);
   const float4 b = *reinterpret_cast<const float4 *>(bias + 4 * (i % n4));
-  v.x = fmaxf(v.x + b.x, 0.f); v.y = fmaxf(v.y + b.y, 0.f); v.z = fmaxf(v.z + b.z, 0.f); v.w = fmaxf(v.w + b.w, 0.f);
+  v.x = relu_nan(v.x + b.x); v.y = relu_nan(v.y + b.y); v.z = relu_nan(v.z + b.z); v.w = relu_nan(v.w + b.w);
   *reinterpret_cast<float4 *>(a + 4 * i) = v;
 }
 // logits[b] = in[b, :] . w + bias[0]: one warp per graph, the lane partition and shuffle tree of the in-CTA last layer (same sums)

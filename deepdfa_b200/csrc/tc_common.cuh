@@ -203,6 +203,7 @@ __device__ __forceinline__ void split8(const float (&x)[8], uint4 &ph, uint4 &pl
 // 20-bit float (1 sign, 5 exponent bits with fp16's bias, 14 mantissa bits).  Absolute error <= 3.1e-5 on r, z, 1.6e-5 on n, relative
 // 3.1e-5 on gh_n (|gh_n| < 6.1e-5 flushes to 0) — an order below plain fp16 (2.4e-4 / 4.9e-4), which measurably moved the parameter
 // gradients (profiles/r03b: 1.6e-5 -> 2e-4 relative), at the same 8 bytes.  Layout: x = r | z << 14 | gh[3:0] << 28 ; y = n | gh[19:4] << 16.
+// gh_n = +-inf and a NaN anywhere in the element are kept (exponent code 31), so the gate backward sees them as torch's does.
 __device__ __forceinline__ uint2 pack_gates(float r, float z, float n, float ghn) {
   // r, z come out of fast_sigmoid (in [0,1]) and n out of fast_tanh (in [-1,1]): no clamping needed.  Rounding to the nearest
   // integer by adding 2^23 (1.5 * 2^23 for the signed value) inside an FMA and reading the low mantissa bits: one FFMA on the
@@ -211,9 +212,14 @@ __device__ __forceinline__ uint2 pack_gates(float r, float z, float n, float ghn
   const uint32_t nq = __float_as_uint(fmaf(n, 32767.f, 12582912.f)) & 0xffffu;
   const uint32_t b = __float_as_uint(ghn);
   // round the mantissa to 14 bits (a carry runs into the exponent, as it should), drop the sign, re-bias the exponent 127 -> 15:
-  // core = [exponent - 112 | mantissa] ; below 2^-14 -> 0, above fp16's range -> largest value
+  // core = [exponent - 112 | mantissa] ; below 2^-14 -> 0, a finite value above fp16's range -> the largest finite code
   const int core = (int)(((b + 0x100u) << 1) >> 10) - (112 << 14);
   uint32_t g = core < (1 << 14) ? 0u : (uint32_t)min(core, (31 << 14) - 1);
+  // Non-finite values take fp16's codes, exponent 31, which no finite value reaches: gh_n = +-inf keeps its sign with a zero
+  // mantissa; a NaN in r, z, n or gh_n makes the whole element NaN (mantissa 1), as every gate gradient of that element is NaN in
+  // torch then.  r, z and n are bounded, so their sum with gh_n is non-finite exactly when one of these holds.
+  const float t = r + z + n + ghn;
+  if (!(fabsf(t) < INFINITY)) g = (31u << 14) | (t != t ? 1u : 0u);
   g |= (b >> 12) & 0x80000u;
   return make_uint2(rq | (zq << 14) | (g << 28), nq | ((g >> 4) << 16));
 }
@@ -224,7 +230,8 @@ __device__ __forceinline__ void unpack_gates(const uint2 &p, float &r, float &z,
   n = (__uint_as_float(((p.y & 0xffffu) ^ 0x4b008000u)) - 8421376.f) * (1.f / 32767.f);
   const uint32_t g = ((p.y >> 16) << 4) | (p.x >> 28);
   const uint32_t e = (g >> 14) & 31u;
-  ghn = e == 0u ? 0.f : __uint_as_float(((g >> 19) << 31) | ((e + 112u) << 23) | ((g & 0x3fffu) << 9));
+  ghn = e == 0u ? 0.f : __uint_as_float(((g >> 19) << 31) | ((e == 31u ? 255u : e + 112u) << 23) | ((g & 0x3fffu) << 9));
+  if (ghn != ghn) r = z = n = ghn;      // pack_gates' NaN code: the element's gates were not finite
 }
 
 // Gate math on the MUFU pipe.  __expf() expands to ex2.approx WITHOUT .ftz plus a range fix-up (FSETP, two predicated FMULs) per
