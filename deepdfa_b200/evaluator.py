@@ -7,10 +7,10 @@ MLP (graph style) or the node head over every valid node (node style), then ONE 
 ``ddfa_eval_metrics_rows``) that adds the batch's confusion counts, its mean BCE and, optionally, its probabilities and labels to
 a persistent fp64 device state.  Nothing syncs with the host until :meth:`FusedEvaluator.compute`.
 
-The batch paths are those of :class:`~deepdfa_b200.trainer.FusedTrainer` and share its plumbing: host batches through static
-per-shape buffers (two sets, ``prefetch``) with optional shape bucketing, resident device batches (one captured graph per
-object), graph ids of a :class:`~deepdfa_b200.arena.GraphArena` assembled inside the captured graph, and eager launches beyond
-``max_graph_shapes``.
+The batch paths are those of :class:`~deepdfa_b200.capture.CapturedBatches`, which :class:`~deepdfa_b200.trainer.FusedTrainer`
+shares: host batches through static per-shape buffers (two sets, ``prefetch``) with optional shape bucketing, resident device
+batches (one captured graph per object), graph ids of a :class:`~deepdfa_b200.arena.GraphArena` assembled inside the captured
+graph, and eager launches beyond ``max_graph_shapes``.
 
 Statement-level localisation (``statements=``): per batch, a score per node (CFG node = statement) and IVDetect's top-k statement
 metric over them (DDFA/sastvd/helpers/evaluate.py:262-322), added by ``ddfa_stmt_metric`` to a second fp64 state.  The scores are
@@ -28,8 +28,8 @@ import torch
 
 from . import _lib
 from . import engine as E
-from . import trainer as T
-from .batched_graph import BatchedCFG, as_batched_cfg
+from .batched_graph import as_batched_cfg
+from .capture import CapturedBatches
 from .module import FlowGNNGGNNModule, _ENGINES
 
 # the fp64 words of the metric state (include/ddfa_b200.h, DDFA_EVAL_STATE_WORDS)
@@ -93,7 +93,7 @@ def statement_metrics_from_state(state, prefix: str = "val_", node_style: bool =
     return out
 
 
-class FusedEvaluator:
+class FusedEvaluator(CapturedBatches):
     def __init__(self, model: FlowGNNGGNNModule, use_cuda_graph: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
                  max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64,
                  statements: Optional[str] = None, ig_steps: int = 50, shap_samples: Optional[int] = None,
@@ -185,11 +185,8 @@ class FusedEvaluator:
         self.ws = E.Workspace(dev)
         # DeepLift's baseline forwards keep their readout state here, apart from the input pass's saved state in self.ws
         self._ref_ws = E.Workspace(dev) if statements in ("deeplift", "deeplift_shap") else None
-        self._slots = {}
-        self._graphs = {}
-        self._warm_shapes = set()
-        self._copy_stream = None
         self._param_key = None
+        super().__init__()
 
     # ---- the metric state ------------------------------------------------------------------------------------------------
     @property
@@ -279,10 +276,7 @@ class FusedEvaluator:
         key = tuple(p.data_ptr() for p in plist)
         if key != self._param_key:
             if self._param_key is not None:
-                for slot in self._slots.values():
-                    for st in slot.get("sets", [slot]):
-                        st["graph"] = None
-                self._graphs.clear()
+                self._drop_graphs()
             self._param_key = key
         return E.ParamPack.from_flat_list(plist, len(m._tables()), m._num_layers)
 
@@ -298,18 +292,17 @@ class FusedEvaluator:
         idx = E.node_indices(g, m.concat_all_absdf, m.feature_keys["feature"], self.device)
         return g, dg, idx, fptr
 
-    def _enqueue(self, params, dg, idx, vuln, fptr, num_graphs: int, num_valid: Optional[int] = None,
-                 valid_nodes: Optional[torch.Tensor] = None):
-        """Enqueues one batch: the inference forward and the metric kernel, then, with ``statements``, the per-node scores and
-        the statement metric.  ``num_graphs``: the batch's graph count (its weight in the loss mean); ``num_valid``: graphs
-        [num_valid, B) are bucket padding; ``valid_nodes``: the int32 device word of the valid node count in node style under
-        bucketing; ``fptr``: the function-level graph_ptr.  Returns (node-style rows, scores): the scores are a fresh [N] tensor,
-        which a captured graph keeps writing on every replay."""
+    def _enqueue(self, params, prepared, vuln, num_valid: Optional[int], valid_nodes: Optional[torch.Tensor]):
+        """Enqueues one batch (``prepared``: what :meth:`_prepare` made of it) over ``params``: the inference forward and the
+        metric kernel, then, with ``statements``, the per-node scores and the statement metric.  ``num_valid``: graphs
+        [num_valid, B) are bucket padding (the real ones are the batch's weight in the loss mean); ``valid_nodes``: the int32
+        device word of the valid node count in node style under bucketing.  Returns the scores (None without ``statements``):
+        a fresh [N] tensor, which a captured graph keeps writing on every replay."""
+        g, dg, idx, fptr = prepared
+        num_graphs = g.batch_size if num_valid is None else num_valid
         m, ws = self.module, self.ws
         eng = _ENGINES[m.engine]
         pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
-        if vuln.dtype != torch.int32:
-            vuln = vuln.to(torch.int32)
         store = (E._p(self._probs), E._p(self._labels), self.max_predictions)
         mws = (self._metric_ws.data_ptr(), self._metric_ws.numel(), E._stream_ptr())
         L = _lib.lib()
@@ -325,7 +318,7 @@ class FusedEvaluator:
             if self._attributes:
                 self._attribute(params, dg, idx, scores)
             self._statement_metric(scores, vuln, fptr, num_valid)
-            return None, scores
+            return scores
         x, h_T, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, head=False, oob_counter=self._oob)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
@@ -338,7 +331,7 @@ class FusedEvaluator:
         if self.statements:          # rows = every valid node in order, so logits[n] is node n's
             E._call("ddfa_stmt_node_probability", E._p(logits), self._num_rows.data_ptr(), N, E._p(scores), E._stream_ptr())
             self._statement_metric(scores, vuln, fptr, num_valid)
-        return rows, scores
+        return scores
 
     def _statement_metric(self, scores, vuln, fptr, num_valid: Optional[int]) -> None:
         if self.statements is None:
@@ -408,135 +401,24 @@ class FusedEvaluator:
                         E._stream_ptr())
         self._draws.add_(1)
 
-    def _slot(self, g):
-        N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
-        bucket = T.bucket_shape(N, Eg, self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes)
-        det = _lib.deterministic_requested()
-        key = ("bucket", bucket[0], bucket[1], B, det) if bucket else ("exact", N, Eg, B, det)
-        slot = self._slots.get(key)
-        if slot is None:
-            if len(self._slots) >= self.max_graph_shapes:
-                return None
-            slot = T.new_stream_slot(g, bucket, self.device, self._node)
-            self._slots[key] = slot
-        return slot
-
     def prefetch(self, batch) -> None:
         """Starts the host->device copy of a (pinned) host batch on a side stream, overlapping the batch that is running; the
         following ``update(batch)`` with the SAME batch object picks the staged copy up.  No-op without ``use_cuda_graph`` or
         for device batches."""
-        if not self.use_cuda_graph:
-            return
-        g = as_batched_cfg(batch)
-        if g.device.type != "cpu":
-            return
-        with torch.cuda.device(self.device):
-            if self._copy_stream is None:
-                self._copy_stream = torch.cuda.Stream(device=self.device)
-            slot = self._slot(g)
-            if slot is not None:
-                slot["staged"] = (id(batch), T.stage(slot, g, self._copy_stream))
+        self._prefetch(batch, None)
 
     def update(self, batch) -> None:
         """Adds one batch (host, resident device or DGL batch; ``(batch, extrafeats)`` tuples as Lightning hands them over are
         accepted) to the metric state.  No host synchronisation."""
         if isinstance(batch, tuple):
             batch = batch[0]
-        g = as_batched_cfg(batch)
-        if self.use_cuda_graph and g.device.type == "cpu":
-            return self._update_streamed(batch, g)
-        return self._update_eager(batch)
-
-    def _update_streamed(self, batch, g):
-        with torch.cuda.device(self.device):
-            slot = self._slot(g)
-            if slot is None:          # more shapes than max_graph_shapes: same kernels, launched eagerly
-                return self._update_eager(batch)
-            params = self._params()
-            N, B = slot["N"], g.batch_size
-            main = torch.cuda.current_stream()
-            staged = slot["staged"]
-            slot["staged"] = None
-            if staged is not None and staged[0] == id(batch):
-                i = staged[1]
-                main.wait_event(slot["sets"][i]["ready"])
-            else:
-                i = T.stage(slot, g, main)
-            st = slot["sets"][i]
-
-            def enqueue():
-                gs = BatchedCFG(st["src"], st["dst"], st["bnn"], dict(st["ndata"]), num_nodes=N)   # no cached device CSR
-                _, dg, idx, fptr = self._prepare(gs)
-                vuln = gs.ndata["_VULN"]
-                if vuln.dtype != torch.int32:
-                    vuln = vuln.to(torch.int32)
-                st["rows"], st["scores"] = self._enqueue(params, dg, idx, vuln.contiguous(), fptr, B, num_valid=slot["valid"],
-                                                         valid_nodes=st["valid_nodes"])
-                st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
-
-            st["graph"] = T.graph_step(self.device, st["graph"], slot["warm"], enqueue)
-            slot["warm"] = True
-            self._keep_scores(st["scores"], g.num_nodes())
-            ev = torch.cuda.Event()
-            ev.record(main)
-            st["free"] = ev
+        self._run(batch, self._params())
 
     def update_ids(self, arena, ids) -> None:
         """Adds the graphs ``ids`` of a device-resident :class:`~deepdfa_b200.arena.GraphArena` (assembled by
         ``ddfa_arena_batch`` inside the captured graph: the H2D copy of the id list plus one graph launch per batch)."""
-        if not self.use_cuda_graph:
-            return self._update_eager(arena.batch(ids))
-        ids_np, B, N, Eg = T.arena_ids(arena, ids, "update_ids")
-        key = ("arena", id(arena), N, Eg, B, _lib.deterministic_requested())
-        slot = self._slots.get(key)
-        with torch.cuda.device(self.device):
-            if slot is None:
-                if len(self._slots) >= self.max_graph_shapes:
-                    return self._update_eager(arena.batch(ids))
-                slot = T.new_arena_slot(arena, B, N, Eg)
-                self._slots[key] = slot
-            params = self._params()
-            T.push_ids(slot, ids_np)
+        self._run_ids(arena, ids, self._params(), "update_ids")
 
-            def enqueue():
-                g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
-                _, dg, idx, fptr = self._prepare(g)
-                slot["rows"], slot["scores"] = self._enqueue(params, dg, idx, g.ndata["_VULN"], fptr, B)
-                slot["keep"] = (g, dg, idx)
-
-            slot["graph"] = T.graph_step(self.device, slot["graph"], slot["warm"], enqueue)
-            slot["warm"] = True
-            self._keep_scores(slot["scores"], N)
-
-    def _update_eager(self, batch):
-        """Device-resident batch objects (one captured graph per object when ``use_cuda_graph``), or plain eager launches."""
-        g, dg, idx, fptr = self._prepare(batch)
-        vuln = g.ndata["_VULN"]
-        if vuln.device != self.device or vuln.dtype != torch.int32:
-            key = "vuln_dev"
-            cached = g._cache.get(key)
-            if cached is None:
-                cached = vuln.to(self.device, non_blocking=True).to(torch.int32).contiguous()
-                g._cache[key] = cached
-            vuln = cached
-        B = g.batch_size
-        with torch.cuda.device(self.device):
-            params = self._params()
-            det = _lib.deterministic_requested()
-            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size, det)
-            graph_key = (id(g), det)
-            capturable = self.use_cuda_graph and as_batched_cfg(batch).device.type == "cuda" and \
-                (graph_key in self._graphs or len(self._graphs) < self.max_resident_graphs)
-            entry = self._graphs.get(graph_key)
-            out = {}
-
-            def enqueue():
-                out["rows"], out["scores"] = self._enqueue(params, dg, idx, vuln, fptr, B)
-            cg = T.graph_step(self.device, entry[0] if entry else None, capturable and shape_key in self._warm_shapes, enqueue)
-            if entry is None and cg is not None:
-                self._graphs[graph_key] = entry = (cg, g, idx, vuln, out["rows"], out["scores"])     # keep the captured tensors alive
-            self._warm_shapes.add(shape_key)
-            self._keep_scores(entry[5] if entry is not None else out["scores"], dg.num_nodes)
-
-    def _keep_scores(self, scores, num_nodes: int) -> None:
+    def _after_run(self, scores, num_nodes: int) -> None:
         self._last_scores = None if scores is None else scores[:num_nodes]
+

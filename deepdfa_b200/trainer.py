@@ -24,7 +24,7 @@ import torch.distributed as dist
 
 from . import _lib
 from . import engine as E
-from .batched_graph import BatchedCFG, as_batched_cfg
+from .capture import CapturedBatches
 from .module import FlowGNNGGNNModule, _ENGINES
 
 _ALIGN = 64  # elements; keeps every parameter 256-byte aligned inside the flat buffers
@@ -89,126 +89,6 @@ def owned_range(numel: int, rank: int, world: int):
     per = (n4 + world - 1) // world
     lo = min(n4, rank * per)
     return 4 * lo, 4 * min(n4, lo + per)
-
-
-# ---- captured-step plumbing shared by FusedTrainer and FusedEvaluator ----------------------------------------------------------
-def graph_step(device, graph, warm: bool, enqueue):
-    """One step through a cached CUDA graph: ``enqueue()`` runs eagerly while the shape is not ``warm`` (its first visit grows
-    the workspace and loads modules outside any capture); after that ``graph`` is replayed, captured first, after a device
-    synchronise, when it is None.  Returns the graph (None when the step ran eagerly)."""
-    if not warm:
-        enqueue()
-        return None
-    if graph is None:
-        torch.cuda.synchronize(device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            enqueue()
-    graph.replay()
-    return graph
-
-
-def bucket_shape(N: int, Eg: int, bucket_nodes: int, bucket_edges: int, min_pad_nodes: int):
-    """Padded (nodes, edges) of a batch under shape bucketing, or None when bucketing is off (``bucket_nodes <= 0``)."""
-    if bucket_nodes <= 0:
-        return None
-    bn, be = bucket_nodes, max(bucket_edges, 1)
-    Nb = (N + max(min_pad_nodes, 1) + bn - 1) // bn * bn
-    Eb = (Eg + be - 1) // be * be
-    return Nb, Eb
-
-
-def new_stream_slot(g, bucket, device, valid_nodes_word: bool) -> dict:
-    """The static per-shape input buffers of host batches shaped like ``g`` (or padded to ``bucket``): two buffer sets, so
-    that while the graph of one set runs the next batch is copied into the other (prefetch).  ``valid_nodes_word``: every set
-    gets an int32 device word with the batch's valid node count (node style under bucketing)."""
-    src, dst = g.edges()
-    N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
-    Ns, Es, Bs = (bucket[0], bucket[1], B + 1) if bucket else (N, Eg, B)
-
-    def new_set():
-        return {"src": torch.empty(Es, dtype=src.dtype, device=device), "dst": torch.empty(Es, dtype=dst.dtype, device=device),
-                "bnn": torch.empty(Bs, dtype=torch.int64, device=device),
-                "ndata": {k: torch.zeros((Ns,) + tuple(v.shape[1:]), dtype=v.dtype, device=device) for k, v in g.ndata.items()},
-                "graph": None, "keep": None, "free": None, "ready": None, "rows": None,
-                "valid_nodes": torch.zeros(1, dtype=torch.int32, device=device) if (bucket and valid_nodes_word) else None}
-    return {"sets": [new_set(), new_set()], "next": 0, "staged": None, "warm": False, "N": Ns,
-            "valid": B if bucket else None,
-            "iota": torch.arange(Es, dtype=src.dtype, device=device) if bucket else None}
-
-
-def stage(slot, g, stream) -> int:
-    """Copies the host batch ``g`` into the slot's next buffer set on ``stream``; returns the set index.  Under bucketing
-    the tails are (re)written too: padding nodes get feature index 0 / _VULN 0, the padding edges become self loops spread
-    round-robin over the padding nodes, and the dummy graph's node count goes into the last ``batch_num_nodes`` entry."""
-    i = slot["next"]
-    slot["next"] = 1 - i
-    st = slot["sets"][i]
-    caller = torch.cuda.current_stream()
-    with torch.cuda.stream(stream):
-        if st["free"] is not None:
-            stream.wait_event(st["free"])           # the graph that last read this set has finished
-        else:
-            stream.wait_stream(caller)              # first use: the set's zero fill, enqueued on the caller's stream, is done
-        src, dst = g.edges()
-        N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
-        st["src"][:Eg].copy_(src, non_blocking=True)
-        st["dst"][:Eg].copy_(dst, non_blocking=True)
-        st["bnn"][:B].copy_(g.batch_num_nodes(), non_blocking=True)
-        for k, v in g.ndata.items():
-            st["ndata"][k][:N].copy_(v, non_blocking=True)
-        if st["valid_nodes"] is not None:
-            st["valid_nodes"].fill_(N)              # node style: the sampler leaves the padding nodes (the tail) out
-        if slot["valid"] is not None:
-            Nb, Eb = slot["N"], st["src"].shape[0]
-            pad_nodes = Nb - N
-            st["bnn"][B:].fill_(pad_nodes)
-            for k in st["ndata"]:
-                st["ndata"][k][N:].zero_()
-            if Eb > Eg:
-                torch.remainder(slot["iota"][: Eb - Eg], pad_nodes, out=st["src"][Eg:])
-                st["src"][Eg:].add_(N)
-                st["dst"][Eg:].copy_(st["src"][Eg:])
-        ev = torch.cuda.Event()
-        ev.record(stream)
-        st["ready"] = ev
-    return i
-
-
-def arena_ids(arena, ids, who: str):
-    """``(ids as int64 numpy, B, N, E)`` of the graph ids of ``arena``; raises IndexError for an empty list or a bad id."""
-    import numpy as np
-    ids_np = np.asarray(ids.cpu() if isinstance(ids, torch.Tensor) else ids, dtype=np.int64).reshape(-1)
-    if ids_np.size == 0 or ids_np.min() < 0 or ids_np.max() >= arena.num_graphs:
-        raise IndexError(f"{who}: empty id list or graph id out of range")
-    return ids_np, int(ids_np.shape[0]), int(arena.nodes_per_graph[ids_np].sum()), int(arena.edges_per_graph[ids_np].sum())
-
-
-def new_arena_slot(arena, B: int, N: int, Eg: int) -> dict:
-    """Static per-shape outputs of the arena batch producer and a ring of pinned id stages: the host may run several steps
-    ahead of the device (that is what the captured graph is for), so a stage is rewritten only after the H2D copy that last
-    read it has completed."""
-    return {"out": arena.alloc_outputs(B, N, Eg), "stages": [torch.empty(B, dtype=torch.int32).pin_memory() for _ in range(4)],
-            "stage_done": [None] * 4, "turn": 0, "steps": 0,
-            "graph": None, "warm": False, "keep": None, "arena": arena}     # the arena stays alive with its graph
-
-
-def push_ids(slot, ids_np) -> None:
-    """Copies the id list into the slot's next pinned stage and from there, in stream order, into its device id buffer; every
-    256 calls the producer's device error counter of the last batch is checked (one synchronisation)."""
-    import numpy as np
-    k = slot["turn"]
-    slot["turn"] = (k + 1) % len(slot["stages"])
-    if slot["stage_done"][k] is not None:
-        slot["stage_done"][k].synchronize()
-    slot["stages"][k].copy_(torch.from_numpy(ids_np.astype(np.int32)))
-    slot["out"]["ids"].copy_(slot["stages"][k], non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record()
-    slot["stage_done"][k] = ev
-    slot["steps"] += 1
-    if slot["keep"] is not None and slot["steps"] % 256 == 0:
-        slot["keep"][0].check()      # the assembler's device error counter (bad id / totals mismatch): one sync every 256 steps
 
 
 _FIRST, _ADD, _APPLY = "first", "add", "apply"     # what a micro-batch does with its gradient (FusedTrainer._phase)
@@ -505,7 +385,7 @@ def _group_property(key, convert=None):
     return property(get, set)
 
 
-class FusedTrainer:
+class FusedTrainer(CapturedBatches):
     def __init__(self, module: FlowGNNGGNNModule, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 1e-2, process_group=None, use_cuda_graph: bool = False, max_graph_shapes: int = 8,
                  max_resident_graphs: int = 64, distributed: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
@@ -737,10 +617,7 @@ class FusedTrainer:
                 self._metric_state = torch.zeros(_lib.EVAL_STATE_WORDS, dtype=torch.float64, device=self.device)
                 self._metric_ws = torch.empty(_lib.lib().call("ddfa_eval_metrics_workspace_bytes"), dtype=torch.uint8, device=self.device)
         self._update = self._update_calls()
-        self._graphs = {}
-        self._stream_slots = {}
-        self._copy_stream = None
-        self._warm_shapes = set()
+        super().__init__()
 
     # The Adam hyperparameters live in self.optimizer.param_groups[0], which is what an LR scheduler changes; the next step
     # (eager or replayed) uses whatever is there when it starts.
@@ -916,8 +793,11 @@ class FusedTrainer:
     def _sum_ints(self, t: torch.Tensor) -> None:
         dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.pg)
 
-    def _node_step_done(self, rows):
-        """After a node-style step: remembers its row list and sends the sampler's status word to the host behind it."""
+    def _after_run(self, rows, num_nodes: int):
+        """After every step, replays included, node style: remembers its row list and sends the sampler's status word to the
+        host behind it."""
+        if not self._node:
+            return
         self._last_rows = rows
         self._status_host.copy_(self._sample_status, non_blocking=True)
         ev = torch.cuda.Event()
@@ -1020,11 +900,12 @@ class FusedTrainer:
                                  "the loss is the mean over the GLOBAL batch)")
         return int(local_graphs)
 
-    def _enqueue(self, g, dg, idx, vuln, global_batch: int, num_valid: Optional[int] = None, valid_nodes: Optional[torch.Tensor] = None,
-                 phase: str = _APPLY):
-        """Enqueues one step (one micro-batch, ``phase`` as :meth:`_phase` says).  Node style returns the row-list buffer the
-        step's loss rows go to; ``valid_nodes``: the int32 device word of its valid node count under bucketing (None: every node
-        is valid)."""
+    def _enqueue(self, ctx, prepared, vuln, num_valid: Optional[int], valid_nodes: Optional[torch.Tensor]):
+        """Enqueues one step of the batch ``prepared`` (``module._prepare``) with ``ctx = (global_batch, phase)``: one
+        micro-batch, ``phase`` as :meth:`_phase` says.  Node style returns the row-list buffer the step's loss rows go to;
+        ``valid_nodes``: the int32 device word of its valid node count under bucketing (None: every node is valid)."""
+        global_batch, phase = ctx
+        g, dg, idx = prepared
         m = self.module
         eng = _ENGINES[m.engine]
         pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
@@ -1039,6 +920,7 @@ class FusedTrainer:
         _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws,
                                      grad_ggnn=self._grad_ggnn)
         prune = dict(grad_ggnn=self._grad_ggnn, grad_tables=self._grad_tables)
+        global_batch = self._global_batch(global_batch, dg.batch_size if num_valid is None else num_valid)
         # the gradient of loss / k (k = 1: 1 / global_batch as ever); the loss itself stays the micro-batch's mean
         _, _, dlogits = E.graph_label_bce(dg, vuln, logits, pw, 1.0 / global_batch, 1.0 / (global_batch * self._k), True,
                                           alloc=self.ws, loss_out=self._loss_local if self.exchange == "p2p" else self.loss_slot,
@@ -1051,9 +933,7 @@ class FusedTrainer:
         if self.track_metrics:
             B = dg.batch_size
             nv = B if num_valid is None else int(num_valid)
-            if vuln.dtype != torch.int32:
-                vuln = vuln.to(torch.int32)
-            self._enqueue_metrics("ddfa_eval_metrics_graph", (E._p(logits), E._p(vuln.contiguous()), E._p(dg.graph_ptr), B, nv), pw, nv)
+            self._enqueue_metrics("ddfa_eval_metrics_graph", (E._p(logits), E._p(vuln), E._p(dg.graph_ptr), B, nv), pw, nv)
 
     def _enqueue_metrics(self, name, head, pw, num_graphs):
         """track_metrics: the step's logits into the training metric state (no prediction store), weighted by the graph count."""
@@ -1102,8 +982,6 @@ class FusedTrainer:
         m, ws = self.module, self.ws
         N = dg.num_nodes
         factor = m.hparams.undersample_node_on_loss_factor
-        if vuln.dtype != torch.int32:
-            vuln = vuln.to(torch.int32)
         if self.world > 1:
             return self._enqueue_node_dp(dg, idx, vuln, eng, pw, valid_nodes, phase)
         x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False,
@@ -1165,92 +1043,23 @@ class FusedTrainer:
             dist.all_reduce(self.flat_g[:lo], op=dist.ReduceOp.SUM, group=self.pg)
             dist.all_reduce(self.flat_g[hi:], op=dist.ReduceOp.SUM, group=self.pg)      # ... b_ih, b_hh, gate, MLP, [loss]
 
-    # ------------------------------------------------------------------------------------
-    # ---- host batches through per-shape static buffers + captured graphs -------------------------------------------------
-    def _graph_step(self, graph, warm: bool, enqueue):
-        return graph_step(self.device, graph, warm, enqueue)
-
-    def _bucket_shape(self, N: int, Eg: int):
-        return bucket_shape(N, Eg, self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes)
-
+    # ---- the batch paths (capture.CapturedBatches) and their hooks ----------------------------------------------------------
     def num_bucket_shapes(self) -> int:
-        return len({k[:6] for k in self._stream_slots if k[0] == "bucket"})     # the phases of one shape count once
+        # keys start (kind, Nb, Eb, B, det, global batch): the phases of one shape count once
+        return len({k[:6] for k in self._stream_slots if k[0] == "bucket"})
 
-    def _stream_slot(self, g, global_batch: Optional[int], phase: str):
-        N, Eg, B = g.num_nodes(), g.num_edges(), g.batch_size
-        gb = self._global_batch(global_batch, B)
-        bucket = self._bucket_shape(N, Eg)
-        # keyed by the deterministic mode too: a captured graph keeps the kernels of the mode it was captured in
-        det = _lib.deterministic_requested()
-        key = ("bucket", bucket[0], bucket[1], B, gb, det) if bucket else ("exact", N, Eg, B, gb, det)
-        key += self._phase_key(phase)
-        slot = self._stream_slots.get(key)
-        if slot is None:
-            if len(self._stream_slots) >= self.max_graph_shapes:
-                return None
-            slot = new_stream_slot(g, bucket, self.device, self._node)
-            slot["gb"] = gb
-            self._stream_slots[key] = slot
-        return slot
+    def _prepare(self, batch):
+        return self.module._prepare(batch)
 
-    def _stage(self, slot, g, stream):
-        return stage(slot, g, stream)
+    def _key_suffix(self, ctx, B: int) -> tuple:
+        global_batch, phase = ctx
+        return (self._global_batch(global_batch, B),) + self._phase_key(phase)
 
     def prefetch(self, batch, global_batch: Optional[int] = None) -> None:
         """Starts the host->device copy of a (pinned) host batch on a side stream so that it overlaps the step that is running;
         the following ``step(batch)`` with the SAME batch object picks the staged copy up (with gradient accumulation: the very
         next micro-batch).  No-op without ``use_cuda_graph`` or for device batches."""
-        if not self.use_cuda_graph:
-            return
-        g = as_batched_cfg(batch)
-        if g.device.type != "cpu":
-            return
-        with torch.cuda.device(self.device):
-            if self._copy_stream is None:
-                self._copy_stream = torch.cuda.Stream(device=self.device)
-            slot = self._stream_slot(g, global_batch, self._phase())
-            if slot is not None:
-                slot["staged"] = (id(batch), self._stage(slot, g, self._copy_stream))
-
-    def _step_streamed(self, batch, g, global_batch: Optional[int], phase: str) -> None:
-        """Host batch + use_cuda_graph: the batch's arrays are copied into device buffers that are STATIC per shape
-        (num_nodes, num_edges, batch_size — or per BUCKET shape with ``bucket_nodes`` / ``bucket_edges``) and one captured
-        CUDA graph per buffer set covers the whole step including the device CSR build — a new batch of a known shape costs
-        its H2D copies (overlappable: ``prefetch``) plus one graph launch.  The first visit of a shape runs eagerly
-        (workspace growth), the next two capture.  Every phase of a shape has a slot of its own."""
-        m = self.module
-        with torch.cuda.device(self.device):
-            slot = self._stream_slot(g, global_batch, phase)
-            if slot is None:          # more shapes than max_graph_shapes: same kernels, launched eagerly
-                return self._step_eager(batch, global_batch, phase)
-            N, gb = slot["N"], slot["gb"]
-            main = torch.cuda.current_stream()
-            staged = slot["staged"]
-            slot["staged"] = None
-            if staged is not None and staged[0] == id(batch):
-                i = staged[1]
-                main.wait_event(slot["sets"][i]["ready"])
-            else:
-                i = self._stage(slot, g, main)
-            st = slot["sets"][i]
-
-            def enqueue():
-                gs = BatchedCFG(st["src"], st["dst"], st["bnn"], dict(st["ndata"]), num_nodes=N)   # no cached device CSR
-                g_, dg, idx = m._prepare(gs)
-                vuln = gs.ndata["_VULN"]
-                if vuln.dtype != torch.int32:
-                    vuln = vuln.to(torch.int32)
-                st["rows"] = self._enqueue(g_, dg, idx, vuln.contiguous(), gb, num_valid=slot["valid"], valid_nodes=st["valid_nodes"],
-                                           phase=phase)
-                st["keep"] = (gs, dg, idx, vuln)         # tensors allocated during capture live in the graph's pool
-
-            st["graph"] = self._graph_step(st["graph"], slot["warm"], enqueue)
-            slot["warm"] = True
-            if self._node:
-                self._node_step_done(st["rows"])
-            ev = torch.cuda.Event()
-            ev.record(main)
-            st["free"] = ev
+        self._prefetch(batch, (global_batch, self._phase()))
 
     def step_ids(self, arena, ids, global_batch: Optional[int] = None) -> torch.Tensor:
         """One optimisation step on the graphs ``ids`` of a device-resident :class:`deepdfa_b200.arena.GraphArena` (SURVEY.md §8
@@ -1258,33 +1067,7 @@ class FusedTrainer:
         ``ddfa_arena_batch`` inside one captured graph, so a step costs the H2D copy of the id list plus one graph launch;
         otherwise it is ``step(arena.batch(ids))``.  One micro-batch, as :meth:`step`."""
         phase = self._begin()
-        if not self.use_cuda_graph:
-            self._step_eager(arena.batch(ids), global_batch, phase)
-            return self._end(phase)
-        m = self.module
-        ids_np, B, N, Eg = arena_ids(arena, ids, "step_ids")
-        gb = self._global_batch(global_batch, B)
-        key = ("arena", id(arena), N, Eg, B, gb, _lib.deterministic_requested()) + self._phase_key(phase)
-        slot = self._stream_slots.get(key)
-        with torch.cuda.device(self.device):
-            if slot is None:
-                if len(self._stream_slots) >= self.max_graph_shapes:
-                    self._step_eager(arena.batch(ids), global_batch, phase)
-                    return self._end(phase)
-                slot = new_arena_slot(arena, B, N, Eg)
-                self._stream_slots[key] = slot
-            push_ids(slot, ids_np)
-
-            def enqueue():
-                g = arena._assemble(slot["out"]["ids"], B, N, Eg, slot["out"])
-                g_, dg, idx = m._prepare(g)
-                slot["rows"] = self._enqueue(g_, dg, idx, g.ndata["_VULN"], gb, phase=phase)
-                slot["keep"] = (g, dg, idx)
-
-            slot["graph"] = self._graph_step(slot["graph"], slot["warm"], enqueue)
-            slot["warm"] = True
-            if self._node:
-                self._node_step_done(slot["rows"])
+        self._run_ids(arena, ids, (global_batch, phase), "step_ids")
         return self._end(phase)
 
     def step(self, batch, global_batch: Optional[int] = None) -> torch.Tensor:
@@ -1292,47 +1075,11 @@ class FusedTrainer:
         global mean loss (valid after the step's stream work completes).  Starts with ``self.optimizer.step()``, which hands
         the current learning rate etc. to this step's Adam launch (an LR scheduler on ``self.optimizer`` sees that call).
         With ``accumulate_grad_batches=k > 1`` the call is one micro-batch: only the last of a window updates the parameters
-        and calls ``optimizer.step()`` (see the constructor)."""
+        and calls ``optimizer.step()`` (see the constructor).  Host batches under ``use_cuda_graph`` run through static
+        per-shape buffers (every phase of a shape has a slot of its own), device batches one captured graph per object."""
         phase = self._begin()
-        gb_ = as_batched_cfg(batch) if self.use_cuda_graph else None
-        if gb_ is not None and gb_.device.type == "cpu":
-            self._step_streamed(batch, gb_, global_batch, phase)
-        else:
-            self._step_eager(batch, global_batch, phase)
+        self._run(batch, (global_batch, phase))
         return self._end(phase)
-
-    def _step_eager(self, batch, global_batch: Optional[int] = None, phase: str = _APPLY) -> None:
-        """Device-resident batch objects (one captured graph per object when ``use_cuda_graph``), or plain eager launches."""
-        m = self.module
-        g, dg, idx = m._prepare(batch)
-        vuln = g.ndata["_VULN"]
-        if vuln.device != self.device or vuln.dtype != torch.int32:
-            key = "vuln_dev"
-            cached = g._cache.get(key)
-            if cached is None:
-                cached = vuln.to(self.device, non_blocking=True).to(torch.int32).contiguous()
-                g._cache[key] = cached
-            vuln = cached
-        global_batch = self._global_batch(global_batch, dg.batch_size)
-        with torch.cuda.device(self.device):
-            det = _lib.deterministic_requested()
-            shape_key = (dg.num_nodes, dg.num_edges, dg.batch_size, det) + self._phase_key(phase)
-            graph_key = (id(g), det) + self._phase_key(phase)
-            capturable = self.use_cuda_graph and as_batched_cfg(batch).device.type == "cuda" and \
-                (graph_key in self._graphs or len(self._graphs) < self.max_resident_graphs)
-            # one captured CUDA graph per resident batch object (its device pointers are baked in); a step that cannot be
-            # captured runs eagerly
-            entry = self._graphs.get(graph_key)
-            out = {}
-
-            def enqueue():
-                out["rows"] = self._enqueue(g, dg, idx, vuln, global_batch, phase=phase)
-            cg = self._graph_step(entry[0] if entry else None, capturable and shape_key in self._warm_shapes, enqueue)
-            if entry is None and cg is not None:
-                self._graphs[graph_key] = (cg, g, idx, vuln, out["rows"])     # keep the captured tensors alive
-            self._warm_shapes.add(shape_key)
-            if self._node:
-                self._node_step_done(out["rows"] if "rows" in out else entry[4])
 
     # ------------------------------------------------------------------------------------
     @staticmethod
