@@ -129,6 +129,7 @@ _SIGNATURES = {
     "ddfa_stmt_node_probability": (_int, [_vp, _vp, _i32, _vp, _vp]),
     "ddfa_stmt_attribution_score": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _vp, _vp]),
     "ddfa_stmt_shap_input": (_int, [_vp, _vp, _i32, _i32, _i32, _f32, _f32, _f32, C.c_uint64, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "ddfa_predict_store": (_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "ddfa_mlp_dgrad_rescale": (_int, [_vp] * 7 + [_i32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_grad_accumulate": (_int, [_vp, _vp, _i64, _i64, _i32, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
@@ -147,6 +148,7 @@ EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluat
 STMT_STATE_WORDS = 16         # DDFA_STMT_STATE_WORDS: fp64 words of the statement metric state
 STMT_MODE_VULN_ONLY, STMT_MODE_FULL = 0, 1    # DDFA_STMT_MODE_*: modes of ddfa_stmt_metric
 STMT_SCORE_ABS, STMT_SCORE_X_TIMES = 0, 1     # DDFA_STMT_SCORE_*: rules of ddfa_stmt_input_grad_score
+PREDICT_MAX_K = 32            # DDFA_PREDICT_MAX_K: the most statements ddfa_predict_store ranks per function
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
 GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate
 ADAM_GROUP_WORDS = 8          # DDFA_ADAM_GROUP_WORDS: fp32 words per row of the parameter-group table

@@ -93,49 +93,28 @@ def statement_metrics_from_state(state, prefix: str = "val_", node_style: bool =
     return out
 
 
-class FusedEvaluator(CapturedBatches):
-    def __init__(self, model: FlowGNNGGNNModule, use_cuda_graph: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
-                 max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64,
-                 statements: Optional[str] = None, ig_steps: int = 50, shap_samples: Optional[int] = None,
-                 baseline_stdev: float = 0.0, noise_stdev: float = 0.0, attribution_seed: int = 0):
-        """``max_predictions`` > 0 keeps the first that many probabilities and labels (``predictions()``; the reference's
-        ``test_preds`` / ``test_labels``); more samples than that make :meth:`compute` raise, the counts stay complete.
-        ``bucket_nodes`` / ``bucket_edges``: shape bucketing of host batches under ``use_cuda_graph``, as in ``FusedTrainer``
-        (one padding graph, excluded from every metric).  The evaluator reads the module's parameters where they live when a
-        batch runs and never writes them; graphs captured over other parameter storage (a ``FusedTrainer`` built later moves
-        the parameters into its flat buffer) are recaptured.
-        ``statements``: the per-statement score of :meth:`last_scores` and of the statement metrics (``STATEMENT_MODES``):
-        ``"probability"`` (node style: the node head's sigmoid), ``"attention"`` (graph style: the readout's softmax gate α_n,
-        summing to 1 over each function), ``"saliency"`` (graph style: Σ_d |∂logit/∂x_{n,d}| of the embedding output x, captum's
-        ``Saliency(abs=True)``) or ``"integrated_gradients"`` (graph style: Σ_d x_{n,d} · (1/m) Σ_{k<m} ∂logit/∂x_{n,d} at
-        ((k + ½)/m)·x, m = ``ig_steps``, zero baseline: captum's ``IntegratedGradients(method="riemann_middle")``).  The target is
-        each function's own logit; one backward with dlogits = 1 serves every function of the batch.  None (the default)
-        enqueues nothing beyond the classification metrics.
-        ``"deeplift"`` (graph style): captum's ``DeepLift(multiply_by_inputs=True)`` with a zero baseline x̄: Σ_d (x − x̄)_{n,d} ·
-        g̃_{n,d}, g̃ the input gradient with each hidden ReLU of the MLP head under the rescale rule — its derivative replaced by
-        (relu(z) − relu(z̄)) / (z − z̄), z̄ the pre-activation of a full forward of the same graph from x̄ — and every other
-        nonlinearity (GRU gates, pooling softmax, gate products) a plain gradient at the input pass's activations, as captum
-        hooks only ``nn.ReLU`` modules.  ``"deeplift_shap"``: captum's ``DeepLiftShap``, the mean of DeepLift over the baselines
-        b_j = ``baseline_stdev`` · ε_j, j < ``shap_samples`` (default 16); with ``baseline_stdev`` = 0 (the default) every baseline
-        is zero and DeepLift runs once, bit-identical to ``"deeplift"``.  ``"gradient_shap"``: captum's ``GradientShap``, the mean
-        over ``shap_samples`` (default 5) samples s of Σ_d (x̃ − b) · ∂logit/∂x at b + α(x̃ − b), x̃ = x + ``noise_stdev`` · ε,
-        b = ``baseline_stdev`` · ε' (zero by default) and α uniform in [0, 1) per function.  The draws are Philox4x32-10 with key
-        ``attribution_seed`` and a device batch counter (``ddfa_stmt_shap_input``, :attr:`attribution_draws`), advanced once per
-        batch these three modes attribute, so captured replays draw fresh values."""
-        if model.device.type != "cuda":
-            raise _lib.DdfaError("FusedEvaluator needs the module on a CUDA device (no CPU fallback)")
+class InferencePass(CapturedBatches):
+    """The inference forward and the per-statement scores of one batch over the module's current parameters, on the batch paths
+    of :class:`~deepdfa_b200.capture.CapturedBatches`: what :class:`FusedEvaluator` and
+    :class:`~deepdfa_b200.predictor.FusedPredictor` enqueue before their own per-batch kernels.  The owner's ``__init__`` checks
+    the module and calls :meth:`_init_inference`."""
+
+    def _init_inference(self, model: FlowGNNGGNNModule, statements, ig_steps, shap_samples, baseline_stdev, noise_stdev,
+                        attribution_seed, use_cuda_graph, bucket_nodes, bucket_edges, max_graph_shapes, bucket_min_pad_nodes,
+                        max_resident_graphs) -> None:
+        """Checks the statement settings (``FusedEvaluator``'s docstring describes them) against the module and allocates what
+        the forward and the scores keep between batches.  An ``encoder_mode`` module (graph style) takes ``"attention"`` only:
+        the gradient modes differentiate a logit."""
+        who = type(self).__name__
         hp = model.hparams
-        if hp.encoder_mode or model._num_layers == 0:
-            raise ValueError("FusedEvaluator: an encoder_mode module returns embeddings, not logits: there is nothing to score")
-        if hp.label_style not in ("graph", "node"):
-            raise ValueError(f"FusedEvaluator: label_style={hp.label_style!r} is not supported ('graph' or 'node')")
-        if int(max_predictions) < 0:
-            raise ValueError(f"max_predictions must be >= 0, got {max_predictions!r}")
         if statements is not None:
             if statements not in STATEMENT_MODES:
-                raise ValueError(f"FusedEvaluator: statements={statements!r} is not one of {sorted(STATEMENT_MODES)} or None")
+                raise ValueError(f"{who}: statements={statements!r} is not one of {sorted(STATEMENT_MODES)} or None")
+            if hp.encoder_mode and statements != "attention":
+                raise ValueError(f"{who}: an encoder_mode module has no logit to attribute: statements='attention' or None, "
+                                 f"got {statements!r}")
             if STATEMENT_MODES[statements] != hp.label_style:
-                raise ValueError(f"FusedEvaluator: statements={statements!r} scores label_style={STATEMENT_MODES[statements]!r} "
+                raise ValueError(f"{who}: statements={statements!r} scores label_style={STATEMENT_MODES[statements]!r} "
                                  f"modules, this one has label_style={hp.label_style!r}")
         if int(ig_steps) < 1:
             raise ValueError(f"ig_steps must be >= 1, got {ig_steps!r}")
@@ -163,32 +142,21 @@ class FusedEvaluator(CapturedBatches):
         self.bucket_nodes, self.bucket_edges, self.bucket_min_pad_nodes = int(bucket_nodes), int(bucket_edges), int(bucket_min_pad_nodes)
         self.max_graph_shapes = int(max_graph_shapes)
         self.max_resident_graphs = int(max_resident_graphs)
-        self.max_predictions = int(max_predictions)
-        L = _lib.lib()
         dev = self.device
         with torch.cuda.device(dev):
-            self._state = torch.zeros(_lib.EVAL_STATE_WORDS, dtype=torch.float64, device=dev)
-            self._metric_ws = torch.empty(L.call("ddfa_eval_metrics_workspace_bytes"), dtype=torch.uint8, device=dev)
-            cap = max(self.max_predictions, 1)
-            self._probs = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
-            self._labels = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
-            self._oob = torch.zeros(1, dtype=torch.int32, device=dev)        # out-of-range embedding indices (compute() raises)
+            self._oob = torch.zeros(1, dtype=torch.int32, device=dev)        # out-of-range embedding indices (the owner raises)
             self._num_rows = torch.zeros(1, dtype=torch.int32, device=dev) if self._node else None
-            self._stmt_state = torch.zeros(_lib.STMT_STATE_WORDS, dtype=torch.float64, device=dev)
-            self._stmt_ws = torch.empty(L.call("ddfa_stmt_metric_workspace_bytes"), dtype=torch.uint8, device=dev) if statements else None
             # the gradients the dgrad chain computes inline (MLP, gate, GRU biases / w_hh) land here, never in the module's .grad
             self._grad_scratch = E.ParamPack.from_flat_list([torch.zeros_like(p) for p in model.param_list()], len(model._tables()),
                                                             model._num_layers) if self._attributes else None
             # the batch counter of the attribution draws (advanced once per attributed batch, inside a captured graph too)
             self._draws = torch.zeros(1, dtype=torch.int64, device=dev)
-        self._last_scores = None
         self.ws = E.Workspace(dev)
         # DeepLift's baseline forwards keep their readout state here, apart from the input pass's saved state in self.ws
         self._ref_ws = E.Workspace(dev) if statements in ("deeplift", "deeplift_shap") else None
         self._param_key = None
-        super().__init__()
+        CapturedBatches.__init__(self)
 
-    # ---- the metric state ------------------------------------------------------------------------------------------------
     @property
     def _attributes(self) -> bool:
         return self.statements in _GRADIENT_MODES
@@ -207,68 +175,6 @@ class FusedEvaluator(CapturedBatches):
             raise ValueError(f"attribution_draws must be >= 0, got {value!r}")
         self._draws.fill_(v)
 
-    def reset(self) -> None:
-        """Zeroes the metric state and the statement state in stream order (the prediction store starts over at position 0)."""
-        self._state.zero_()
-        self._stmt_state.zero_()
-
-    def state(self) -> torch.Tensor:
-        """The float64 device metric state (``EVAL_STATE_WORDS`` words, layout in include/ddfa_b200.h), a view: the evaluator
-        keeps accumulating into it.  Every word is a sum, so ``dist.all_reduce(ev.state())`` adds ranks exactly (integers below
-        2**53) and :meth:`metrics_from_state` turns the sum into the global metrics."""
-        return self._state
-
-    metrics_from_state = staticmethod(metrics_from_state)
-    statement_metrics_from_state = staticmethod(statement_metrics_from_state)
-
-    def statement_state(self) -> torch.Tensor:
-        """The float64 device statement state (``STMT_STATE_WORDS`` words, layout in include/ddfa_b200.h, DDFA_STMT_STATE_WORDS),
-        a view, separate from :meth:`state`.  Every word is an integer count, so ``dist.all_reduce(ev.statement_state())`` adds
-        ranks exactly and :meth:`statement_metrics_from_state` turns the sum into the global statement metrics."""
-        return self._stmt_state
-
-    def last_scores(self) -> torch.Tensor:
-        """The fp32 device scores ``[N]`` of the last batch's statements, in the batch's node order (without the padding graph's
-        nodes under bucketing).  The next :meth:`update` overwrites them: copy them per batch to keep them."""
-        if self.statements is None:
-            raise ValueError("FusedEvaluator.last_scores: built with statements=None (no per-statement score)")
-        if self._last_scores is None:
-            raise ValueError("FusedEvaluator.last_scores: no batch was evaluated yet")
-        return self._last_scores
-
-    def compute(self, prefix: str = "val_") -> dict:
-        """The metrics of everything evaluated since the last :meth:`reset` (one synchronisation).  Raises ``ValueError`` when
-        no sample was evaluated or predictions overflowed ``max_predictions``, and ``IndexError`` when a batch had node feature
-        indices outside the embedding tables."""
-        s = self._state.cpu()
-        bad = int(self._oob.item())
-        if bad:
-            self._oob.zero_()
-            raise IndexError(f"{bad} node feature indices outside [0, {self.module.input_dim}) in an evaluated batch")
-        n = int(s[TP] + s[FP] + s[TN] + s[FN])
-        if n == 0:
-            raise ValueError("FusedEvaluator.compute: no sample was evaluated since the last reset()")
-        if self._probs is not None and s[OVERFLOW] > 0:
-            raise ValueError(f"FusedEvaluator.compute: {n} predictions, max_predictions={self.max_predictions}: build the "
-                             f"evaluator with max_predictions >= {n}")
-        out = metrics_from_state(s, prefix)
-        if self.statements is not None:
-            ss = self._stmt_state.cpu()
-            if ss[S_NAN] > 0:
-                raise ValueError(f"FusedEvaluator.compute: {int(ss[S_NAN])} functions had a NaN statement score "
-                                 f"(statements={self.statements!r})")
-            out.update(statement_metrics_from_state(ss, prefix, node_style=self._node))
-        return out
-
-    def predictions(self):
-        """``(probs, labels)``: fp32 device tensors of the first ``min(stored, max_predictions)`` samples in evaluation order
-        (graph order, or node order within a batch).  Reads the stored count: one synchronisation."""
-        if self._probs is None:
-            raise ValueError("FusedEvaluator.predictions: built with max_predictions=0 (no prediction store)")
-        k = int(self._state[STORED].item())
-        return self._probs[:k], self._labels[:k]
-
-    # ---- per batch -------------------------------------------------------------------------------------------------------
     def _params(self):
         """A ParamPack over the module's current parameter storage; a change of storage drops every captured graph."""
         m = self.module
@@ -292,33 +198,20 @@ class FusedEvaluator(CapturedBatches):
         idx = E.node_indices(g, m.concat_all_absdf, m.feature_keys["feature"], self.device)
         return g, dg, idx, fptr
 
-    def _enqueue(self, params, prepared, vuln, num_valid: Optional[int], valid_nodes: Optional[torch.Tensor]):
-        """Enqueues one batch (``prepared``: what :meth:`_prepare` made of it) over ``params``: the inference forward and the
-        metric kernel, then, with ``statements``, the per-node scores and the statement metric.  ``num_valid``: graphs
-        [num_valid, B) are bucket padding (the real ones are the batch's weight in the loss mean); ``valid_nodes``: the int32
-        device word of the valid node count in node style under bucketing.  Returns the scores (None without ``statements``):
-        a fresh [N] tensor, which a captured graph keeps writing on every replay."""
+    def _forward(self, params, prepared, vuln, valid_nodes: Optional[torch.Tensor], scores: Optional[torch.Tensor]):
+        """The inference forward of one batch (``prepared``: what :meth:`_prepare` made of it) over ``params``.  Graph style:
+        ``(logits [B] or None in encoder_mode, pooled [B, out_dim])``, the readout's attention written into ``scores`` with
+        ``statements="attention"``.  Node style: ``(logits, rows)``, the node head over every valid node in order (``valid_nodes``:
+        the int32 device word of the valid node count under bucketing, None: every node)."""
         g, dg, idx, fptr = prepared
-        num_graphs = g.batch_size if num_valid is None else num_valid
         m, ws = self.module, self.ws
         eng = _ENGINES[m.engine]
-        pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
-        store = (E._p(self._probs), E._p(self._labels), self.max_predictions)
-        mws = (self._metric_ws.data_ptr(), self._metric_ws.numel(), E._stream_ptr())
-        L = _lib.lib()
-        N = dg.num_nodes
-        scores = torch.empty(N, dtype=torch.float32, device=self.device) if self.statements else None
         if not self._node:
             att = scores if self.statements == "attention" else None
-            _, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, oob_counter=self._oob,
-                                     attention=att)
-            B = dg.batch_size
-            L.call("ddfa_eval_metrics_graph", E._p(logits), E._p(vuln), E._p(dg.graph_ptr), B, B if num_valid is None else int(num_valid),
-                   pw, float(num_graphs), self._state.data_ptr(), *store, *mws)
-            if self._attributes:
-                self._attribute(params, dg, idx, scores)
-            self._statement_metric(scores, vuln, fptr, num_valid)
-            return scores
+            pooled, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws,
+                                          oob_counter=self._oob, attention=att)
+            return logits, pooled
+        N = dg.num_nodes
         x, h_T, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, head=False, oob_counter=self._oob)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
@@ -326,20 +219,18 @@ class FusedEvaluator(CapturedBatches):
         rows = ws.get("node_rows", (N,), torch.int32)
         E.node_sample(vuln, valid_nodes, None, 0, None, rows, self._num_rows, None, alloc=ws)
         logits, _ = E.node_head_fwd(params, x, h_T, rows, self._num_rows, alloc=ws)
-        L.call("ddfa_eval_metrics_rows", E._p(logits), E._p(vuln), E._p(rows), self._num_rows.data_ptr(), N, pw, float(num_graphs),
-               self._state.data_ptr(), *store, *mws)
-        if self.statements:          # rows = every valid node in order, so logits[n] is node n's
-            E._call("ddfa_stmt_node_probability", E._p(logits), self._num_rows.data_ptr(), N, E._p(scores), E._stream_ptr())
-            self._statement_metric(scores, vuln, fptr, num_valid)
-        return scores
+        return logits, rows
 
-    def _statement_metric(self, scores, vuln, fptr, num_valid: Optional[int]) -> None:
-        if self.statements is None:
+    def _scores(self, params, prepared, logits, scores: Optional[torch.Tensor]) -> None:
+        """The per-node scores :meth:`_forward` does not write into ``scores`` (None: none): the node head's probabilities in
+        node style (rows = every valid node in order, so logits[n] is node n's), the gradient modes' attributions in graph style."""
+        if scores is None:
             return
-        B = fptr.numel() - 1
-        mode = _lib.STMT_MODE_FULL if self._node else _lib.STMT_MODE_VULN_ONLY
-        E._call("ddfa_stmt_metric", E._p(scores), E._p(vuln), E._p(fptr), B, B if num_valid is None else int(num_valid), mode, 0.5,
-                self._stmt_state.data_ptr(), self._stmt_ws.data_ptr(), self._stmt_ws.numel(), E._stream_ptr())
+        g, dg, idx, fptr = prepared
+        if self._node:
+            E._call("ddfa_stmt_node_probability", E._p(logits), self._num_rows.data_ptr(), dg.num_nodes, E._p(scores), E._stream_ptr())
+        elif self._attributes:
+            self._attribute(params, dg, idx, scores)
 
     def _attribute(self, params, dg, idx, scores) -> None:
         """Saliency / integrated gradients / DeepLift(Shap) / GradientShap of every function's logit with respect to the
@@ -403,9 +294,161 @@ class FusedEvaluator(CapturedBatches):
 
     def prefetch(self, batch) -> None:
         """Starts the host->device copy of a (pinned) host batch on a side stream, overlapping the batch that is running; the
-        following ``update(batch)`` with the SAME batch object picks the staged copy up.  No-op without ``use_cuda_graph`` or
-        for device batches."""
+        next call that runs the SAME batch object picks the staged copy up.  No-op without ``use_cuda_graph`` or for device
+        batches."""
         self._prefetch(batch, None)
+
+
+class FusedEvaluator(InferencePass):
+    def __init__(self, model: FlowGNNGGNNModule, use_cuda_graph: bool = True, bucket_nodes: int = 0, bucket_edges: int = 0,
+                 max_graph_shapes: int = 8, max_predictions: int = 0, bucket_min_pad_nodes: int = 64, max_resident_graphs: int = 64,
+                 statements: Optional[str] = None, ig_steps: int = 50, shap_samples: Optional[int] = None,
+                 baseline_stdev: float = 0.0, noise_stdev: float = 0.0, attribution_seed: int = 0):
+        """``max_predictions`` > 0 keeps the first that many probabilities and labels (``predictions()``; the reference's
+        ``test_preds`` / ``test_labels``); more samples than that make :meth:`compute` raise, the counts stay complete.
+        ``bucket_nodes`` / ``bucket_edges``: shape bucketing of host batches under ``use_cuda_graph``, as in ``FusedTrainer``
+        (one padding graph, excluded from every metric).  The evaluator reads the module's parameters where they live when a
+        batch runs and never writes them; graphs captured over other parameter storage (a ``FusedTrainer`` built later moves
+        the parameters into its flat buffer) are recaptured.
+        ``statements``: the per-statement score of :meth:`last_scores` and of the statement metrics (``STATEMENT_MODES``):
+        ``"probability"`` (node style: the node head's sigmoid), ``"attention"`` (graph style: the readout's softmax gate α_n,
+        summing to 1 over each function), ``"saliency"`` (graph style: Σ_d |∂logit/∂x_{n,d}| of the embedding output x, captum's
+        ``Saliency(abs=True)``) or ``"integrated_gradients"`` (graph style: Σ_d x_{n,d} · (1/m) Σ_{k<m} ∂logit/∂x_{n,d} at
+        ((k + ½)/m)·x, m = ``ig_steps``, zero baseline: captum's ``IntegratedGradients(method="riemann_middle")``).  The target is
+        each function's own logit; one backward with dlogits = 1 serves every function of the batch.  None (the default)
+        enqueues nothing beyond the classification metrics.
+        ``"deeplift"`` (graph style): captum's ``DeepLift(multiply_by_inputs=True)`` with a zero baseline x̄: Σ_d (x − x̄)_{n,d} ·
+        g̃_{n,d}, g̃ the input gradient with each hidden ReLU of the MLP head under the rescale rule — its derivative replaced by
+        (relu(z) − relu(z̄)) / (z − z̄), z̄ the pre-activation of a full forward of the same graph from x̄ — and every other
+        nonlinearity (GRU gates, pooling softmax, gate products) a plain gradient at the input pass's activations, as captum
+        hooks only ``nn.ReLU`` modules.  ``"deeplift_shap"``: captum's ``DeepLiftShap``, the mean of DeepLift over the baselines
+        b_j = ``baseline_stdev`` · ε_j, j < ``shap_samples`` (default 16); with ``baseline_stdev`` = 0 (the default) every baseline
+        is zero and DeepLift runs once, bit-identical to ``"deeplift"``.  ``"gradient_shap"``: captum's ``GradientShap``, the mean
+        over ``shap_samples`` (default 5) samples s of Σ_d (x̃ − b) · ∂logit/∂x at b + α(x̃ − b), x̃ = x + ``noise_stdev`` · ε,
+        b = ``baseline_stdev`` · ε' (zero by default) and α uniform in [0, 1) per function.  The draws are Philox4x32-10 with key
+        ``attribution_seed`` and a device batch counter (``ddfa_stmt_shap_input``, :attr:`attribution_draws`), advanced once per
+        batch these three modes attribute, so captured replays draw fresh values."""
+        if model.device.type != "cuda":
+            raise _lib.DdfaError("FusedEvaluator needs the module on a CUDA device (no CPU fallback)")
+        hp = model.hparams
+        if hp.encoder_mode or model._num_layers == 0:
+            raise ValueError("FusedEvaluator: an encoder_mode module returns embeddings, not logits: there is nothing to score")
+        if hp.label_style not in ("graph", "node"):
+            raise ValueError(f"FusedEvaluator: label_style={hp.label_style!r} is not supported ('graph' or 'node')")
+        if int(max_predictions) < 0:
+            raise ValueError(f"max_predictions must be >= 0, got {max_predictions!r}")
+        self._init_inference(model, statements, ig_steps, shap_samples, baseline_stdev, noise_stdev, attribution_seed, use_cuda_graph,
+                             bucket_nodes, bucket_edges, max_graph_shapes, bucket_min_pad_nodes, max_resident_graphs)
+        self.max_predictions = int(max_predictions)
+        L = _lib.lib()
+        dev = self.device
+        with torch.cuda.device(dev):
+            self._state = torch.zeros(_lib.EVAL_STATE_WORDS, dtype=torch.float64, device=dev)
+            self._metric_ws = torch.empty(L.call("ddfa_eval_metrics_workspace_bytes"), dtype=torch.uint8, device=dev)
+            cap = max(self.max_predictions, 1)
+            self._probs = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
+            self._labels = torch.zeros(cap, dtype=torch.float32, device=dev) if self.max_predictions else None
+            self._stmt_state = torch.zeros(_lib.STMT_STATE_WORDS, dtype=torch.float64, device=dev)
+            self._stmt_ws = torch.empty(L.call("ddfa_stmt_metric_workspace_bytes"), dtype=torch.uint8, device=dev) if statements else None
+        self._last_scores = None
+
+    # ---- the metric state ------------------------------------------------------------------------------------------------
+    def reset(self) -> None:
+        """Zeroes the metric state and the statement state in stream order (the prediction store starts over at position 0)."""
+        self._state.zero_()
+        self._stmt_state.zero_()
+
+    def state(self) -> torch.Tensor:
+        """The float64 device metric state (``EVAL_STATE_WORDS`` words, layout in include/ddfa_b200.h), a view: the evaluator
+        keeps accumulating into it.  Every word is a sum, so ``dist.all_reduce(ev.state())`` adds ranks exactly (integers below
+        2**53) and :meth:`metrics_from_state` turns the sum into the global metrics."""
+        return self._state
+
+    metrics_from_state = staticmethod(metrics_from_state)
+    statement_metrics_from_state = staticmethod(statement_metrics_from_state)
+
+    def statement_state(self) -> torch.Tensor:
+        """The float64 device statement state (``STMT_STATE_WORDS`` words, layout in include/ddfa_b200.h, DDFA_STMT_STATE_WORDS),
+        a view, separate from :meth:`state`.  Every word is an integer count, so ``dist.all_reduce(ev.statement_state())`` adds
+        ranks exactly and :meth:`statement_metrics_from_state` turns the sum into the global statement metrics."""
+        return self._stmt_state
+
+    def last_scores(self) -> torch.Tensor:
+        """The fp32 device scores ``[N]`` of the last batch's statements, in the batch's node order (without the padding graph's
+        nodes under bucketing).  The next :meth:`update` overwrites them: copy them per batch to keep them."""
+        if self.statements is None:
+            raise ValueError("FusedEvaluator.last_scores: built with statements=None (no per-statement score)")
+        if self._last_scores is None:
+            raise ValueError("FusedEvaluator.last_scores: no batch was evaluated yet")
+        return self._last_scores
+
+    def compute(self, prefix: str = "val_") -> dict:
+        """The metrics of everything evaluated since the last :meth:`reset` (one synchronisation).  Raises ``ValueError`` when
+        no sample was evaluated or predictions overflowed ``max_predictions``, and ``IndexError`` when a batch had node feature
+        indices outside the embedding tables."""
+        s = self._state.cpu()
+        bad = int(self._oob.item())
+        if bad:
+            self._oob.zero_()
+            raise IndexError(f"{bad} node feature indices outside [0, {self.module.input_dim}) in an evaluated batch")
+        n = int(s[TP] + s[FP] + s[TN] + s[FN])
+        if n == 0:
+            raise ValueError("FusedEvaluator.compute: no sample was evaluated since the last reset()")
+        if self._probs is not None and s[OVERFLOW] > 0:
+            raise ValueError(f"FusedEvaluator.compute: {n} predictions, max_predictions={self.max_predictions}: build the "
+                             f"evaluator with max_predictions >= {n}")
+        out = metrics_from_state(s, prefix)
+        if self.statements is not None:
+            ss = self._stmt_state.cpu()
+            if ss[S_NAN] > 0:
+                raise ValueError(f"FusedEvaluator.compute: {int(ss[S_NAN])} functions had a NaN statement score "
+                                 f"(statements={self.statements!r})")
+            out.update(statement_metrics_from_state(ss, prefix, node_style=self._node))
+        return out
+
+    def predictions(self):
+        """``(probs, labels)``: fp32 device tensors of the first ``min(stored, max_predictions)`` samples in evaluation order
+        (graph order, or node order within a batch).  Reads the stored count: one synchronisation."""
+        if self._probs is None:
+            raise ValueError("FusedEvaluator.predictions: built with max_predictions=0 (no prediction store)")
+        k = int(self._state[STORED].item())
+        return self._probs[:k], self._labels[:k]
+
+    # ---- per batch -------------------------------------------------------------------------------------------------------
+    def _enqueue(self, params, prepared, vuln, num_valid: Optional[int], valid_nodes: Optional[torch.Tensor]):
+        """Enqueues one batch (``prepared``: what :meth:`_prepare` made of it) over ``params``: the inference forward and the
+        metric kernel, then, with ``statements``, the per-node scores and the statement metric.  ``num_valid``: graphs
+        [num_valid, B) are bucket padding (the real ones are the batch's weight in the loss mean); ``valid_nodes``: the int32
+        device word of the valid node count in node style under bucketing.  Returns the scores (None without ``statements``):
+        a fresh [N] tensor, which a captured graph keeps writing on every replay."""
+        g, dg, idx, fptr = prepared
+        num_graphs = g.batch_size if num_valid is None else num_valid
+        m = self.module
+        pw = 1.0 if m.hparams.positive_weight is None else float(m.hparams.positive_weight)
+        store = (E._p(self._probs), E._p(self._labels), self.max_predictions)
+        mws = (self._metric_ws.data_ptr(), self._metric_ws.numel(), E._stream_ptr())
+        L = _lib.lib()
+        N = dg.num_nodes
+        scores = torch.empty(N, dtype=torch.float32, device=self.device) if self.statements else None
+        logits, rows = self._forward(params, prepared, vuln, valid_nodes, scores)
+        if not self._node:
+            B = dg.batch_size
+            L.call("ddfa_eval_metrics_graph", E._p(logits), E._p(vuln), E._p(dg.graph_ptr), B, B if num_valid is None else int(num_valid),
+                   pw, float(num_graphs), self._state.data_ptr(), *store, *mws)
+        else:
+            L.call("ddfa_eval_metrics_rows", E._p(logits), E._p(vuln), E._p(rows), self._num_rows.data_ptr(), N, pw, float(num_graphs),
+                   self._state.data_ptr(), *store, *mws)
+        self._scores(params, prepared, logits, scores)
+        self._statement_metric(scores, vuln, fptr, num_valid)
+        return scores
+
+    def _statement_metric(self, scores, vuln, fptr, num_valid: Optional[int]) -> None:
+        if self.statements is None:
+            return
+        B = fptr.numel() - 1
+        mode = _lib.STMT_MODE_FULL if self._node else _lib.STMT_MODE_VULN_ONLY
+        E._call("ddfa_stmt_metric", E._p(scores), E._p(vuln), E._p(fptr), B, B if num_valid is None else int(num_valid), mode, 0.5,
+                self._stmt_state.data_ptr(), self._stmt_ws.data_ptr(), self._stmt_ws.numel(), E._stream_ptr())
 
     def update(self, batch) -> None:
         """Adds one batch (host, resident device or DGL batch; ``(batch, extrafeats)`` tuples as Lightning hands them over are

@@ -586,6 +586,36 @@ int ddfa_stmt_shap_input(const float *x, const int32_t *graph_ptr, int32_t num_g
                          float *diff, void *image, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K9''  prediction store (csrc/predict.cu): per function of a batch, its probability, its DDFA embedding and its top-k
+ * statements, appended to a device result store at a device cursor.  Nothing is read from the host, so the call can be
+ * captured into a CUDA graph and every replay appends.
+ *
+ * ddfa_predict_store: function b < num_valid owns nodes [graph_ptr[b], graph_ptr[b+1]) (int32 [num_graphs + 1]; label_style="node":
+ *   the function-level graph_ptr) and goes to store position p = cursor[0] + b, cursor[0] read on the device.  Positions
+ *   >= capacity are dropped and counted in cursor[1]; cursor[0] advances by the number stored.  Functions [num_valid, num_graphs)
+ *   are bucket padding and are ignored.  cursor: int64[2] on the device, [0] stored, [1] dropped, 8-byte aligned.
+ *   prob_out (fp32 [capacity]), given exactly when logits or node_probs is (never both):
+ *     logits (graph style, fp32 [num_graphs]): prob_out[p] = 1.f / (1.f + expf(-logits[b])), the p of ddfa_eval_metrics_*;
+ *     node_probs (node style, fp32 per node): the maximum over the function's nodes (a function is flagged when any statement is,
+ *     evaluate.py:276); a NaN among them gives NaN, a function without nodes 0.
+ *   emb_out (fp32 [capacity, out_dim]), given exactly when pooled (fp32 [num_graphs, out_dim]) is: emb_out[p, :] = pooled[b, :].
+ *   top_idx_out (int32 [capacity, k]) / top_score_out (fp32 [capacity, k]), given with scores (fp32 per node) exactly when k > 0,
+ *     0 <= k <= DDFA_PREDICT_MAX_K: rank j's node index local to the function (n - graph_ptr[b]) and its raw score.  The ranking
+ *     is ddfa_stmt_metric's: score descending, equal scores (-0.0 == +0.0) in node order (Python's stable sorted(...,
+ *     reverse=True)); NaN ranks after every number, -inf included, NaNs in node order.  Ranks j >= the function's node count
+ *     get -1 and NaN.
+ *   One CTA per function (grid-stride over min(num_graphs, 264) CTAs), min(k, nodes) selection rounds over its scores, each
+ *   the maximum of a unique 64-bit (score, node) key below the previous round's: exact, no atomics, bit-reproducible in both
+ *   DDFA_TUNE_DETERMINISTIC modes, correct for any segment length.  Two launches (the second advances the cursor), none when
+ *   num_valid == 0.
+ * ------------------------------------------------------------------------------------- */
+#define DDFA_PREDICT_MAX_K 32
+int ddfa_predict_store(const float *logits, const float *node_probs, const float *pooled, int32_t out_dim, const float *scores,
+                       int32_t k, const int32_t *graph_ptr, int32_t num_graphs, int32_t num_valid, float *prob_out,
+                       float *emb_out, int32_t *top_idx_out, float *top_score_out, int64_t *cursor, int64_t capacity,
+                       void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K10  torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 (DDFA/configs/
  * config_default.yaml:43-47) over one flat parameter buffer.  step_count: int32[1] device
  * counter, incremented by the kernel (graph-capture safe).
