@@ -49,6 +49,8 @@ _SIGNATURES = {
     "ddfa_graph_ptr": (_int, [_vp, _i32, _vp, _vp]),
     "ddfa_arena_batch_workspace_bytes": (_sz, [_i32]),
     "ddfa_arena_batch": (_int, [_vp, _i32, _i32] + [_vp] * 6 + [_i32, _vp, _i32, _i32] + [_vp] * 7 + [_vp, _sz, _vp]),
+    "ddfa_cache_batch_workspace_bytes": (_sz, [_i32]),
+    "ddfa_cache_batch": (_int, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "ddfa_embed_concat_fwd": (_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_embed_concat_fwd_image": (_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "ddfa_embed_concat_bwd": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
@@ -139,7 +141,7 @@ TUNE_L2_HINTS, TUNE_PDL_MASK, TUNE_GATHER_VARIANT, TUNE_FWD_PAIR, TUNE_GATE_BWD_
 TUNE_DETERMINISTIC = 6
 
 _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_version", "ddfa_last_error", "ddfa_device_supported", "ddfa_launch_count", "ddfa_engine_available",
-              "ddfa_build_csr_workspace_bytes", "ddfa_arena_batch_workspace_bytes", "ddfa_gru_step_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes_steps",
+              "ddfa_build_csr_workspace_bytes", "ddfa_arena_batch_workspace_bytes", "ddfa_cache_batch_workspace_bytes", "ddfa_gru_step_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes", "ddfa_gru_step_bwd_workspace_bytes_steps",
               "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes",
               "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
               "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes",

@@ -7,7 +7,9 @@ from __future__ import annotations
 import torch
 
 from . import _lib
+from . import engine as E
 from .batched_graph import BatchedCFG, as_batched_cfg
+from .encoder_cache import EncoderCache
 
 
 def graph_step(device, graph, warm: bool, enqueue):
@@ -129,6 +131,20 @@ def push_ids(slot, ids_np) -> None:
         slot["keep"][0].check()      # the assembler's device error counter (bad id / totals mismatch): one sync every 256 steps
 
 
+def new_cache_slot(cache, B: int, N: int) -> dict:
+    """An arena slot's counterpart for an :class:`~deepdfa_b200.encoder_cache.EncoderCache`: the static outputs of
+    ``ddfa_cache_batch`` and the same ring of pinned id stages."""
+    return {"out": cache.alloc_outputs(B, N), "stages": [torch.empty(B, dtype=torch.int32).pin_memory() for _ in range(4)],
+            "stage_done": [None] * 4, "turn": 0, "steps": 0,
+            "graph": None, "warm": False, "keep": None, "arena": cache}     # the cache stays alive with its graph
+
+
+def cache_graph(cb) -> E.DeviceGraph:
+    """The :class:`~deepdfa_b200.engine.DeviceGraph` of a batch gathered from an encoder cache: graph_ptr only (no CSR; what
+    runs after the GGNN reads none)."""
+    return E.DeviceGraph(cb.num_nodes(), 0, cb.batch_size, None, None, None, None, cb.graph_ptr, cb.device)
+
+
 class CapturedBatches:
     """The three batch paths, their caches and their capture policy, for a class that runs one batch at a time.
 
@@ -143,7 +159,11 @@ class CapturedBatches:
       on the device, ``num_valid`` the real graph count under bucketing (None: every graph is real), ``valid_nodes`` the int32
       device word of the real node count in node style under bucketing (None: every node is real).  What it returns is kept
       with the captured graph;
-    * ``_after_run(result, num_nodes)``: after every run, replays included, with that result and the batch's real node count.
+    * ``_after_run(result, num_nodes)``: after every run, replays included, with that result and the batch's real node count;
+    * ``_check_cache(cache, who)`` and ``_prepare_cache(cb)``: the id path over an encoder cache (``_run_ids`` with an
+      :class:`~deepdfa_b200.encoder_cache.EncoderCache`): what the owner refuses to run from cached rows (it raises), and the
+      ``prepared`` tuple of a gathered batch, whose device graph has graph_ptr only and whose embedding indices are the
+      :class:`~deepdfa_b200.encoder_cache.CachedRows`.
 
     ``_stream_slots`` (host and arena slots) and ``_graphs`` (resident graphs, the graph at index 0 of each entry) are the live
     caches: clearing them drops the captured graphs."""
@@ -248,6 +268,8 @@ class CapturedBatches:
 
     # ---- graph ids of an arena, assembled inside the captured graph ----------------------------------------------------------
     def _run_ids(self, arena, ids, ctx, who: str) -> None:
+        if isinstance(arena, EncoderCache):
+            return self._run_cache(arena, ids, ctx, who)
         if not self.use_cuda_graph:
             return self._run_resident(arena.batch(ids), ctx)
         ids_np, B, N, Eg = arena_ids(arena, ids, who)
@@ -271,6 +293,56 @@ class CapturedBatches:
             slot["graph"] = graph_step(self.device, slot["graph"], slot["warm"], enqueue)
             slot["warm"] = True
             self._after_run(slot["result"], N)
+
+    def _run_cache(self, cache, ids, ctx, who: str) -> None:
+        """Graph ids over an encoder cache: the batch's rows, labels and graph_ptr gathered by ``ddfa_cache_batch`` into static
+        per-shape buffers inside the captured graph, then the owner's launches after the GGNN.  The cache is checked against the
+        module first, so a stale captured graph is never replayed; a cache that fails the check loses its slots, and so does,
+        when a new slot is made, every other cache that no longer matches the module.  Beyond ``max_graph_shapes`` slots, or without
+        ``use_cuda_graph``, the same launches run eagerly over freshly allocated outputs."""
+        self._check_cache(cache, who)
+        try:
+            cache.check(self.module)
+        except ValueError:
+            self._drop_cache_slots(lambda c: c is cache)      # its graphs can never replay again: free them and the cache
+            raise
+        ids_np, B, N, _ = arena_ids(cache.arena, ids, who)
+        key = ("cache", id(cache), N, B, _lib.deterministic_requested()) + self._key_suffix(ctx, B)
+        with torch.cuda.device(self.device):
+            slot = self._stream_slots.get(key) if self.use_cuda_graph else None
+            if slot is None and self.use_cuda_graph:
+                # slots of caches that no longer match the module (a rebuilt cache's predecessor) hold the old planes and
+                # count against max_graph_shapes: they go before a new slot is counted
+                self._drop_cache_slots(lambda c: c is not cache and not c.matches(self.module))
+                if len(self._stream_slots) < self.max_graph_shapes:
+                    slot = new_cache_slot(cache, B, N)
+                    self._stream_slots[key] = slot
+            if slot is None:
+                cb = cache.batch(ids_np)
+                self._after_run(self._enqueue(ctx, self._prepare_cache(cb), self._vuln(cb), None, None), N)
+                return
+            push_ids(slot, ids_np)
+
+            def enqueue():
+                cb = cache._assemble(slot["out"]["ids"], B, N, slot["out"])
+                prepared = self._prepare_cache(cb)
+                vuln = self._vuln(cb)
+                slot["result"] = self._enqueue(ctx, prepared, vuln, None, None)
+                slot["keep"] = prepared + (vuln,)       # keep[0]: the gathered batch, whose error counter push_ids checks
+
+            slot["graph"] = graph_step(self.device, slot["graph"], slot["warm"], enqueue)
+            slot["warm"] = True
+            self._after_run(slot["result"], N)
+
+    def _drop_cache_slots(self, stale) -> None:
+        """Forgets the slots (static outputs, captured graph, id stages) of every encoder cache ``c`` with ``stale(c)``, and with
+        them this owner's references to those caches, so a cache nothing else holds is freed.  Waits for the device first when
+        a captured graph is among them: it may still be running."""
+        keys = [k for k, s in self._stream_slots.items() if k[0] == "cache" and stale(s["arena"])]
+        if any(self._stream_slots[k]["graph"] is not None for k in keys):
+            torch.cuda.synchronize(self.device)
+        for k in keys:
+            del self._stream_slots[k]
 
     # ---- device-resident batch objects, or eager launches --------------------------------------------------------------------
     def _run_resident(self, batch, ctx) -> None:

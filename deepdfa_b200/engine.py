@@ -416,6 +416,20 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
             saved = Saved(T, D, x, hs, ss, gs, w_fold, b_fold, None, None, None, None, None, idx,
                           h_img=h_imgs if use_images else None)
         return x, h_cur, saved
+    pooled, logits, gate_logit, seg_max, seg_sum, mlp_act = _readout(params, dg, x, h_cur, training, alloc, attention)
+    saved = None
+    if training:
+        saved = Saved(T, D, x, hs, ss, gs, w_fold, b_fold, pooled, gate_logit, seg_max, seg_sum, mlp_act, idx,
+                      h_img=h_imgs if use_images else None)
+    return pooled, logits, saved
+
+
+def _readout(params: ParamPack, dg: DeviceGraph, x: torch.Tensor, h_final: torch.Tensor, training: bool, alloc, attention):
+    """The readout + MLP head over the rows ``x`` / ``h_final`` ([N, D]) of the batch ``dg`` (its graph_ptr only):
+    ``(pooled, logits, gate_logit, seg_max, seg_sum, mlp_act)``, the last four kept for the backward when ``training``."""
+    N, D = x.shape
+    B = dg.batch_size
+    nl = len(params.mlp_w)
     pooled = alloc.get("pooled", (B, 2 * D))
     logits = alloc.get("logits", (B,)) if nl > 0 else None
     keep_gate = training or attention is not None
@@ -423,17 +437,32 @@ def forward(params: ParamPack, dg: DeviceGraph, idx: List[torch.Tensor], n_steps
     seg_max = alloc.get("seg_max", (B,)) if keep_gate else None
     seg_sum = alloc.get("seg_sum", (B,)) if keep_gate else None
     mlp_act = alloc.get("mlp_act", (max(nl - 1, 1), B, 2 * D)) if (training and nl > 1) else None
-    _call("ddfa_readout_mlp_fwd", _p(h_cur), _p(x), _p(dg.graph_ptr), B, D, _p(params.w_gate), _p(params.b_gate),
+    st = _stream_ptr()
+    _call("ddfa_readout_mlp_fwd", _p(h_final), _p(x), _p(dg.graph_ptr), B, D, _p(params.w_gate), _p(params.b_gate),
            ptr_array([_p(t) for t in params.mlp_w]) if nl else None,
            ptr_array([_p(t) for t in params.mlp_b]) if nl else None,
            nl, _p(pooled), _p(logits), _p(gate_logit), _p(seg_max), _p(seg_sum), _p(mlp_act), st)
     if attention is not None:
         _call("ddfa_stmt_attention", _p(gate_logit), _p(seg_max), _p(seg_sum), _p(dg.graph_ptr), B, _p(attention), st)
-    saved = None
-    if training:
-        saved = Saved(T, D, x, hs, ss, gs, w_fold, b_fold, pooled, gate_logit, seg_max, seg_sum, mlp_act, idx,
-                      h_img=h_imgs if use_images else None)
-    return pooled, logits, saved
+    return pooled, logits, gate_logit, seg_max, seg_sum, mlp_act
+
+
+def readout_forward(params: ParamPack, dg: DeviceGraph, x: torch.Tensor, h_final: torch.Tensor, n_steps: int, *, training: bool,
+                    alloc=None, attention: Optional[torch.Tensor] = None):
+    """The readout + MLP head of :func:`forward` over given GGNN outputs — the rows an encoder cache gathered (``x`` the
+    embedding rows, ``h_final`` h_T, [N, D] each) — with no embedding and no GGNN launch: ``(pooled, logits, Saved or None)``,
+    the Saved holding x, h_T and the readout state, what ``backward(..., grad_ggnn=False)`` reads.  ``dg`` needs graph_ptr
+    only."""
+    _require_cuda(*params.flat_list(), x, h_final, dg.graph_ptr)
+    _lib.apply_deterministic_mode()
+    alloc = alloc or _FreshAlloc(dg.device)
+    T, D = n_steps, x.shape[1]
+    pooled, logits, gate_logit, seg_max, seg_sum, mlp_act = _readout(params, dg, x, h_final, training, alloc, attention)
+    if not training:
+        return pooled, logits, None
+    hs = [None] * (T + 1)
+    hs[0], hs[T] = x, h_final
+    return pooled, logits, Saved(T, D, x, hs, [], [], None, None, pooled, gate_logit, seg_max, seg_sum, mlp_act, [])
 
 
 def backward(params: ParamPack, dg: DeviceGraph, saved: Saved, grads: ParamPack, *, dlogits: Optional[torch.Tensor] = None,

@@ -29,7 +29,8 @@ import torch
 from . import _lib
 from . import engine as E
 from .batched_graph import as_batched_cfg
-from .capture import CapturedBatches
+from .capture import CapturedBatches, cache_graph
+from .encoder_cache import CachedRows
 from .module import FlowGNNGGNNModule, _ENGINES
 
 # the fp64 words of the metric state (include/ddfa_b200.h, DDFA_EVAL_STATE_WORDS)
@@ -198,6 +199,17 @@ class InferencePass(CapturedBatches):
         idx = E.node_indices(g, m.concat_all_absdf, m.feature_keys["feature"], self.device)
         return g, dg, idx, fptr
 
+    def _prepare_cache(self, cb):
+        """A batch gathered from an encoder cache: its graph_ptr-only device graph (per node in node style), the function-level
+        graph_ptr and the cached rows in place of the embedding indices."""
+        dg = cache_graph(cb)
+        return cb, E.per_node_view(cb, dg) if self._node else dg, cb.rows, dg.graph_ptr
+
+    def _check_cache(self, cache, who: str) -> None:
+        if self._attributes:
+            raise ValueError(f"{who}: statements={self.statements!r} differentiates through the GGNN, which an EncoderCache "
+                             "skips; pass a GraphArena, or use statements='attention', 'probability' or None")
+
     def _forward(self, params, prepared, vuln, valid_nodes: Optional[torch.Tensor], scores: Optional[torch.Tensor]):
         """The inference forward of one batch (``prepared``: what :meth:`_prepare` made of it) over ``params``.  Graph style:
         ``(logits [B] or None in encoder_mode, pooled [B, out_dim])``, the readout's attention written into ``scores`` with
@@ -206,13 +218,22 @@ class InferencePass(CapturedBatches):
         g, dg, idx, fptr = prepared
         m, ws = self.module, self.ws
         eng = _ENGINES[m.engine]
+        cached = isinstance(idx, CachedRows)       # an encoder cache's rows: no embedding, no GGNN launch
         if not self._node:
             att = scores if self.statements == "attention" else None
-            pooled, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws,
-                                          oob_counter=self._oob, attention=att)
+            if cached:
+                pooled, logits, _ = E.readout_forward(params, dg, idx.x, idx.h, m.hparams.n_steps, training=False, alloc=ws,
+                                                      attention=att)
+            else:
+                pooled, logits, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws,
+                                              oob_counter=self._oob, attention=att)
             return logits, pooled
         N = dg.num_nodes
-        x, h_T, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, head=False, oob_counter=self._oob)
+        if cached:
+            x, h_T = idx.x, idx.h
+        else:
+            x, h_T, _ = E.forward(params, dg, idx, m.hparams.n_steps, training=False, engine=eng, alloc=ws, head=False,
+                                  oob_counter=self._oob)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
             valid_nodes.fill_(N)
@@ -459,7 +480,11 @@ class FusedEvaluator(InferencePass):
 
     def update_ids(self, arena, ids) -> None:
         """Adds the graphs ``ids`` of a device-resident :class:`~deepdfa_b200.arena.GraphArena` (assembled by
-        ``ddfa_arena_batch`` inside the captured graph: the H2D copy of the id list plus one graph launch per batch)."""
+        ``ddfa_arena_batch`` inside the captured graph: the H2D copy of the id list plus one graph launch per batch).
+        ``arena`` may also be an :class:`~deepdfa_b200.encoder_cache.EncoderCache` of this module: the batch's cached GGNN rows
+        are gathered (``ddfa_cache_batch``) and only the readout / node head and the metrics run.  ``statements=None``,
+        ``"attention"`` and ``"probability"`` only (the gradient modes raise ``ValueError``); ``ValueError`` when the module's
+        encoder changed since the cache was built."""
         self._run_ids(arena, ids, self._params(), "update_ids")
 
     def _after_run(self, scores, num_nodes: int) -> None:

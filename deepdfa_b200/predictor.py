@@ -96,7 +96,9 @@ class FusedPredictor(InferencePass):
 
     def predict_ids(self, arena, ids) -> None:
         """Predicts the graphs ``ids`` of a device-resident :class:`~deepdfa_b200.arena.GraphArena`, assembled inside the captured
-        graph."""
+        graph.  ``arena`` may also be an :class:`~deepdfa_b200.encoder_cache.EncoderCache` of this module, as for
+        ``FusedEvaluator.update_ids``: only the readout / node head runs over the cached rows (``encoder_mode``: the embedding is
+        the readout's pooled vector over them); ``statements=None``, ``"attention"`` or ``"probability"``."""
         self._run_ids(arena, ids, self._params(), "predict_ids")
 
     # ---- per batch -------------------------------------------------------------------------------------------------------

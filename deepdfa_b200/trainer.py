@@ -24,7 +24,8 @@ import torch.distributed as dist
 
 from . import _lib
 from . import engine as E
-from .capture import CapturedBatches
+from .capture import CapturedBatches, cache_graph
+from .encoder_cache import CachedRows, encoder_names
 from .module import FlowGNNGGNNModule, _ENGINES
 
 _ALIGN = 64  # elements; keeps every parameter 256-byte aligned inside the flat buffers
@@ -917,8 +918,11 @@ class FusedTrainer(CapturedBatches):
                                                                  self._num_rows.data_ptr(), dg.num_nodes),
                                       pw, g.batch_size if num_valid is None else num_valid)
             return rows
-        _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws,
-                                     grad_ggnn=self._grad_ggnn)
+        if isinstance(idx, CachedRows):      # an encoder cache's rows: the readout over them, no GGNN launch
+            _, logits, saved = E.readout_forward(self.params, dg, idx.x, idx.h, m.hparams.n_steps, training=True, alloc=self.ws)
+        else:
+            _, logits, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=self.ws,
+                                         grad_ggnn=self._grad_ggnn)
         prune = dict(grad_ggnn=self._grad_ggnn, grad_tables=self._grad_tables)
         global_batch = self._global_batch(global_batch, dg.batch_size if num_valid is None else num_valid)
         # the gradient of loss / k (k = 1: 1 / global_batch as ever); the loss itself stays the micro-batch's mean
@@ -984,8 +988,7 @@ class FusedTrainer(CapturedBatches):
         factor = m.hparams.undersample_node_on_loss_factor
         if self.world > 1:
             return self._enqueue_node_dp(dg, idx, vuln, eng, pw, valid_nodes, phase)
-        x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False,
-                                  grad_ggnn=self._grad_ggnn)
+        x, h_T, saved = self._node_rows(dg, idx, eng)
         if valid_nodes is None:
             valid_nodes = ws.get("node_valid", (1,), torch.int32)
             valid_nodes.fill_(N)
@@ -1010,14 +1013,20 @@ class FusedTrainer(CapturedBatches):
         self._sample_stream.wait_stream(main)
         with torch.cuda.stream(self._sample_stream):      # it needs _VULN and the valid count only: under the GGNN forward
             draw.run(self._sum_ints)
-        x, h_T, saved = E.forward(self.params, dg, idx, m.hparams.n_steps, training=True, engine=eng, alloc=ws, head=False,
-                                  grad_ggnn=self._grad_ggnn)
+        x, h_T, saved = self._node_rows(dg, idx, eng)
         main.wait_stream(self._sample_stream)
         logits, act = E.node_head_fwd(self.params, x, h_T, rows, self._num_rows, alloc=ws)
         self._last_logits = logits
         dlogits = E.node_bce_global(logits, vuln, rows, self._num_rows, self._s_global, pw,
                                     self._loss_local if self.exchange == "p2p" else self.loss_slot, grad_scale=1.0 / self._k, alloc=ws)
         return self._node_backward(dg, saved, eng, dlogits, x, h_T, rows, act, phase)
+
+    def _node_rows(self, dg, idx, eng):
+        """``(x, h_T, Saved or None)`` of a node-style step: the GGNN forward without the readout, or an encoder cache's rows."""
+        if isinstance(idx, CachedRows):
+            return idx.x, idx.h, None
+        return E.forward(self.params, dg, idx, self.module.hparams.n_steps, training=True, engine=eng, alloc=self.ws, head=False,
+                         grad_ggnn=self._grad_ggnn)
 
     def _node_backward(self, dg, saved, eng, dlogits, x, h_T, rows, act, phase):
         ws = self.ws
@@ -1051,6 +1060,18 @@ class FusedTrainer(CapturedBatches):
     def _prepare(self, batch):
         return self.module._prepare(batch)
 
+    def _prepare_cache(self, cb):
+        return cb, E.per_node_view(cb, cache_graph(cb)) if self._node else cache_graph(cb), cb.rows
+
+    def _check_cache(self, cache, who: str) -> None:
+        """A cache holds what a FROZEN encoder computes: a trainer that trains any encoder tensor refuses it."""
+        if self._grad_ggnn:
+            ntab = len(self.module._tables())
+            names = [n for n, t in zip(encoder_names(self.module), self._trainable[:ntab + 6]) if t]
+            raise ValueError(f"{who}: an EncoderCache holds the output of a frozen graph encoder, but this trainer trains the encoder "
+                             f"tensor(s) {names}; freeze the embedding tables and the GatedGraphConv (requires_grad_(False)) before "
+                             "building the trainer, or pass a GraphArena")
+
     def _key_suffix(self, ctx, B: int) -> tuple:
         global_batch, phase = ctx
         return (self._global_batch(global_batch, B),) + self._phase_key(phase)
@@ -1065,7 +1086,14 @@ class FusedTrainer(CapturedBatches):
         """One optimisation step on the graphs ``ids`` of a device-resident :class:`deepdfa_b200.arena.GraphArena` (SURVEY.md §8
         f1: the batch producer).  With ``use_cuda_graph`` the batch is assembled into static per-shape buffers by
         ``ddfa_arena_batch`` inside one captured graph, so a step costs the H2D copy of the id list plus one graph launch;
-        otherwise it is ``step(arena.batch(ids))``.  One micro-batch, as :meth:`step`."""
+        otherwise it is ``step(arena.batch(ids))``.  One micro-batch, as :meth:`step`.
+
+        ``arena`` may also be an :class:`~deepdfa_b200.encoder_cache.EncoderCache` of this trainer's module when the trainer
+        was built over a frozen encoder (embedding tables and GatedGraphConv with ``requires_grad=False``; ``ValueError``
+        otherwise, naming the trainable encoder tensors).  The step is then the frozen step with the GGNN forward replaced by
+        ``ddfa_cache_batch``, a gather of the graphs' cached rows; everything after it (readout or node head, loss, their
+        backward, exchange, guard, Adam, metrics, accumulation) is unchanged.  The cache is checked against the module first
+        (``EncoderCache.check``: ``ValueError`` when the encoder changed), so a captured step is never replayed over stale rows."""
         phase = self._begin()
         self._run_ids(arena, ids, (global_batch, phase), "step_ids")
         return self._end(phase)

@@ -127,6 +127,28 @@ int ddfa_arena_batch(const int32_t *graph_ids, int32_t batch_size, int32_t num_g
                      int32_t *out_indptr_t, int32_t *out_indices_t, int64_t *const *out_feats, int32_t *out_vuln,
                      void *workspace, size_t workspace_bytes, void *stream);
 
+/* Batch assembly from an encoder cache: the output of a FROZEN graph encoder (embedding + GatedGraphConv), computed once for
+ * every node of an arena and kept as two fp32 planes h_all = h_T and x_all = the embedding rows, [num_nodes_all, D] each in
+ * arena node order (node_off int32[num_graphs + 1] and vuln_all int32[num_nodes_all] as for ddfa_arena_batch).
+ * Out, for the graphs graph_ids[0..B) in that order: graph_ptr int32[B+1], _VULN int32[N] and the rows of both planes,
+ * out_h / out_x fp32 [N, D] — what the readout, the node head and their backward read.  No CSR is built and no edge is read.
+ * batch_nodes = N, the batch's node total (the caller knows it from its host copy of the graph sizes).  Each graph's rows
+ * are one contiguous slab per plane, cut into chunks of 128 float4 (2 KB per plane), one warp per chunk: a graph gets
+ * ceil(n * D / 512) warps' worth of work, a 0-node graph none, so a large graph in a skewed batch is spread over as many
+ * warps as its size needs.  Row offsets are 64-bit (a Big-Vul-size plane passes 2^32 bytes).  D: a positive multiple of 4;
+ * h_all, x_all, out_h and out_x 16-byte aligned.  Output pointers may be NULL when N = 0.
+ * Error contract of ddfa_arena_batch: a bad id (outside [0, num_graphs), or whose nodes lie outside [0, num_nodes_all)) or
+ * a node total other than batch_nodes leaves every output untouched and raises the int32 counter at workspace[0]: its low
+ * 16 bits count bad ids, bit 16 flags the total.  Only device words are read: the call is capturable.  Workspace layout
+ * (ddfa_cache_batch_workspace_bytes(B) bytes): int32 counter, int32 node_ptr[B + 1] (graph_ptr staged until the ids are
+ * known to be good), int32 chunk_ptr[B + 1] (each graph's first chunk).  A short workspace returns DDFA_ERR_WORKSPACE
+ * before any launch. */
+size_t ddfa_cache_batch_workspace_bytes(int32_t batch_size);
+int ddfa_cache_batch(const int32_t *graph_ids, int32_t batch_size, int32_t num_graphs, const int32_t *node_off,
+                     const int32_t *vuln_all, const float *h_all, const float *x_all, int32_t num_nodes_all, int32_t D,
+                     int32_t batch_nodes, int32_t *out_graph_ptr, int32_t *out_vuln, float *out_h, float *out_x,
+                     void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * K1  embedding + concat.  Replaces ggnn.py:84-92 (4x nn.Embedding + torch.cat, or one).
  * idx[k]: int64[N] with values in [0,V); tables[k]: fp32[V,H]; x: fp32[N, K*H].
