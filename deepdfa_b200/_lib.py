@@ -132,6 +132,9 @@ _SIGNATURES = {
     "ddfa_stmt_attribution_score": (_int, [_vp, _vp, _vp, _i32, _i32, _f32, _i32, _vp, _vp]),
     "ddfa_stmt_shap_input": (_int, [_vp, _vp, _i32, _i32, _i32, _f32, _f32, _f32, C.c_uint64, _vp, _i32, _vp, _vp, _vp, _vp]),
     "ddfa_predict_store": (_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "ddfa_curve_workspace_bytes": (_sz, [_i64]),
+    "ddfa_curve_sort": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ddfa_curve_metrics": (_int, [_vp, _vp, _vp, _i64, _vp, _i32] + [_vp] * 10 + [_vp, _sz, _vp]),
     "ddfa_mlp_dgrad_rescale": (_int, [_vp] * 7 + [_i32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_grad_accumulate": (_int, [_vp, _vp, _i64, _i64, _i32, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
@@ -145,11 +148,13 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
               "ddfa_act_image_bytes", "ddfa_ggnn_workspace_bytes", "ddfa_embed_concat_bwd_workspace_bytes", "ddfa_readout_bwd_workspace_bytes",
               "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
               "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes",
-              "ddfa_stmt_metric_workspace_bytes", "ddfa_gru_tc_wide_gemm_workspace_bytes", "ddfa_gru_tc_wide_wgrad_slices"}
+              "ddfa_stmt_metric_workspace_bytes", "ddfa_gru_tc_wide_gemm_workspace_bytes", "ddfa_gru_tc_wide_wgrad_slices",
+              "ddfa_curve_workspace_bytes"}
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
 STMT_STATE_WORDS = 16         # DDFA_STMT_STATE_WORDS: fp64 words of the statement metric state
 STMT_MODE_VULN_ONLY, STMT_MODE_FULL = 0, 1    # DDFA_STMT_MODE_*: modes of ddfa_stmt_metric
 STMT_SCORE_ABS, STMT_SCORE_X_TIMES = 0, 1     # DDFA_STMT_SCORE_*: rules of ddfa_stmt_input_grad_score
+CURVE_INFO_WORDS = 8          # DDFA_CURVE_INFO_WORDS: int64 words of the curve info (lengths, class counts, error counts)
 PREDICT_MAX_K = 32            # DDFA_PREDICT_MAX_K: the most statements ddfa_predict_store ranks per function
 P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank the guarded peer-memory exchange needs
 GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate

@@ -94,6 +94,94 @@ def statement_metrics_from_state(state, prefix: str = "val_", node_style: bool =
     return out
 
 
+# the int64 words of the curve info (include/ddfa_b200.h, DDFA_CURVE_INFO_WORDS)
+C_DISTINCT, C_PR_POINTS, C_POSITIVES, C_NEGATIVES, C_NAN, C_BAD_LABELS, C_ONE_CLASS = range(7)
+
+
+def _bin_thresholds(binned_thresholds, device) -> torch.Tensor:
+    """The fp32 device thresholds of the binned curve.  An integer k gives BinnedPrecisionRecallCurve's default as recalled for
+    torchmetrics < 0.10 (torchmetrics is not a dependency, so this is not checked against it): ``torch.linspace(0, 1.0, k)``,
+    built in fp32 on the host and moved to the device.  Otherwise the given thresholds, compared with the probabilities as given."""
+    if isinstance(binned_thresholds, numbers.Integral) and not isinstance(binned_thresholds, bool):
+        if int(binned_thresholds) < 1:
+            raise ValueError(f"binned_thresholds must be >= 1, got {binned_thresholds!r}")
+        host = torch.linspace(0, 1.0, int(binned_thresholds), dtype=torch.float32)
+        return host.pin_memory().to(device, non_blocking=True)
+    t = torch.as_tensor(binned_thresholds)
+    if t.dim() != 1 or t.numel() == 0 or not t.dtype.is_floating_point:
+        raise ValueError(f"binned_thresholds: an int or a non-empty 1-D float sequence, got {binned_thresholds!r}")
+    return t.to(device=device, dtype=torch.float32).contiguous()
+
+
+def binary_curves(probs: torch.Tensor, labels: torch.Tensor, binned_thresholds=100) -> dict:
+    """The threshold curves of fp32 CUDA probabilities and 0 / 1 labels, computed on the device (``ddfa_curve_sort`` /
+    ``ddfa_curve_metrics``) with torchmetrics < 0.10's rules, as ``BaseModule.test_epoch_end`` (base_module.py:348-383) runs them:
+
+    - ``pr_curve``: ``(precision, recall, thresholds)`` of ``PrecisionRecallCurve``.  Cut at the first threshold that reaches
+      full recall, thresholds ascending, precision 1 / recall 0 appended (one point more than thresholds).  sklearn's
+      ``precision_recall_curve`` does not cut, so it returns more points.
+    - ``roc_curve``: ``(fpr, tpr, thresholds)`` of ``ROC``: a leading (0, 0) point at ``thresholds[1] + 1``, thresholds descending.
+    - ``pr_curve_binned``: ``(precision, recall, thresholds)`` of ``BinnedPrecisionRecallCurve(1, thresholds=binned_thresholds)``:
+      ``(TP + 1e-6) / (TP + FP + 1e-6)`` and ``TP / (TP + FN + 1e-6)`` at ``p >= t``, then 1 / 0 appended.
+    - ``AUROC`` (trapezoids over the ROC curve) and ``AveragePrecision`` (``-Σ (r[k+1] - r[k]) · p[k]`` over the PR curve):
+      Python floats, fp64 sums in a fixed order, bit-reproducible.
+
+    Precision, recall, fpr and tpr are fp64 device tensors from the exact int64 counts; thresholds are the stored fp32 values bit
+    for bit (a zero shows as +0.0: the reference ties -0.0 with +0.0).  One synchronisation.  For several ranks, ``all_gather``
+    each rank's ``FusedEvaluator.predictions()`` and call this on the concatenation.  Raises ``DdfaError`` for tensors off the GPU
+    and ``ValueError`` for no samples, NaN probabilities, labels other than 0 / 1, or a single class."""
+    for name, t in (("probs", probs), ("labels", labels)):
+        if not torch.is_tensor(t) or t.device.type != "cuda":
+            raise _lib.DdfaError(f"binary_curves: {name} must be a CUDA tensor (there is no CPU path), got "
+                                 f"{t.device if torch.is_tensor(t) else type(t).__name__}")
+        if t.dtype != torch.float32 or t.dim() != 1:
+            raise ValueError(f"binary_curves: {name} must be a 1-D float32 tensor, got {t.dtype} of shape {tuple(t.shape)}")
+    if labels.device != probs.device or labels.numel() != probs.numel():
+        raise ValueError(f"binary_curves: probs ({probs.numel()} on {probs.device}) and labels ({labels.numel()} on "
+                         f"{labels.device}) differ")
+    n = probs.numel()
+    if n == 0:
+        raise ValueError("binary_curves: no samples")
+    dev = probs.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        p, y = probs.contiguous(), labels.contiguous()
+        bins = _bin_thresholds(binned_thresholds, dev)
+        nb = bins.numel()
+        ws = torch.empty(L.call("ddfa_curve_workspace_bytes", n), dtype=torch.uint8, device=dev)
+        thr = torch.empty(n, dtype=torch.float32, device=dev)
+        tps = torch.empty(n, dtype=torch.int64, device=dev)
+        fps = torch.empty(n, dtype=torch.int64, device=dev)
+        f64 = lambda k: torch.empty(k, dtype=torch.float64, device=dev)   # noqa: E731
+        pr_p, pr_r, pr_t = f64(n + 1), f64(n + 1), torch.empty(n, dtype=torch.float32, device=dev)
+        fpr, tpr, roc_t = f64(n + 1), f64(n + 1), torch.empty(n + 1, dtype=torch.float32, device=dev)
+        bin_p, bin_r = f64(nb + 1), f64(nb + 1)
+        words = f64(2 + _lib.CURVE_INFO_WORDS)        # [AUROC, AP] then the info words: one copy to the host
+        summary, info = words[:2], words[2:].view(torch.int64)
+        st = E._stream_ptr()
+        E._call("ddfa_curve_sort", p.data_ptr(), y.data_ptr(), n, thr.data_ptr(), tps.data_ptr(), fps.data_ptr(), info.data_ptr(),
+                ws.data_ptr(), ws.numel(), st)
+        E._call("ddfa_curve_metrics", thr.data_ptr(), tps.data_ptr(), fps.data_ptr(), n, bins.data_ptr(), nb, pr_p.data_ptr(),
+                pr_r.data_ptr(), pr_t.data_ptr(), fpr.data_ptr(), tpr.data_ptr(), roc_t.data_ptr(), bin_p.data_ptr(),
+                bin_r.data_ptr(), summary.data_ptr(), info.data_ptr(), ws.data_ptr(), ws.numel(), st)
+        host = words.cpu()
+    auroc, ap = host[:2].tolist()
+    w = host[2:].view(torch.int64).tolist()
+    if w[C_NAN]:
+        raise ValueError(f"binary_curves: {w[C_NAN]} of {n} probabilities are NaN")
+    if w[C_BAD_LABELS]:
+        raise ValueError(f"binary_curves: {w[C_BAD_LABELS]} of {n} labels are neither 0 nor 1")
+    if w[C_ONE_CLASS]:
+        raise ValueError(f"binary_curves: only one class present ({w[C_POSITIVES]} positives, {w[C_NEGATIVES]} negatives): the "
+                         "ROC curve and AUROC are undefined")
+    m, k = w[C_DISTINCT], w[C_PR_POINTS]
+    return {"pr_curve": (pr_p[:k + 1], pr_r[:k + 1], pr_t[:k]),
+            "roc_curve": (fpr[:m + 1], tpr[:m + 1], roc_t[:m + 1]),
+            "pr_curve_binned": (bin_p, bin_r, bins),
+            "AUROC": auroc,
+            "AveragePrecision": ap}
+
+
 class InferencePass(CapturedBatches):
     """The inference forward and the per-statement scores of one batch over the module's current parameters, on the batch paths
     of :class:`~deepdfa_b200.capture.CapturedBatches`: what :class:`FusedEvaluator` and
@@ -434,6 +522,28 @@ class FusedEvaluator(InferencePass):
             raise ValueError("FusedEvaluator.predictions: built with max_predictions=0 (no prediction store)")
         k = int(self._state[STORED].item())
         return self._probs[:k], self._labels[:k]
+
+    def curves(self, prefix: str = "test_", binned_thresholds=100) -> dict:
+        """:func:`binary_curves` of :meth:`predictions`, with ``{prefix}`` keys: ``{prefix}pr_curve``, ``{prefix}roc_curve``,
+        ``{prefix}pr_curve_binned``, ``{prefix}AUROC`` and ``{prefix}AveragePrecision`` — what ``test_epoch_end`` writes to
+        ``pr.csv`` / ``pr_binned.csv``, and the two threshold-free scores.  Raises as :meth:`compute` does (no prediction store,
+        nothing evaluated, overflow, node feature indices outside the tables) and as :func:`binary_curves` does.  The metric
+        state is only read."""
+        if self._probs is None:
+            raise ValueError("FusedEvaluator.curves: built with max_predictions=0 (no prediction store)")
+        s = self._state.cpu()
+        bad = int(self._oob.item())
+        if bad:
+            raise IndexError(f"{bad} node feature indices outside [0, {self.module.input_dim}) in an evaluated batch")
+        n = int(s[TP] + s[FP] + s[TN] + s[FN])
+        if n == 0:
+            raise ValueError("FusedEvaluator.curves: no sample was evaluated since the last reset()")
+        if s[OVERFLOW] > 0:
+            raise ValueError(f"FusedEvaluator.curves: {n} predictions, max_predictions={self.max_predictions}: build the "
+                             f"evaluator with max_predictions >= {n}")
+        k = int(s[STORED])
+        out = binary_curves(self._probs[:k], self._labels[:k], binned_thresholds)
+        return {f"{prefix}{key}": v for key, v in out.items()}
 
     # ---- per batch -------------------------------------------------------------------------------------------------------
     def _enqueue(self, params, prepared, vuln, num_valid: Optional[int], valid_nodes: Optional[torch.Tensor]):

@@ -638,6 +638,49 @@ int ddfa_predict_store(const float *logits, const float *node_probs, const float
                        void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K9'''  threshold curves of a test pass (csrc/curves.cu): what BaseModule.test_epoch_end (base_module.py:348-383) computes from
+ * test_preds / test_labels with torchmetrics < 0.10 — the exact precision-recall curve, the binned one — plus the ROC curve,
+ * AUROC and average precision, over n fp32 probabilities and n fp32 labels (the layout of the K9 prediction store).  Nothing
+ * syncs with the host: the curve lengths go to device words.
+ *
+ * ddfa_curve_sort: torchmetrics' _binary_clf_curve.  The probabilities sorted in descending order (an LSD radix sort of 8-bit
+ *   digits over the 32-bit order-preserving key of p; -0.0 is keyed as +0.0, as the reference ties them); at the last sample of
+ *   every run of equal values, in descending order j = 0 .. m-1: thresholds[j] = the value (the stored fp32 bits; +0.0 for a
+ *   zero), tps[j] / fps[j] = the samples with p >= thresholds[j] whose label is 1 / is not.  thresholds fp32 [n], tps / fps
+ *   int64 [n]; entries j >= m are not written.
+ * info: DDFA_CURVE_INFO_WORDS int64 words, 8-byte aligned, zeroed and filled by ddfa_curve_sort, read (and [1] written) by
+ *   ddfa_curve_metrics:
+ *   [0] m, distinct thresholds  [1] PR curve points before the appended (1, 0)  [2] positives (label == 1)  [3] negatives
+ *   [4] NaN probabilities  [5] labels other than 0 / 1 (NaN included; they count as negatives)  [6] 1 when only one class is
+ *   present (no positive or no negative: the ROC curve and AUROC are undefined)  [7] reserved
+ *   The outputs are computed whatever the error words say (never a fault); with [4] > 0 they follow the key order of NaN and are
+ *   meaningless.
+ * ddfa_curve_metrics (over ddfa_curve_sort's outputs; P = info[2], N = info[3], L = info[1]):
+ *   PR curve, torchmetrics < 0.10's _precision_recall_curve_compute_single_class: truncated at the first j where tps[j] == P
+ *     (L = j + 1 points), reversed, then precision 1 / recall 0 appended: pr_precision / pr_recall fp64 [n + 1] (L + 1 written),
+ *     pr_thresholds fp32 [n] (L written): for k < L, q = L - 1 - k: tps[q] / (tps[q] + fps[q]), tps[q] / P, thresholds[q].
+ *   ROC curve, _roc_compute_single_class: a leading (0, 0) point at thresholds[0] + 1.f, then fpr = fps / N, tpr = tps / P (0
+ *     where N or P is 0): roc_fpr / roc_tpr fp64 [n + 1], roc_thresholds fp32 [n + 1] (m + 1 written).
+ *   summary fp64 [2]: [0] AUROC = sum over the ROC points of (fpr[j+1] - fpr[j]) * (tpr[j] + tpr[j+1]) / 2 (NaN with one class),
+ *     [1] average precision = -sum over the PR points of (recall[k+1] - recall[k]) * precision[k] (NaN without positives).  fp64
+ *     terms, per-CTA partials over a grid that depends on n only, added in CTA order: bit-reproducible in both
+ *     DDFA_TUNE_DETERMINISTIC modes.
+ *   Binned curve, BinnedPrecisionRecallCurve: for the fp32 thresholds bin_thresholds[0 .. num_bins), TP / FP = the samples with
+ *     p >= t_i by label (binary search over thresholds), FN = P - TP; bin_precision[i] = (TP + 1e-6) / (TP + FP + 1e-6),
+ *     bin_recall[i] = TP / (TP + FN + 1e-6) in fp64, then 1 / 0 at [num_bins]: fp64 [num_bins + 1] each.
+ * workspace: ddfa_curve_workspace_bytes(n) bytes, 16-byte aligned, scratch; one buffer serves both calls.  Every entry runs on
+ *   `stream` and can be captured.  ddfa_curve_sort: 1 memset + 16 launches; ddfa_curve_metrics: 3 launches.  1 <= n.
+ * ------------------------------------------------------------------------------------- */
+#define DDFA_CURVE_INFO_WORDS 8
+size_t ddfa_curve_workspace_bytes(int64_t n);
+int ddfa_curve_sort(const float *probs, const float *labels, int64_t n, float *thresholds, int64_t *tps, int64_t *fps,
+                    int64_t *info, void *workspace, size_t workspace_bytes, void *stream);
+int ddfa_curve_metrics(const float *thresholds, const int64_t *tps, const int64_t *fps, int64_t n, const float *bin_thresholds,
+                       int32_t num_bins, double *pr_precision, double *pr_recall, float *pr_thresholds, double *roc_fpr,
+                       double *roc_tpr, float *roc_thresholds, double *bin_precision, double *bin_recall, double *summary,
+                       int64_t *info, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * K10  torch.optim.Adam(lr, betas, eps, weight_decay) with coupled L2 (DDFA/configs/
  * config_default.yaml:43-47) over one flat parameter buffer.  step_count: int32[1] device
  * counter, incremented by the kernel (graph-capture safe).
