@@ -137,6 +137,17 @@ _SIGNATURES = {
     "ddfa_curve_metrics": (_int, [_vp, _vp, _vp, _i64, _vp, _i32] + [_vp] * 10 + [_vp, _sz, _vp]),
     "ddfa_mlp_dgrad_rescale": (_int, [_vp] * 7 + [_i32, _i32, _i32, _vp, _vp, _vp]),
     "ddfa_grad_accumulate": (_int, [_vp, _vp, _i64, _i64, _i32, _vp]),
+    "ddfa_csv_index_workspace_bytes": (_sz, [_i64]),
+    "ddfa_csv_index_count": (_int, [_vp, _i64, _vp, _vp, _sz, _vp]),
+    "ddfa_csv_index_rows": (_int, [_vp, _i64, _vp, _vp, _sz, _vp]),
+    "ddfa_csv_fields": (_int, [_vp, _vp, _i64, _vp, _i32, _vp, _vp, _vp]),
+    "ddfa_row_sort_workspace_bytes": (_sz, [_i32]),
+    "ddfa_row_sort": (_int, [_vp, _i64, _i32, _vp, _i64, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "ddfa_csv_graphs_workspace_bytes": (_sz, [_i32]),
+    "ddfa_csv_graphs": (_int, [_vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ddfa_csv_union": (_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _sz] + [_vp] * 6 + [_vp]),
+    "ddfa_csv_join_workspace_bytes": (_sz, [_i32]),
+    "ddfa_csv_join": (_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _sz, _vp]),
     "ddfa_sgemm": (_int, [_int, _int, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _i32, _f32, _vp, _i32, _i32, _vp]),
 }
 
@@ -149,7 +160,8 @@ _NO_STATUS = {"ddfa_gru_gates_packed_bytes", "ddfa_tuning_get", "ddfa_abi_versio
               "ddfa_grad_norm_workspace_bytes", "ddfa_p2p_guard_state_bytes", "ddfa_node_sample_workspace_bytes",
               "ddfa_node_dp_exchange_words", "ddfa_node_head_bwd_workspace_bytes", "ddfa_eval_metrics_workspace_bytes",
               "ddfa_stmt_metric_workspace_bytes", "ddfa_gru_tc_wide_gemm_workspace_bytes", "ddfa_gru_tc_wide_wgrad_slices",
-              "ddfa_curve_workspace_bytes"}
+              "ddfa_curve_workspace_bytes", "ddfa_csv_index_workspace_bytes", "ddfa_row_sort_workspace_bytes",
+              "ddfa_csv_graphs_workspace_bytes", "ddfa_csv_join_workspace_bytes"}
 EVAL_STATE_WORDS = 16         # DDFA_EVAL_STATE_WORDS: fp64 words of the evaluation metric state
 STMT_STATE_WORDS = 16         # DDFA_STMT_STATE_WORDS: fp64 words of the statement metric state
 STMT_MODE_VULN_ONLY, STMT_MODE_FULL = 0, 1    # DDFA_STMT_MODE_*: modes of ddfa_stmt_metric
@@ -160,6 +172,10 @@ P2P_GUARD_FLAG_WORDS = 96     # DDFA_P2P_GUARD_FLAG_WORDS: flag words per rank t
 GRAD_ACC_SET, GRAD_ACC_ADD, GRAD_ACC_APPLY = 0, 1, 2     # DDFA_GRAD_ACC_*: modes of ddfa_grad_accumulate
 ADAM_GROUP_WORDS = 8          # DDFA_ADAM_GROUP_WORDS: fp32 words per row of the parameter-group table
 ADAM_MAX_GROUPS = 64          # DDFA_ADAM_MAX_GROUPS: rows the grouped Adam entry points accept
+CSV_MAX_COLS = 8              # DDFA_CSV_MAX_COLS: columns one ddfa_csv_fields / ddfa_csv_join call reads or writes
+CSV_GRAPH_INFO_WORDS = 8      # DDFA_CSV_GRAPH_INFO_WORDS: int64 words of ddfa_csv_graphs' info
+(CSV_ERR_NOT_INT, CSV_ERR_NO_FIELD, CSV_ERR_NO_EDGES, CSV_ERR_NEGATIVE, CSV_ERR_NODE_COUNT, CSV_ERR_NO_FEATURE,
+ CSV_ERR_DUPLICATE) = range(1, 8)     # DDFA_CSV_ERR_*: reasons in the error words of the F2 loader
 
 
 class _Lib:

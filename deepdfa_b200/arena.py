@@ -100,7 +100,14 @@ class GraphArena:
             singles.extend(BG.unbatch(g) if g.batch_size != 1 else [g])
         if not singles:
             raise ValueError("GraphArena.from_graphs: no graphs")
-        big = BG.batch(singles)
+        return cls.from_union(BG.batch(singles), device)
+
+    @classmethod
+    def from_union(cls, big: BatchedCFG, device="cuda") -> "GraphArena":
+        """The arena of ``big``, the disjoint union of its graphs as ``dgl.batch`` lays it out (COO with node ids offset per
+        graph, ``batch_num_nodes`` / ``batch_num_edges``, ndata), on the host or already on ``device``.  Shared by
+        :meth:`from_graphs` and :func:`deepdfa_b200.bigvul_io.load_arena`."""
+        device = torch.device(device)
         if big.num_nodes() >= 2 ** 31 or big.num_edges() >= 2 ** 31:
             raise ValueError("GraphArena: more than 2^31 nodes or edges")
         if len([k for k in big.ndata if k != "_VULN"]) > 8:

@@ -137,3 +137,51 @@ def make_edge_cases(input_dim: int = 1002, seed: int = 7) -> BatchedCFG:
     src, dst = src[keep], dst[keep]
     del rng
     return BatchedCFG(torch.from_numpy(src), torch.from_numpy(dst), g.batch_num_nodes(), g.ndata)
+
+
+BIGVUL_TAIL = "_all_limitall_1000_limitsubkeys_1000"
+_CODE = np.array(["x = 1;", "f(a, b);", 'puts("hi, \\"there\\"");', "if (a)\n{", "return;", "", "nan", "p->q = r[\"k\"];",
+                  "/* é ü */", "a\r\nb"])
+
+
+def write_bigvul_files(root, num_graphs: int, seed: int = 0, mu: float = 3.7, sigma: float = 0.8, big_graph: int = 3000) -> dict:
+    """Processed Big-Vul files in the reference's schema under ``root/bigvul`` (dbize.py:104-105: ``nodes.csv`` with an
+    unnamed index, ``dgl_id``, ``code``, ``vuln``, ``graph_id``, ``node_id``, ``_label`` and ``edges.csv``; dbize_absdf.py: one shuffled
+    ``nodes_feat__ABS_DATAFLOW_<sub>_all_..._fixed.csv`` per subkey): lognormal graph sizes (``mu`` / ``sigma`` of the log, at
+    least 2 nodes, graph 0 has ``big_graph`` nodes), about two edge rows per node, unsorted non-contiguous graph ids.  Returns
+    the columns as written: {"nodes": {...}, "edges": {...}, "features": {sub: {graph_id, node_id, value}}}."""
+    import pandas as pd
+    from pathlib import Path
+    rng = np.random.default_rng(seed)
+    folder = Path(root) / "bigvul"
+    folder.mkdir(parents=True, exist_ok=True)
+    sizes = np.clip(np.rint(rng.lognormal(mu, sigma, num_graphs)), 2, None).astype(np.int64)
+    sizes[0] = big_graph
+    gid_of = rng.permutation(np.arange(num_graphs, dtype=np.int64) * 3 + 100)
+    N = int(sizes.sum())
+    first = np.repeat(np.cumsum(sizes) - sizes, sizes)
+    local = np.arange(N) - first
+    g_node = np.repeat(gid_of, sizes)
+    node_id = 1000 + 4 * local + np.repeat(rng.integers(0, 50, num_graphs), sizes)
+    vuln = (rng.random(N) < 0.05).astype(np.int64)
+    ecount = 2 * sizes
+    Ne = int(ecount.sum())
+    eg = np.repeat(np.arange(num_graphs), ecount)
+    n_e = sizes[eg]
+    src = (rng.random(Ne) * n_e).astype(np.int64)
+    dst = (rng.random(Ne) * n_e).astype(np.int64)
+    head = np.cumsum(ecount) - ecount
+    src[head], dst[head] = sizes - 1, 0                 # every graph names its highest dgl id
+    nodes = {"graph_id": g_node, "node_id": node_id, "vuln": vuln}
+    edges = {"graph_id": gid_of[eg], "innode": src, "outnode": dst}
+    pd.DataFrame({"dgl_id": local, "code": _CODE[rng.integers(0, len(_CODE), N)], "vuln": vuln, "graph_id": g_node,
+                  "node_id": node_id, "_label": "CALL"}).to_csv(folder / "nodes.csv")
+    pd.DataFrame(edges).to_csv(folder / "edges.csv")
+    features = {}
+    for sub in ABS_DATAFLOW_SUBKEYS:
+        stem = f"_ABS_DATAFLOW_{sub}{BIGVUL_TAIL}"
+        order = rng.permutation(N)
+        f = {"graph_id": g_node[order], "node_id": node_id[order], "value": rng.integers(0, 1002, N)}
+        pd.DataFrame({"graph_id": f["graph_id"], "node_id": f["node_id"], stem: f["value"]}).to_csv(folder / f"nodes_feat_{stem}_fixed.csv")
+        features[sub] = f
+    return {"nodes": nodes, "edges": edges, "features": features}

@@ -818,6 +818,76 @@ int ddfa_allreduce_adam_p2p_groups_guarded(void *const *peer_params, const void 
 int ddfa_grad_accumulate(float *acc, float *grads, int64_t begin, int64_t end, int32_t mode, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * F2  processed Big-Vul files -> arena, on the device (csrc/csv_load.cu; SURVEY.md §8 row f2).  Replaces the host loaders
+ * deepdfa_b200/bigvul_io.py restates: pd.read_csv of nodes.csv / edges.csv / nodes_feat_*.csv (written by DataFrame.to_csv,
+ * DDFA/sastvd/scripts/dbize.py:104-105, dbize_absdf.py:44), the per-graph dgl.graph + add_self_loop of dbize_graphs.py:17-27,
+ * the left merge of graphmogrifier.py:20-40 and the per-graph ndata of graphmogrifier.py:59-95.  Nothing here allocates:
+ * every scratch buffer is a caller workspace sized by the matching *_workspace_bytes query.
+ *
+ * CSV dialect (pandas to_csv): ',' separates fields, '"' quotes them and "" escapes a quote inside; a row ends at a '\n' outside
+ * quotes (an optional '\r' before it is dropped); blank lines are skipped.  Quote state is the parity of the quotes before a byte.
+ *
+ * ddfa_csv_index_count / ddfa_csv_index_rows: the row index of text[0, nbytes) (16-byte aligned; the caller appends a final
+ *   '\n' when the file lacks one).  count writes info int64[2] = {rows, quote parity at the end (1: unterminated quote)};
+ *   rows then sizes row_end int64[rows], which rows fills with the offset of each row's terminating '\n' (row 0: the header).
+ *   Row r > 0 spans (row_end[r - 1], row_end[r]), blank lines before it skipped.  count: 2 launches, rows: 1.
+ * ddfa_csv_fields: the data rows 1 .. rows-1 (output index r - 1), the columns at positions columns[0 .. num_columns)
+ *   (ascending, at most DDFA_CSV_MAX_COLS) parsed to out[s] int64[rows - 1]: a signed decimal integer, optionally quoted,
+ *   optionally followed by '.' and zeros.  Each row is read only up to its last requested column.  info int64[1 + 2 * num_columns]:
+ *   [0] the first bad row, as the unsigned word (r - 1) << 8 | reason << 4 | slot (all ones: none; reason DDFA_CSV_ERR_NOT_INT
+ *   or DDFA_CSV_ERR_NO_FIELD), then {min, max} of each column over the rows.  2 launches.
+ * ddfa_row_sort: perm int32[n] = the row ids 0 .. n-1 stably sorted by (major[row], minor[row]) (minor NULL: by major alone),
+ *   an LSD radix sort of 8-bit digits of key - key_min over key_bits bits (the host knows the range from ddfa_csv_fields).
+ *   1 + 3 * (ceil(minor_bits / 8) + ceil(major_bits / 8)) launches.
+ * ddfa_csv_graphs: the node rows sorted by graph_id (node_perm) form the graphs, in ascending graph_id; each graph's edges
+ *   are the edge rows (sorted by graph_id: edge_perm) of its graph_id, in file row order.  Edge rows of other graph ids are not
+ *   read.  info int64[DDFA_CSV_GRAPH_INFO_WORDS]: [0] G, [1] union edges (edge rows of the graphs + one self-loop per node),
+ *   [2] the first bad graph as j << 8 | reason << 4 (all ones: none; DDFA_CSV_ERR_NO_EDGES, DDFA_CSV_ERR_NEGATIVE endpoint,
+ *   DDFA_CSV_ERR_NODE_COUNT: max endpoint + 1 != node rows), for it [3] max endpoint + 1, [4] node rows, [5] graph_id.
+ *   The workspace (ddfa_csv_graphs_workspace_bytes(node_rows)) carries the graph segments to ddfa_csv_union.  6-10 launches.
+ * ddfa_csv_union (after ddfa_csv_graphs, with its workspace, num_graphs = info[0], when info[2] shows no error and
+ *   info[1] < 2^31): the union COO src / dst int32[info[1]] = each graph's edge rows (src = innode, dst = outnode) offset by
+ *   its first node, then its self-loops v -> v, graph after graph — what BG.batch of the add_self_loop'd graphs holds; arena
+ *   node i = node row node_perm[i]; vuln int32[node_rows] = int32(float(vuln_col)) (attach_node_data's torch.Tensor(...).int());
+ *   nodes_per_graph / edges_per_graph / graph_ids int64[G].  2 launches.
+ * ddfa_csv_join: the left merge of one feature file on (graph_id, node_id): feat_perm sorts its rows by that pair
+ *   (ddfa_row_sort); out[s][i] = values[s][the feature row of arena node i].  info int64[1]: the first arena node without a
+ *   feature row (DDFA_CSV_ERR_NO_FEATURE) or with two (DDFA_CSV_ERR_DUPLICATE) as i << 8 | reason << 4; all ones: none.
+ *   Workspace: the sorted keys, ddfa_csv_join_workspace_bytes(feature_rows).  1 memset + 2 launches.
+ * Every entry runs on `stream` and reads no device word on the host.
+ * ------------------------------------------------------------------------------------- */
+#define DDFA_CSV_MAX_COLS 8
+#define DDFA_CSV_GRAPH_INFO_WORDS 8
+#define DDFA_CSV_ERR_NOT_INT 1
+#define DDFA_CSV_ERR_NO_FIELD 2
+#define DDFA_CSV_ERR_NO_EDGES 3
+#define DDFA_CSV_ERR_NEGATIVE 4
+#define DDFA_CSV_ERR_NODE_COUNT 5
+#define DDFA_CSV_ERR_NO_FEATURE 6
+#define DDFA_CSV_ERR_DUPLICATE 7
+size_t ddfa_csv_index_workspace_bytes(int64_t nbytes);
+int ddfa_csv_index_count(const uint8_t *text, int64_t nbytes, int64_t *info, void *workspace, size_t workspace_bytes, void *stream);
+int ddfa_csv_index_rows(const uint8_t *text, int64_t nbytes, int64_t *row_end, void *workspace, size_t workspace_bytes, void *stream);
+int ddfa_csv_fields(const uint8_t *text, const int64_t *row_end, int64_t rows, const int32_t *columns, int32_t num_columns,
+                    int64_t *const *out, int64_t *info, void *stream);
+size_t ddfa_row_sort_workspace_bytes(int32_t n);
+int ddfa_row_sort(const int64_t *major, int64_t major_min, int32_t major_bits, const int64_t *minor, int64_t minor_min,
+                  int32_t minor_bits, int32_t n, int32_t *perm, void *workspace, size_t workspace_bytes, void *stream);
+size_t ddfa_csv_graphs_workspace_bytes(int32_t node_rows);
+int ddfa_csv_graphs(const int64_t *node_gid, const int32_t *node_perm, int32_t node_rows, const int64_t *edge_gid,
+                    const int32_t *edge_perm, int32_t edge_rows, const int64_t *innode, const int64_t *outnode, int64_t *info,
+                    void *workspace, size_t workspace_bytes, void *stream);
+int ddfa_csv_union(const int64_t *node_gid, const int32_t *node_perm, int32_t node_rows, const int64_t *vuln_col,
+                   const int32_t *edge_perm, const int64_t *innode, const int64_t *outnode, int32_t num_graphs,
+                   const void *workspace, size_t workspace_bytes, int32_t *src, int32_t *dst, int32_t *vuln,
+                   int64_t *nodes_per_graph, int64_t *edges_per_graph, int64_t *graph_ids, void *stream);
+size_t ddfa_csv_join_workspace_bytes(int32_t feature_rows);
+int ddfa_csv_join(const int64_t *node_gid, const int64_t *node_nid, const int32_t *node_perm, int32_t node_rows,
+                  const int64_t *feat_gid, const int64_t *feat_nid, const int32_t *feat_perm, int32_t feature_rows,
+                  const int64_t *const *values, int32_t num_values, int64_t *const *out, int64_t *info, void *workspace,
+                  size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Generic row-major fp32 GEMM on the SIMT engine (building block, exported for tests):
  *   C[M,N] = alpha * op(A) op(B) + beta * C,  op(X) = X or X^T per trans flag.
  * split_k > 1 accumulates partial products with atomics (requires beta == 1, C pre-initialised; rejected in deterministic mode).
